@@ -1,14 +1,14 @@
 #!/usr/bin/env python
 """bench.py — decode tok/s of the quantized-MoE hot path at DeepSeek-V3 shapes.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (config.workload): DeepSeek-V3 671B Q4_K_M single-stream decode, the MoE-block hot path of every
 token: 58 MoE layers x [router (fp32 GEMV + grouped top-8) -> 8 routed experts (gate/up Q4_K, down Q6_K,
-H=7168, I=2048, 256 experts resident per layer) -> 1 shared expert].  671B does not fit one B200, so a step
-walks 58 layers over `--resident-layers` distinct full-size weight sets (each 7.4 GB >> L2, revisit distance
->= 2 sets >> L2: every byte comes from HBM); attention / dense layers / lm_head are NOT in the step and the
+H=7168, I=2048, 256 experts resident per layer) -> 1 shared expert].  671B does not fit one 80 GB H100, so a step
+walks 58 layers over `--resident-layers` distinct full-size weight sets (each 7.4 GB >> the 50 MB L2, revisit distance
+>= 3 sets: every byte comes from HBM); attention / dense layers / lm_head are NOT in the step and the
 metric says so.  Weights are synthetic well-formed GGUF blocks, activations random (data: synthetic).
 
 One step = one token per GPU through the 58 layers.  N > 1: experts are sharded E/N per GPU
@@ -60,7 +60,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth)"
 
 
 class ClockSampler:
@@ -202,13 +202,13 @@ class RefCpuMoe:
 
 def amx_baseline(seconds=6.0):
     """The reference's AMX INT4 MoE (kt_kernel_ext.moe.AMXInt4_MOE, the "CPU-AMX" path of north_star) through the shimmed
-    build oracle/_ref/libktamx.so — only on hosts with AMX; otherwise says why not.  Build-host numbers: profiles/."""
+    build oracle/_ref/libktamx.so — only on hosts with AMX; otherwise says why not."""
     try:
         import numpy as np
 
         from oracle.bindings import AmxRef, f32_to_bf16_bits
         if not AmxRef.available():
-            return {"unavailable": AmxRef.why_unavailable(), "build_host_measurement": "profiles/r02_amx_baseline_buildhost.json"}
+            return {"unavailable": AmxRef.why_unavailable()}
         En = 16
         rng = np.random.default_rng(0)
         mk = lambda shape: f32_to_bf16_bits(rng.standard_normal(shape, dtype=np.float32))  # noqa: E731
@@ -241,7 +241,7 @@ def run_reference_arm(args, rank):
     if rank != 0:
         return
     world = max(1, args.gpus)
-    cpu = RefCpuMoe(tokens=world)            # same config as the B200 arm: `world` tokens per step
+    cpu = RefCpuMoe(tokens=world)            # same config as the GPU arm: `world` tokens per step
     for _ in range(args.warmup):
         cpu.token()
     t0 = time.perf_counter()
@@ -268,7 +268,7 @@ def workload_config(args, world):
             "parallelism": f"ep{world}" if world > 1 else "single",
             "block_launch": ("plain grid + programmatic dependent launch" if os.environ.get("KTB200_BLK_COOP", "1") == "0"
                              else "cooperative + programmatic dependent launch"),
-            "l2": "inputs larger than L2: each layer set is 7.4 GB and is revisited after >= 2 other sets",
+            "l2": f"inputs larger than L2: each layer set is 7.4 GB and is revisited after {args.resident_layers - 1} other sets",
             "next_layer_prefetch": os.environ.get("KTB200_BENCH_PREFETCH", "0") != "0" and world == 1,
             "note": "layer inputs are not chained (random-init weights overflow bf16 within a few layers); every layer routes and computes on the step's hidden state with its own router/expert weights"}
 
@@ -278,7 +278,7 @@ def workload_config(args, world):
 def full_decode_leg(args, lib, native, dev, local_rank, layers, L, moe_layer_call, world):
     """The WHOLE DeepSeek-V3 decode step (BASELINE config 2: "... decode bs=1 ... MLA path"), one CUDA graph:
     61 x [input RMSNorm -> q_a / kv_a (Q4_K, ktb200_linear) -> q_a norm -> q_b -> kv norm + RoPE + paged cache write
-    (ktb200_mla_prep) -> W_UK absorb (bmm) -> MLA paged decode over `ctx` cached tokens (ktb200_mla_decode, tcgen05) -> W_UV
+    (ktb200_mla_prep) -> W_UK absorb (bmm) -> MLA paged decode over `ctx` cached tokens (ktb200_mla_decode, wgmma) -> W_UV
     (bmm) -> o_proj -> residual + post RMSNorm -> dense MLP (3 layers) | MoE block (58 layers)] -> final norm -> lm_head.
     Weights synthetic at the real shapes and all resident and distinct except the MoE sets (the resident `layers`)."""
     import ctypes as C
@@ -394,7 +394,7 @@ def full_decode_leg(args, lib, native, dev, local_rank, layers, L, moe_layer_cal
         e1.record(); torch.cuda.synchronize()
         return e0.elapsed_time(e1) / steps, launches
 
-    steps = max(5, min(args.steps, 20))
+    steps = args.steps
     ms_full, launches = timed(lambda: step(True, True), steps)
     ms_noattn, _ = timed(lambda: step(True, False), steps)
     attn_bytes = NL * ((H * QL + H * (KVL + ROPE) + QL * NH * (NOPE + ROPE) + NH * VD * H) * 144 // 256 + 2 * NH * NOPE * KVL * 2 + (ctx + 1) * (KVL + ROPE) * 2)
@@ -414,20 +414,23 @@ def full_decode_leg(args, lib, native, dev, local_rank, layers, L, moe_layer_cal
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20, help="timed steps of every leg (decode, host-buffer, whole step, prefill, FP8)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--resident-layers", type=int, default=8)
+    # 4 sets of 7.4 GB: every layer's weights come from HBM, and the whole-step and FP8 legs still fit 80 GB beside them
+    ap.add_argument("--resident-layers", type=int, default=4)
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--ctx", type=int, default=4096, help="cached tokens per sequence in the whole-step leg")
     ap.add_argument("--no-full-step", action="store_true")
     ap.add_argument("--no-prefill", action="store_true", help="skip the 1024-token grouped-GEMM leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed step computed (every "
+                    "layer's output, routed expert ids and routing weights) as DIR/<name>.npy in float32 / float64")
     args = ap.parse_args()
     # This process owns the GPU and decodes on ONE stream: the persistent MoE-block kernel is launched as a plain grid
-    # with programmatic dependent launch (its 148 CTAs become co-resident as the previous layer's CTAs exit) instead of
+    # with programmatic dependent launch (its one CTA per SM becomes co-resident as the previous layer's CTAs exit) instead of
     # cooperatively — the cooperative attribute (library default: safe when several streams share the GPU) makes every
-    # launch wait for the previous grid to drain and costs ~4 % here.  Recorded in config["block_launch"].
+    # launch wait for the previous grid to drain.  Recorded in config["block_launch"].
     os.environ.setdefault("KTB200_BLK_COOP", "0")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -443,7 +446,7 @@ def main():
     from ktransformers_b200 import native
     from ktransformers_b200.util.synth import synth_blocks
 
-    assert torch.cuda.is_available(), "the B200 path has no CPU fallback"
+    assert torch.cuda.is_available(), "the CUDA path has no CPU fallback"
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -512,7 +515,7 @@ def main():
         Wr = torch.randn((E, H), device=dev, generator=g, dtype=torch.float32)
         # e_score_correction_bias: a trained model's bias keeps the experts balanced; a randn bias (std 1 against sigmoid
         # scores in 0.3..0.7) would send EVERY token to the same few experts — harmless at N = 1, a pathological 2x load
-        # imbalance for expert-parallel shards (measured: profiles/ep_trace_n8_r02.txt).  The reference's own MoE bench routes
+        # imbalance for expert-parallel shards.  The reference's own MoE bench routes
         # uniformly at random (kt-kernel/bench/bench_moe.py:235-239); a small bias keeps the routing token-dependent.
         br = 0.01 * torch.randn((E,), device=dev, generator=g, dtype=torch.float32)
         gcfg = native.GateConfig(E, H, K, N_GROUP, TOPK_GROUP, 0, 0, 1, ROUTED_SCALE, Wr.data_ptr(), br.data_ptr(), BF16)
@@ -531,11 +534,13 @@ def main():
     x_own = torch.zeros((1, H), dtype=torch.bfloat16, device=dev)          # this GPU's token
     x_all = torch.zeros((T, H), dtype=torch.bfloat16, device=dev)
     x_all_f32 = torch.zeros((T, H), dtype=torch.float32, device=dev)
-    ids = torch.zeros((T, K), dtype=torch.int64, device=dev)
-    wts = torch.zeros((T, K), dtype=torch.float32, device=dev)
+    # every layer of a step has its own output slots (layer l -> [l]), so that a step leaves all of its results behind
+    ids_out = torch.zeros((N_MOE_LAYERS, T, K), dtype=torch.int64, device=dev)
+    wts_out = torch.zeros((N_MOE_LAYERS, T, K), dtype=torch.float32, device=dev)
+    y_out = torch.zeros((N_MOE_LAYERS, 1, H), dtype=torch.bfloat16, device=dev)   # layer output for this GPU's token
+    ids, wts, y = ids_out[0], wts_out[0], y_out[0]
     part = torch.zeros((T, H), dtype=hid_torch, device=dev)                # NCCL route: fp32 partial sums
     own_f32 = torch.zeros((1, H), dtype=torch.float32, device=dev)
-    y = torch.zeros((1, H), dtype=torch.bfloat16, device=dev)              # layer output for this GPU's token
     x_host = torch.zeros((1, H), dtype=torch.bfloat16).pin_memory()
     y_host = torch.zeros((1, H), dtype=torch.bfloat16).pin_memory()
     out_host = torch.zeros((1, H), dtype=torch.bfloat16).pin_memory()
@@ -544,6 +549,7 @@ def main():
 
     def layer_device(l):
         Lr = layers[l % L]
+        y, ids, wts = y_out[l], ids_out[l], wts_out[l]
         if world == 1:
             # KDeepseekV3MoE.forward in one call: router + routed experts + shared expert (one persistent launch)
             native.check(lib.ktb200_moe_block_forward(C.byref(Lr["gcfg"]), Lr["moe"], Lr["mlp"], 1, x_own.data_ptr(), y.data_ptr(),
@@ -699,6 +705,12 @@ def main():
     barrier()
     ms = e0.elapsed_time(e1)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        # the arrays a caller of the timed step receives, as its last replay left them (all steps compute the same token)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "moe_block_out.npy"), y_out.float().cpu().numpy())        # [58][1][H]
+        np.save(os.path.join(args.dump_outputs, "routed_ids.npy"), ids_out.cpu().numpy().astype(np.float64))   # [58][T][8]
+        np.save(os.path.join(args.dump_outputs, "routed_weights.npy"), wts_out.cpu().numpy())           # [58][T][8]
     t_ms = torch.tensor([ms], device=dev)
     if world > 1:
         dist.all_reduce(t_ms, op=dist.ReduceOp.MAX)
@@ -812,11 +824,11 @@ def main():
                 prefill_layer(l)
             torch.cuda.synchronize()
             n0 = native.launch_count()
-            reps = 2 * L
+            reps = args.steps
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             for l in range(reps):
-                prefill_layer(l)        # L resident layer sets of 7.3 GB each: far larger than L2, every pass is cold
+                prefill_layer(l)        # cycles the L resident layer sets of 7.3 GB each: far larger than L2, every pass is cold
             e1.record(); torch.cuda.synchronize()
             ms_l = e0.elapsed_time(e1) / reps
             experts_hit = int(torch.unique(idp).numel())
@@ -826,7 +838,7 @@ def main():
                        "tok_s_moe_58_layers": Tp / (N_MOE_LAYERS * ms_l * 1e-3), "experts_hit": experts_hit,
                        "tflops_equiv": 2.0 * Tp * K * 3 * H * I / (ms_l * 1e-3) / 1e12,
                        "hbm": {"algorithmic_bytes": bytes_l, "achieved_GBps": bytes_l / (ms_l * 1e-3) / 1e9, "frac": bytes_l / (ms_l * 1e-3) / 1e9 / peak, "peak_source": how},
-                       "path": "MOE.forward on 1024 tokens, routing like kt-kernel/bench/bench_moe.py (uniform random): count/scan/scatter + Q8_K quantise + 3 grouped tcgen05 kind::i8 GEMMs + combine (csrc/grouped.cu); parity: tests/test_gpu_parity.py -k grouped"}
+                       "path": "MOE.forward on 1024 tokens, routing like kt-kernel/bench/bench_moe.py (uniform random): count/scan/scatter + Q8_K quantise + 3 grouped wgmma int8 GEMMs + combine (csrc/grouped.cu); parity: tests/test_gpu_parity.py -k grouped"}
         except Exception as e:  # pragma: no cover
             prefill = {"error": f"{type(e).__name__}: {e}"}
 
@@ -834,7 +846,7 @@ def main():
     fp8 = None
     if rank == 0 and world == 1 and not args.no_prefill:
         try:
-            fp8 = {"kernel": "fp8_linear_kernel (TMA -> tcgen05.mma.kind::f8f6f4 -> TMEM, csrc/fp8_linear.cu)", "bound": "hbm", "shapes": {}}
+            fp8 = {"kernel": "fp8_linear_kernel (TMA -> e4m3 widened to fp16 in registers -> fp16 wgmma, csrc/fp8_linear.cu)", "bound": "hbm", "shapes": {}}
             peak, how = measured_peak_gbs()
             for name, Kf, Nf, copies in (("lm_head 7168->129280", 7168, 129280, 2), ("o_proj 16384->7168", 16384, 7168, 4)):
                 hs, keep = [], []
@@ -848,7 +860,7 @@ def main():
                 for i in range(copies):
                     native.check(lib.ktb200_fp8_linear_forward(hs[i], 1, xf.data_ptr(), yf.data_ptr(), None, S()))
                 torch.cuda.synchronize()
-                n_it = 5 * copies
+                n_it = args.steps
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record()
                 for i in range(n_it):

@@ -1,4 +1,4 @@
-/* ktb200 — B200-native (sm_100a) drop-in for kt-kernel's quantized-MoE decode hot path.
+/* ktb200 — H100-native (sm_90a) drop-in for kt-kernel's quantized-MoE decode hot path.
  *
  * C-ABI boundary: plain pointers and sizes only, no torch / pybind types.  Every entry point
  * names the reference interface it replaces.  All `*_dev` pointers are CUDA device pointers on the
@@ -80,7 +80,7 @@ void ktb200_moe_destroy(ktb200_moe* moe);
 
 /* Replaces MOE::load_weights / load_weights_task (kt-kernel/ext_bindings.cpp:447-471).
  * Q6_K tensors are permuted IN PLACE, once, into the 16-byte-aligned "8-row SoA" layout that the
- * sm_100a kernels stream (DESIGN.md §3); other types are consumed as raw ggml blocks.
+ * sm_90a kernels stream (DESIGN.md §3); other types are consumed as raw ggml blocks.
  * Byte count is unchanged.  Idempotent per handle. */
 int ktb200_moe_load_weights(ktb200_moe* moe, void* stream);
 
@@ -125,7 +125,7 @@ float* ktb200_moe_intermediate(ktb200_moe* moe);
  * weight: DEVICE ptr, e4m3 bytes [out][in] (16-byte aligned, in % 128 == 0); weight_scale_inv: DEVICE fp32 [ceil(out/128)][in/128].
  * forward: x [qlen][in] -> y [qlen][out] in hidden_type (x is quantised per token and 128 values inside the kernel, exactly like
  * act_quant; rows >= *bsz untouched).  An all-zero 128-block of x yields NaN outputs, as it does in the reference (0 / 0).
- * TMA + tcgen05.mma.kind::f8f6f4 + TMEM; stream-ordered; everything is allocated at create -> CUDA-graph capturable.
+ * TMA + fp16 wgmma on e4m3 weights widened in registers; stream-ordered; everything is allocated at create -> CUDA-graph capturable.
  * ------------------------------------------------------------------------------------------ */
 typedef struct ktb200_fp8_linear ktb200_fp8_linear;
 int ktb200_fp8_linear_create(int in_features, int out_features, const void* weight_e4m3_dev, const float* weight_scale_inv_dev, int hidden_type, int device,
@@ -316,7 +316,7 @@ int ktb200_mla_decode(const ktb200_mla_params* p, void* stream);
 /* Diagnostics: while non-NULL, one CTA of ktb200_mla_decode dumps the raw scores of its first tile (>= 2048 floats). */
 void ktb200_debug_mla(float* debug_dev);
 /* Debug aid of the grouped (prefill) expert GEMM: when non-null, CTA 0 of the gate and down GEMMs writes clock64 stamps of its
- * first 96 stages, [kernel 2][role 3 = producer, issuer, epilogue][stage 96][4] int64 (tools/grouped_probe.py prints them). */
+ * first 96 stages, [kernel 2][role 3 = producer, MMA warpgroup, unused][stage 96][4] int64 (tools/grouped_probe.py prints them). */
 void ktb200_debug_grouped(long long* trace_dev);
 
 /* ------------------------------------------------------------------------------------------

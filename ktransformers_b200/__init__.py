@@ -1,4 +1,4 @@
-"""ktransformers_b200 — B200-native (sm_100a) drop-in for kt-kernel's quantized-MoE decode hot path.
+"""ktransformers_b200 — H100-native (sm_90a) drop-in for kt-kernel's quantized-MoE decode hot path.
 
 Layout mirrors the slice of the reference it replaces:
 

@@ -1,4 +1,4 @@
-// Shared device helpers for the ktb200 kernels (sm_100a only).
+// Shared device helpers for the ktb200 kernels (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

@@ -1,7 +1,7 @@
 // Dense Q4_K linear (y = x . W^T, decode batches of <= 8 rows) on the bulk-copy ring: q_a / kv_a / q_b / o_proj of the MLA
 // block and every other KLinearB200 with Q4_K weights (archive/ktransformers/operators/linear.py:57-155 KLinearBase.forward;
 // CPU twin operators/llamafile/linear.cpp:37-70).  The expert kernel (rows_bulk_q4k_kernel) wants rows of >= 16 super-
-// blocks — one lane per block — which leaves q_b (6 blocks per row) on the register-staged kernel at ~1 TB/s and gives
+// blocks — one lane per block — which leaves q_b (6 blocks per row) on the slower register-staged kernel and gives
 // o_proj (64 blocks per row) 9 KB slots.  Here a ring slot is a SEGMENT of <= 32 consecutive blocks of the row-major weight
 // stream, one lane per block:
 //     short rows (nblk <= 16): a segment is R = 32 / nblk whole rows (one contiguous copy), reduced per group of nblk lanes

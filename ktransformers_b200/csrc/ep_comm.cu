@@ -1,7 +1,7 @@
 // Expert-parallel token exchange over NVLink peer memory (one process per GPU; every rank maps the others' buffers).
 //
 // Replaces the two latency-bound NCCL collectives of an expert-parallel decode layer (all-gather of the N tokens,
-// reduce-scatter of the N x H fp32 partial sums: ~12 us each at these sizes) with two small hand-written kernels that
+// reduce-scatter of the N x H fp32 partial sums) with two small hand-written kernels that
 // store / load peer memory directly and synchronise with system-scope flags:
 //
 //   ktb200_ep_all_gather_tokens   rank r stores its token row into row r of EVERY peer's token buffer (14 KB each),

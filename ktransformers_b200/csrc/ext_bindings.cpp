@@ -69,7 +69,7 @@ class CPUInfer {   // kt-kernel/cpu_backend/cpuinfer.h:39-119: here a stream-ord
     }
 };
 
-class B200_MOE {   // the T of bind_moe_module<T>: GGUF K-quant experts resident in HBM on the sm_100a kernels
+class B200_MOE {   // the T of bind_moe_module<T>: GGUF K-quant experts resident in HBM on the sm_90a kernels
    public:
     explicit B200_MOE(const GeneralMOEConfig& c) : config(c) {
         ktb200_moe_config k{};
@@ -116,7 +116,7 @@ static void forward_inner(void* a) {
         [](cls& self, uintptr_t val) { self.name = reinterpret_cast<void*>(val); })
 
 PYBIND11_MODULE(kt_kernel_ext_b200, m) {
-    m.doc() = "B200 (sm_100a) drop-in for kt_kernel_ext's MoE path";
+    m.doc() = "H100 (sm_90a) drop-in for kt_kernel_ext's MoE path";
     m.def("version", [] { return std::string(ktb200_version()); });
     py::class_<CPUInfer>(m, "CPUInfer")
         .def(py::init<int>())

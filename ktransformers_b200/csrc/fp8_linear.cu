@@ -3,12 +3,19 @@
 //     s[t][kb] = max|x[t][128 kb .. +128]| / 448,   xq = e4m3(x / s)                         (per token and 128 of K)
 //     acc[t][n] += dot_e4m3(xq[t][kb], W[n][kb]) * s[t][kb] * scale_inv[n / 128][kb]          fp32, kb ascending
 //     y = cast(acc)
-// One byte per weight: a pure HBM stream.  The weights never pass through registers: TMA drops [128 rows x 128 bytes] boxes of W
-// into shared memory in the 128-byte-swizzle layout, which IS the K-major A operand of tcgen05.mma.kind::f8f6f4; the quantised
-// activations (16 token rows, padded) are the B operand; the products of two e4m3 values are exact in the fp32 accumulator (TMEM).
-// After every 128 of K (4 MMAs) the epilogue takes the partial dot out of TMEM and applies the two scales in the reference's order.
-//     grid = (ceil(N / 128) row tiles, K splits), two CTAs per SM; 192 threads: warp 0 TMA producer (4-stage ring), warp 1 issuer,
-//     warps 2-5 quantise x for the CTA's K range while the first weight boxes are in flight, then run the epilogue.
+// One byte per weight: a pure HBM stream.  TMA drops [128 rows x 128 bytes] boxes of W into shared memory (128-byte swizzle);
+// each MMA warpgroup widens its 64 rows to fp16 in registers (exact: e4m3 is a subset of fp16) and feeds them as the A operand
+// of an fp16 wgmma whose B operand is the quantised activations (16 token rows, padded), also held as fp16.  The products of two
+// e4m3 values are exact and sum in fp32; the e4m3 form of the MMA would sum them with fewer bits on this architecture.  Every
+// 128 of K (8 MMAs of K = 16) the partial dot is taken out of the accumulator and the two scales are applied in the
+// reference's order.
+// K order inside each 64-value half of a 128 block: the thread that supplies weight row r for the MMA reads 16 contiguous
+// bytes, physical k = 16 c + 4 s + e (c = lane % 4, s = the K = 16 step of the half, e = 0..3), and hands them to the fragment
+// slots that the MMA treats as logical k = 16 s + 2 c + e (e < 2) and 16 s + 8 + 2 c + (e - 2); the B tile stores x in that
+// same logical order (a permutation of K inside a dot product changes nothing).
+//     grid = (ceil(N / 128) row tiles, K splits), two CTAs per SM; 288 threads: warps 0-7 = two warpgroups of 64 weight rows
+//     each (quantise x for the CTA's K range while the first weight boxes are in flight, then MMA and scale), warp 8 the TMA
+//     producer (4-stage ring).
 // K splits add their fp32 partial sums with atomics into a zeroed workspace; the last CTA of a row tile converts and re-zeroes.
 #include <cuda.h>
 #include <cuda_fp8.h>
@@ -17,17 +24,17 @@
 
 #include "common.cuh"
 #include "handles.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace ktb {
-using namespace umma;
+using namespace wg;
 
 constexpr int kFT = 16;                    // token rows per pass (the MMA's N)
-constexpr int kFStages = 4, kFA = 128 * 128, kFB = kFT * 128, kFMaxKb = 16;   // 64 + 32 KB: two CTAs per SM, 128 KB of weight boxes in flight
+constexpr int kFStages = 4, kFA = 128 * 128, kFB = kFT * 128 * 2, kFMaxKb = 8;   // 64 + 32 KB: two CTAs per SM, 128 KB of weight boxes in flight
 constexpr int kFOffB = kFStages * kFA, kFOffS = kFOffB + kFMaxKb * kFB, kFOffMisc = kFOffS + kFT * kFMaxKb * 4;
+constexpr int kFConsumerWarps = 8, kFThreads = (kFConsumerWarps + 1) * 32;
 struct Fp8Misc {
-    unsigned long long a_full[kFStages], a_free[kFStages], d_full[2], d_free[2], b_ready;
-    uint32_t tmem_base;
+    unsigned long long a_full[kFStages], a_free[kFStages];
     int last;
 };
 constexpr int kFSmem = kFOffMisc + (int)sizeof(Fp8Misc) + 1024;
@@ -39,8 +46,8 @@ struct Fp8Params {
     float* ws;                // [kFT][N] fp32, zero between calls (K splits only)
     unsigned* tickets;        // [row tiles], zero between calls
     const int* bsz;
-    const uint8_t* xq;        // [kFT][K] e4m3 and
-    const float* xs;          // [kFT][nkb] scales from fp8_act_quant_kernel (batches of more than 2 tokens), else null
+    const uint8_t* xq;        // [T][K] e4m3 and
+    const float* xs;          // [T][nkb] scales from fp8_act_quant_kernel (batches of more than 2 tokens), else null
     int hidden_type, T, K, N, nkb, kb_per_split, ksplit, t0;
 };
 
@@ -70,6 +77,19 @@ __device__ __forceinline__ void fp8_load4(const void* x, long off, int hidden_ty
         }
     }
 }
+// 4 e4m3 bytes (physical k = 4 q .. 4 q + 3 of a 128 block) of token row t -> the fp16 B tile of that block (see the K order above)
+__device__ __forceinline__ void fp8_store_b(uint8_t* bt, int t, int q, uint32_t packed) {
+    const int h = q >> 4, c = (q >> 2) & 3, s = q & 3, l0 = 16 * s + 2 * c, l1 = l0 + 8;
+    const __half2_raw lo = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(packed & 0xffffu), __NV_E4M3);
+    const __half2_raw hi = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(packed >> 16), __NV_E4M3);
+    uint8_t* row = bt + h * (kFT * 128) + t * 128;
+    *reinterpret_cast<uint32_t*>(row + (((l0 >> 3) ^ (t & 7)) << 4) + (l0 & 7) * 2) = (uint32_t)lo.x | ((uint32_t)lo.y << 16);
+    *reinterpret_cast<uint32_t*>(row + (((l1 >> 3) ^ (t & 7)) << 4) + (l1 & 7) * 2) = (uint32_t)hi.x | ((uint32_t)hi.y << 16);
+}
+__device__ __forceinline__ uint32_t fp8x2_to_f16x2(uint32_t two) {
+    const __half2_raw v = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)two, __NV_E4M3);
+    return (uint32_t)v.x | ((uint32_t)v.y << 16);
+}
 // batches of more than 2 tokens: quantise x ONCE (one warp per block) instead of once per row tile
 __global__ void __launch_bounds__(256) fp8_act_quant_kernel(const void* x, int hidden_type, int T, int K, uint8_t* xq, float* xs) {
     const int lane = threadIdx.x & 31, blk = blockIdx.x * 8 + (threadIdx.x >> 5), nkb = K / 128;
@@ -84,7 +104,7 @@ __global__ void __launch_bounds__(256) fp8_act_quant_kernel(const void* x, int h
     if (lane == 0) xs[t * nkb + kb] = s;
 }
 
-__global__ void __launch_bounds__(192, 2) fp8_linear_kernel(const __grid_constant__ CUtensorMap wmap, const Fp8Params p) {
+__global__ void __launch_bounds__(kFThreads, 2) fp8_linear_kernel(const __grid_constant__ CUtensorMap wmap, const Fp8Params p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
@@ -95,20 +115,14 @@ __global__ void __launch_bounds__(192, 2) fp8_linear_kernel(const __grid_constan
     const int row0 = blockIdx.x * 128;
     const int kb0 = blockIdx.y * p.kb_per_split, nk = min(p.kb_per_split, p.nkb - kb0);
     if (tid == 0) {
-        for (int s = 0; s < kFStages; s++) { bar_init(smem_u32(&misc.a_full[s]), 1); bar_init(smem_u32(&misc.a_free[s]), 1); }
-        for (int b = 0; b < 2; b++) { bar_init(smem_u32(&misc.d_full[b]), 1); bar_init(smem_u32(&misc.d_free[b]), 4); }
-        bar_init(smem_u32(&misc.b_ready), 4);
+        for (int s = 0; s < kFStages; s++) { bar_init(smem_u32(&misc.a_full[s]), 1); bar_init(smem_u32(&misc.a_free[s]), kFConsumerWarps); }
         bar_fence_init();
         tma_prefetch_desc(&wmap);
     }
-    if (warp == 1) tmem_alloc(smem_u32(&misc.tmem_base), 32);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = misc.tmem_base;
     griddep_launch_dependents();   // a PDL-launched successor may set up and prefetch its own weights while this grid streams
 
-    if (warp == 0) {
+    if (warp == kFConsumerWarps) {
         // ---------------------------------------------------------------- weight boxes: independent of x, start at once
         if (lane == 0) {
             for (int i = 0; i < nk; i++) {
@@ -118,121 +132,127 @@ __global__ void __launch_bounds__(192, 2) fp8_linear_kernel(const __grid_constan
                 tma_load_2d(base + s * kFA, &wmap, smem_u32(&misc.a_full[s]), (kb0 + i) * 128, row0);
             }
         }
-    } else if (warp == 1) {
-        // ---------------------------------------------------------------- issuer (converged warp)
-        constexpr uint32_t idesc = instr_desc(1, 0, 0, 0, 0, 128, kFT);   // f32 += e4m3 . e4m3, K-major both
-        bar_wait(smem_u32(&misc.b_ready), 0);
-        for (int i = 0; i < nk; i++) {
-            const int s = i % kFStages, buf = i & 1;
-            bar_wait(smem_u32(&misc.a_full[s]), (i / kFStages) & 1);
-            bar_wait(smem_u32(&misc.d_free[buf]), ((i >> 1) & 1) ^ 1);
-            tc_fence_after();
-#pragma unroll
-            for (int j = 0; j < 4; j++)
-                mma_f8(tmem + buf * kFT, smem_desc(base + s * kFA + j * 32, 16, 1024, kLayoutSw128), smem_desc(base + kFOffB + i * kFB + j * 32, 16, 1024, kLayoutSw128), idesc,
-                       j != 0);
-            mma_commit(smem_u32(&misc.a_free[s]));
-            mma_commit(smem_u32(&misc.d_full[buf]));
+        return;
+    }
+    // -------------------------------------------------------------------- act_quant for this K range (warps 0-7)
+    constexpr int kCT = kFConsumerWarps * 32;
+    // rows T .. 15 of the B tiles: zeros (their accumulator columns are never read)
+    for (int i = tid; i < nk * (kFB / 16); i += kCT) {
+        const int r = (i >> 3) & (kFT - 1);
+        if (r >= p.T) *reinterpret_cast<uint4*>(smem + kFOffB + i * 16) = make_uint4(0, 0, 0, 0);
+    }
+    griddep_wait();   // x (or its quantised copy) comes from the kernel before this one; the weight boxes above did not wait
+    if (p.xq) {
+        // already quantised by fp8_act_quant_kernel: this CTA's K range into the B tiles, 4 bytes per thread and step
+        for (int i = tid; i < p.T * nk * 32; i += kCT) {
+            const int q = i & 31, kb = (i >> 5) % nk, t = (i >> 5) / nk;
+            fp8_store_b(smem + kFOffB + kb * kFB, t, q, *reinterpret_cast<const uint32_t*>(p.xq + (long)t * p.K + (long)(kb0 + kb) * 128 + q * 4));
         }
+        for (int i = tid; i < p.T * nk; i += kCT) a_s[(i / nk) * p.kb_per_split + (i % nk)] = p.xs[(i / nk) * p.nkb + kb0 + (i % nk)];
     } else {
-        // ---------------------------------------------------------------- act_quant for this K range, then the epilogue
-        const int ew = warp - 2;
-        // rows T .. 15 of the B tiles: zeros (their accumulator columns are never read)
-        for (int i = (tid - 64); i < nk * (kFB / 16); i += 128) {
-            const int r = (i >> 3) & (kFT - 1);
-            if (r >= p.T) *reinterpret_cast<uint4*>(smem + kFOffB + i * 16) = make_uint4(0, 0, 0, 0);
-        }
-        griddep_wait();   // x (or its quantised copy) comes from the kernel before this one; the weight boxes above did not wait
-        if (p.xq) {
-            // already quantised by fp8_act_quant_kernel: copy this CTA's K range into the swizzled B tiles (16-byte pieces)
-            for (int i = tid - 64; i < p.T * nk * 8; i += 128) {
-                const int pc = i & 7, kb = (i >> 3) % nk, t = (i >> 3) / nk;
-                *reinterpret_cast<uint4*>(smem + kFOffB + kb * kFB + t * 128 + ((pc ^ (t & 7)) << 4)) =
-                    *reinterpret_cast<const uint4*>(p.xq + (long)t * p.K + (long)(kb0 + kb) * 128 + pc * 16);
-            }
-            for (int i = tid - 64; i < p.T * nk; i += 128) a_s[(i / nk) * p.kb_per_split + (i % nk)] = p.xs[(i / nk) * p.nkb + kb0 + (i % nk)];
-        } else {
-            // one warp per (token, 128 of K), lane owns 4 consecutive values; 8 blocks' loads are issued before the first is reduced
-            for (int g0 = ew; g0 < p.T * nk; g0 += 4 * 8) {
-                float v[8][4];
+        // one warp per (token, 128 of K), lane owns 4 consecutive values; 8 blocks' loads are issued before the first is reduced
+        for (int g0 = warp; g0 < p.T * nk; g0 += kFConsumerWarps * 8) {
+            float v[8][4];
 #pragma unroll
-                for (int u = 0; u < 8; u++) {
-                    const int blk = g0 + 4 * u;
-                    if (blk < p.T * nk) {
-                        const int t = blk / nk, kb = blk - t * nk;
-                        fp8_load4(p.x, (long)t * p.K + (long)(kb0 + kb) * 128 + lane * 4, p.hidden_type, v[u]);
-                    }
-                }
-#pragma unroll
-                for (int u = 0; u < 8; u++) {
-                    const int blk = g0 + 4 * u;
-                    if (blk < p.T * nk) {   // warp-uniform
-                        const int t = blk / nk, kb = blk - t * nk;
-                        uint32_t packed;
-                        const float s = fp8_quant_block(v[u], packed);
-                        *reinterpret_cast<uint32_t*>(smem + kFOffB + kb * kFB + t * 128 + (((lane >> 2) ^ (t & 7)) << 4) + (lane & 3) * 4) = packed;
-                        if (lane == 0) a_s[t * p.kb_per_split + kb] = s;
-                    }
+            for (int u = 0; u < 8; u++) {
+                const int blk = g0 + kFConsumerWarps * u;
+                if (blk < p.T * nk) {
+                    const int t = blk / nk, kb = blk - t * nk;
+                    fp8_load4(p.x, (long)t * p.K + (long)(kb0 + kb) * 128 + lane * 4, p.hidden_type, v[u]);
                 }
             }
-        }
-        fence_async_smem();
-        asm volatile("bar.sync 1, 128;" ::: "memory");   // a_s is read by all four epilogue warps
-        if (lane == 0) bar_arrive(smem_u32(&misc.b_ready));
-
-        const int sp = warp & 3, row = 32 * sp + lane;
-        float acc[kFT];
 #pragma unroll
-        for (int t = 0; t < kFT; t++) acc[t] = 0.f;
-        const float* sinv = p.scale_inv + (long)blockIdx.x * p.nkb + kb0;
-        for (int i = 0; i < nk; i++) {
-            const int buf = i & 1;
-            const float bs = __ldg(sinv + i);
-            bar_wait(smem_u32(&misc.d_full[buf]), (i >> 1) & 1);
-            tc_fence_after();
-            uint32_t d[kFT];
-            tmem_ld16(tmem + ((uint32_t)(32 * sp) << 16) + buf * kFT, d);
-            tmem_wait_ld();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) bar_arrive(smem_u32(&misc.d_free[buf]));
-#pragma unroll
-            for (int t = 0; t < kFT; t++)
-                if (t < p.T) acc[t] = __fadd_rn(acc[t], __fmul_rn(__fmul_rn(__uint_as_float(d[t]), a_s[t * p.kb_per_split + i]), bs));   // (dot * a_s) * b_s, then +=
-        }
-        const int n = row0 + row;
-        const int live = p.bsz ? max(0, min(p.T, *p.bsz - p.t0)) : p.T;   // rows at or beyond the live batch size stay untouched
-        if (p.ksplit == 1) {
-            if (n < p.N)
-#pragma unroll
-                for (int t = 0; t < kFT; t++)
-                    if (t < live) store_hidden(p.y, (long)t * p.N + n, p.hidden_type, acc[t]);
-        } else {
-            if (n < p.N)
-#pragma unroll
-                for (int t = 0; t < kFT; t++)
-                    if (t < p.T) atomicAdd(p.ws + (long)t * p.N + n, acc[t]);
-            __threadfence();
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            if (tid == 64) misc.last = atomicAdd(p.tickets + blockIdx.x, 1u) == (unsigned)(p.ksplit - 1);
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            if (misc.last) {
-                __threadfence();
-                if (n < p.N)
-                    for (int t = 0; t < p.T; t++) {
-                        const float v = __ldcg(p.ws + (long)t * p.N + n);
-                        p.ws[(long)t * p.N + n] = 0.f;
-                        if (t < live) store_hidden(p.y, (long)t * p.N + n, p.hidden_type, v);
-                    }
-                if (tid == 64) p.tickets[blockIdx.x] = 0;
+            for (int u = 0; u < 8; u++) {
+                const int blk = g0 + kFConsumerWarps * u;
+                if (blk < p.T * nk) {   // warp-uniform
+                    const int t = blk / nk, kb = blk - t * nk;
+                    uint32_t packed;
+                    const float s = fp8_quant_block(v[u], packed);
+                    fp8_store_b(smem + kFOffB + kb * kFB, t, lane, packed);
+                    if (lane == 0) a_s[t * p.kb_per_split + kb] = s;
+                }
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem, 32);
+    fence_async_smem();
+    asm volatile("bar.sync 1, %0;" ::"n"(kCT) : "memory");   // B tiles and a_s are read by both warpgroups
+
+    // -------------------------------------------------------------------- MMA + scales: warpgroup g owns weight rows 64 g .. 64 g + 63
+    const int g = warp >> 2, r0 = 64 * g + 16 * (warp & 3) + (lane >> 2), c = lane & 3;
+    float acc[8], d[8];
+#pragma unroll
+    for (int q = 0; q < 8; q++) acc[q] = 0.f;
+    const float* sinv = p.scale_inv + (long)blockIdx.x * p.nkb + kb0;
+    for (int i = 0; i < nk; i++) {
+        const int s = i % kFStages;
+        const float bs = __ldg(sinv + i);
+        bar_wait(smem_u32(&misc.a_full[s]), (i / kFStages) & 1);
+        uint4 w[2][2];   // [row r0, r0 + 8][half of the 128 block]: bytes 16 c .. 16 c + 15 of the half
+#pragma unroll
+        for (int rr = 0; rr < 2; rr++)
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int r = r0 + 8 * rr;
+                w[rr][h] = *reinterpret_cast<const uint4*>(smem + s * kFA + r * 128 + ((((4 * h + c) ^ (r & 7))) << 4));
+            }
+        uint32_t a[2][4][4];   // all A fragments of the block before the first MMA: no register writes between the MMAs
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int st = 0; st < 4; st++) {
+                const uint32_t w0 = st == 0 ? w[0][h].x : st == 1 ? w[0][h].y : st == 2 ? w[0][h].z : w[0][h].w;
+                const uint32_t w1 = st == 0 ? w[1][h].x : st == 1 ? w[1][h].y : st == 2 ? w[1][h].z : w[1][h].w;
+                a[h][st][0] = fp8x2_to_f16x2(w0 & 0xffffu); a[h][st][1] = fp8x2_to_f16x2(w1 & 0xffffu);
+                a[h][st][2] = fp8x2_to_f16x2(w0 >> 16); a[h][st][3] = fp8x2_to_f16x2(w1 >> 16);
+            }
+        fence();
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int st = 0; st < 4; st++)
+                mma_f16_rs_m64n16(d, a[h][st], smem_desc(base + kFOffB + i * kFB + h * (kFT * 128) + st * 32, 16, 1024, kLayoutSw128), (h | st) != 0);
+        commit();
+        wait<0>();
+        fence_regs(d);
+        // free the stage only now: the MMAs that consumed the registers loaded from it have completed, so every one of those
+        // shared-memory loads has delivered before TMA may overwrite the stage
+        __syncwarp();
+        if (lane == 0) bar_arrive(smem_u32(&misc.a_free[s]));
+#pragma unroll
+        for (int q = 0; q < 8; q++) {   // register q: token 8 (q / 4) + 2 (lane % 4) + q % 2, row r0 + 8 (q / 2 % 2)
+            const int t = 8 * (q >> 2) + 2 * (lane & 3) + (q & 1);
+            if (t < p.T) acc[q] = __fadd_rn(acc[q], __fmul_rn(__fmul_rn(d[q], a_s[t * p.kb_per_split + i]), bs));   // (dot * a_s) * b_s, then +=
+        }
+    }
+    const int live = p.bsz ? max(0, min(p.T, *p.bsz - p.t0)) : p.T;   // rows at or beyond the live batch size stay untouched
+    if (p.ksplit == 1) {
+#pragma unroll
+        for (int q = 0; q < 8; q++) {
+            const int t = 8 * (q >> 2) + 2 * (lane & 3) + (q & 1), n = row0 + r0 + 8 * ((q >> 1) & 1);
+            if (t < live && n < p.N) store_hidden(p.y, (long)t * p.N + n, p.hidden_type, acc[q]);
+        }
+    } else {
+#pragma unroll
+        for (int q = 0; q < 8; q++) {
+            const int t = 8 * (q >> 2) + 2 * (lane & 3) + (q & 1), n = row0 + r0 + 8 * ((q >> 1) & 1);
+            if (t < p.T && n < p.N) atomicAdd(p.ws + (long)t * p.N + n, acc[q]);
+        }
+        __threadfence();
+        asm volatile("bar.sync 1, %0;" ::"n"(kCT) : "memory");
+        if (tid == 0) misc.last = atomicAdd(p.tickets + blockIdx.x, 1u) == (unsigned)(p.ksplit - 1);
+        asm volatile("bar.sync 1, %0;" ::"n"(kCT) : "memory");
+        if (misc.last) {
+            __threadfence();
+            for (int i = tid; i < 128 * p.T; i += kCT) {
+                const int t = i >> 7, n = row0 + (i & 127);
+                if (n < p.N) {
+                    const float v = __ldcg(p.ws + (long)t * p.N + n);
+                    p.ws[(long)t * p.N + n] = 0.f;
+                    if (t < live) store_hidden(p.y, (long)t * p.N + n, p.hidden_type, v);
+                }
+            }
+            if (tid == 0) p.tickets[blockIdx.x] = 0;
+        }
     }
 }
 
@@ -327,10 +347,10 @@ int ktb200_fp8_linear_forward(ktb200_fp8_linear* l, int qlen, const void* x, voi
         if (p.T > 2) {   // quantise once, then the GEMM as a programmatic dependent launch: its weight boxes stream while the quantiser drains
             p.xq = l->xq; p.xs = l->xs;
             fp8_act_quant_kernel<<<(p.T * l->nkb + 7) / 8, 256, 0, (cudaStream_t)stream>>>(p.x, l->hidden_type, p.T, l->K, l->xq, l->xs);
-            KTB_CUDA_CHECK(launch_pdl(fp8_linear_kernel, dim3(l->row_tiles, l->ksplit), dim3(192), (size_t)kFSmem, (cudaStream_t)stream, l->map, p));
+            KTB_CUDA_CHECK(launch_pdl(fp8_linear_kernel, dim3(l->row_tiles, l->ksplit), dim3(kFThreads), (size_t)kFSmem, (cudaStream_t)stream, l->map, p));
             count_launch(2);
         } else {
-            KTB_CUDA_CHECK(launch_pdl(fp8_linear_kernel, dim3(l->row_tiles, l->ksplit), dim3(192), (size_t)kFSmem, (cudaStream_t)stream, l->map, p));
+            KTB_CUDA_CHECK(launch_pdl(fp8_linear_kernel, dim3(l->row_tiles, l->ksplit), dim3(kFThreads), (size_t)kFSmem, (cudaStream_t)stream, l->map, p));
             count_launch(1);
         }
     }

@@ -1,4 +1,4 @@
-// Streaming integer GEMV kernels for quantised-MoE decode (sm_100a).
+// Streaming integer GEMV kernels for quantised-MoE decode (sm_90a).
 //
 // Both kernels are HBM-bound byte streamers (3.1 FLOP/B at bs=1): every weight byte is read exactly
 // once with 16-byte read-only loads that bypass L1, many loads are put in flight per lane before any

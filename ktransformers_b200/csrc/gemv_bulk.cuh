@@ -1,7 +1,6 @@
 // Fourth generation of the expert GEMV kernels: bulk-copy (TMA engine) staging + one lane per super-block.
 //
-// What ncu said about the cp.async generation (profiles/r01c_kernels.md): DRAM at ~50 % of peak, issue slots
-// 40-50 % busy with only 12 warps per SM, and of the ~700 warp instructions a warp spent per 8 KB unit almost
+// Why not the cp.async generation: of the ~700 warp instructions a warp spent per 8 KB unit almost
 // 230 were the copy itself (16 LDGSTS per lane, each with its own 64-bit address arithmetic) plus index
 // divisions — LSU/MIO time shared with the LDS of the dot product.  Here:
 //

@@ -1,38 +1,38 @@
-// Grouped expert GEMM for prefill-sized batches on the Blackwell tensor path — MOE::forward_many
+// Grouped expert GEMM for prefill-sized batches on the Hopper tensor path — MOE::forward_many
 // (archive/csrc/ktransformers_ext/operators/llamafile/moe.cpp:248-365 ≡ kt-kernel/operators/llamafile/moe.hpp:461-746):
 //     count tokens per expert -> per-token Q8_K quantisation + scatter into per-expert contiguous order ->
 //     per-expert GEMM (gate, up) -> silu * mul -> requantise -> per-expert GEMM (down) -> per-token weighted gather.
 // The decode kernels stream every (token, expert) pair's weights; here an expert's weights are read ONCE per 32-token tile.
 //
 // Arithmetic: the reference's dot is an exact integer per super-block — sum_j sc_j * (sum over sub-block j of q * x8) — scaled in
-// fp32.  The integer tensor path (tcgen05.mma kind::i8, s32 accumulators in TMEM) computes the INNER sums exactly: one MMA of
-// K = 32 per Q4_K sub-block (A = the raw 4-bit quants as u8, B = the Q8_K activation bytes), its own accumulator per sub-block;
-// Q6_K sub-blocks are 16 long, so one K = 32 MMA covers two of them against a B operand of 64 rows — the 32 tokens with the odd
-// sub-block zeroed, then the 32 tokens with the even one zeroed.  The epilogue multiplies every accumulator by its 6/8-bit
-// sub-block scale in int32, converts ONCE per super-block and applies (d_w * d_x) * isum - (dmin_w * d_x) * msum in fp32, the
-// decode kernels' formula; msum (Q4_K mins x activation block sums) is one K = 16 fp16 MMA of exact small integers.
+// fp32.  The integer tensor path (wgmma u8/s8 . s8 -> s32) computes the INNER sums exactly: one MMA of K = 32 per Q4_K sub-block
+// (A = the raw 4-bit quants as u8, B = the Q8_K activation bytes), its own accumulator per sub-block; Q6_K sub-blocks are 16
+// long, so one K = 32 MMA covers two of them against a B operand of 64 rows — the 32 tokens with the odd sub-block zeroed, then
+// the 32 tokens with the even one zeroed.  The MMA warpgroups multiply every accumulator by its 6/8-bit sub-block scale in
+// int32, convert ONCE per super-block and apply (d_w * d_x) * isum - (dmin_w * d_x) * msum in fp32, the decode kernels'
+// formula; msum (Q4_K mins x activation block sums) is one K = 16 fp16 MMA of exact small integers.
 // Nothing is rounded that the reference does not round.
 //
 // grouped_gemm_kernel: persistent CTAs, tile = (expert, 128 weight rows, 32 tokens), stage = half a super-block (128 of K):
 //     warps 0-7    producers (half a weight row per thread): weights (global, 16-byte loads, next stage prefetched in registers) -> int8 A tile in the K-major
 //                  128-byte-swizzle layout (Q4_K: nibble split; Q6_K: 4 + 2 bit merge, -32); activation rows gathered through the
-//                  sorted pair list -> B tile; row headers (scales, d, dmin) and token scales for the epilogue
-//     warp  8      tcgen05 issuer: 4 integer MMAs per stage (+ the mins MMA on the second half), 4 shared-memory stages,
-//                  2 TMEM buffers of 256 columns
-//     warps 9-16   epilogue: tcgen05.ld, int32 scale-and-add, fp32 finish per super-block, stores at the end of the tile
+//                  sorted pair list -> B tile; row headers (scales, d, dmin) and token scales for the scale-and-add
+//     warps 8-15   two MMA warpgroups, 64 weight rows each: the integer MMAs of a stage (+ the mins MMA on the second half),
+//                  int32 scale-and-add in registers, fp32 finish per super-block, stores at the end of the tile; 3 shared-memory
+//                  stages between the two roles
 #include <cuda_fp16.h>
 
 #include "act_quant.cuh"
 #include "common.cuh"
 #include "handles.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace ktb {
 
-using namespace umma;
+using namespace wg;
 
 constexpr int kGM = 128, kGN = 32, kGStages = 3, kGRaw = 6, kGHdr = 6;
-constexpr int kGProdWarps = 8, kGEpiWarps = 8, kGThreads = (kGProdWarps + 1 + kGEpiWarps) * 32;   // 17 warps: at most 5 per scheduler, 96 registers each
+constexpr int kGProdWarps = 8, kGMmaWarps = 8, kGThreads = (kGProdWarps + kGMmaWarps) * 32;   // 16 warps: producers 96 registers, MMA warpgroups 160
 constexpr int kGA = kGM * 128;            // 16,384: 128 rows x 128 int8 of K, one swizzle atom column
 constexpr int kGB = 2 * kGN * 128;        //  8,192: 32 rows (Q4_K) or 64 rows (Q6_K even / odd variants)
 constexpr int kGA2 = kGM * 32, kGB2 = kGN * 32;
@@ -41,9 +41,8 @@ constexpr int kOffB = kGStages * kGA, kOffA2 = kOffB + kGStages * kGB, kOffB2 = 
               kOffMiscG = kOffRaw + kGRaw * kRawSlot;
 
 struct GrpMisc {
-    unsigned long long ab_full[kGStages], smem_free[kGStages], tmem_full[2], tmem_free[2], hdr_free[kGHdr];
-    uint32_t tmem_base, pad[3];
-    // what only the epilogue reads rides in its own, deeper ring: the operand stages are released by the MMAs alone
+    unsigned long long ab_full[kGStages], smem_free[kGStages], hdr_free[kGHdr];
+    // what only the scale-and-add reads rides in its own, deeper ring
     float dxs[kGHdr][kGN];
     uint4 hdr[kGHdr][kGM];      // Q4_K: the block header (d, dmin, 12 scale bytes); Q6_K: 8 scales of the half, d as f32
 };
@@ -62,7 +61,7 @@ struct GrpGemmParams {
     const int* nt_prefix;      // [E + 1] 32-token tiles before every expert
     int E;
     float* out;                // [P][R] fp32
-    long long* trace;          // optional (ktb200_debug_grouped): clock64 stamps of CTA 0, [role 3][stage 96][4]
+    long long* trace;          // optional (ktb200_debug_grouped): clock64 stamps of CTA 0, [role 3][stage 96][4] (role 2 unused)
 };
 
 // byte b of a register array (b is a compile-time constant after unrolling: no local-memory byte addressing)
@@ -114,16 +113,11 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nblk = p.Kc / QK_K, nst = 2 * nblk, MT = p.R / kGM;
     if (tid == 0) {
-        for (int s = 0; s < kGStages; s++) { bar_init(smem_u32(&misc.ab_full[s]), kGProdWarps); bar_init(smem_u32(&misc.smem_free[s]), 1); }
-        for (int s = 0; s < kGHdr; s++) bar_init(smem_u32(&misc.hdr_free[s]), kGEpiWarps);
-        for (int b = 0; b < 2; b++) { bar_init(smem_u32(&misc.tmem_full[b]), 1); bar_init(smem_u32(&misc.tmem_free[b]), kGEpiWarps); }
+        for (int s = 0; s < kGStages; s++) { bar_init(smem_u32(&misc.ab_full[s]), kGProdWarps); bar_init(smem_u32(&misc.smem_free[s]), kGMmaWarps); }
+        for (int s = 0; s < kGHdr; s++) bar_init(smem_u32(&misc.hdr_free[s]), kGMmaWarps);
         bar_fence_init();
     }
-    if (warp == kGProdWarps) tmem_alloc(smem_u32(&misc.tmem_base), 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = misc.tmem_base;
     const int total_tiles = p.nt_prefix[p.E] * MT;
     int stage = 0, sphase = 0;   // shared-memory stage of the current iteration and how often it has wrapped (parity)
     int hs = 0, hphase = 0;      // the same for the header ring
@@ -131,6 +125,7 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
     if (warp < kGProdWarps) {
         // ========================================================================== producers: thread = (weight row r, half `part`)
         // `part` is warp-uniform (warps 0-3: first half of the row's share, warps 4-7: second) so that no branch below diverges
+        regs_dec<96>();
         const int pt = tid, r = pt & (kGM - 1), part = pt >> 7, sw = r & 7, bn = pt >> 3, pc = pt & 7;
         const uint32_t raw_dst = base + kOffRaw + pt * kRawPitch;
         const uint8_t* raw_src = smem + kOffRaw + pt * kRawPitch;
@@ -290,121 +285,107 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
             }
         }
         cp_async_wait<0>();
-    } else if (warp == kGProdWarps) {
-        // ========================================================================== tensor-core issuer (converged warp)
-        constexpr uint32_t idesc_i8 = FMT == 0 ? instr_desc(2, 0, 1, 0, 0, kGM, kGN) : instr_desc(2, 1, 1, 0, 0, kGM, 2 * kGN);   // s32 += (u8 | s8) . s8
-        constexpr uint32_t idesc_f16 = instr_desc(1, 0, 0, 0, 0, kGM, kGN);
-        unsigned it = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            for (int st = 0; st < nst; st++, it++) {
-                const int buf = it & 1;
-                const bool tr = p.trace && blockIdx.x == 0 && lane == 0 && tile == 0 && st < 96;
-                if (tr) p.trace[(1 * 96 + st) * 4 + 0] = clock64();
-                bar_wait(smem_u32(&misc.ab_full[stage]), sphase);
-                if (tr) p.trace[(1 * 96 + st) * 4 + 1] = clock64();
-                bar_wait(smem_u32(&misc.tmem_free[buf]), ((it >> 1) & 1) ^ 1);
-                if (tr) p.trace[(1 * 96 + st) * 4 + 2] = clock64();
-                tc_fence_after();
-                const uint32_t a = base + stage * kGA, b = base + kOffB + stage * kGB, d = tmem + buf * 256;
-#pragma unroll
-                for (int c = 0; c < 4; c++)
-                    mma_i8(d + c * (FMT == 0 ? 32 : 64), smem_desc(a + c * 32, 16, 1024, kLayoutSw128), smem_desc(b + c * 32, 16, 1024, kLayoutSw128), idesc_i8, 0);
-                if (FMT == 0 && (st & 1))
-                    mma_f16(d + 128, smem_desc(base + kOffA2 + stage * kGA2, 128, 256, kLayoutNone), smem_desc(base + kOffB2 + stage * kGB2, 128, 256, kLayoutNone), idesc_f16, 0);
-                mma_commit(smem_u32(&misc.smem_free[stage]));
-                mma_commit(smem_u32(&misc.tmem_full[buf]));
-                if (tr) p.trace[(1 * 96 + st) * 4 + 3] = clock64();
-                if (++stage == kGStages) { stage = 0; sphase ^= 1; }
-            }
-        }
     } else {
-        // ========================================================================== epilogue: 8 warps = 128 rows x 2 column halves
-        const int ew = warp - kGProdWarps - 1, sp = warp & 3, ch = ew >> 2, row = 32 * sp + lane;
-        const uint32_t tbase = tmem + ((uint32_t)(32 * sp) << 16) + 16 * ch;
-        unsigned it = 0;
+        // ========================================================================== MMA warpgroups: g owns weight rows 64 g .. 64 g + 63
+        // thread = rows ra = 64 g + 16 (warp % 4) + lane / 4 and ra + 8; accumulator register 4 jb + 2 h + e holds row ra + 8 h,
+        // column 8 jb + 2 (lane % 4) + e; isum / acc use the same index for (row, token) with the token columns of jb < 4
+        regs_inc<160>();   // 256 x 96 + 256 x 160 = 64 K registers
+        const int mw = warp - kGProdWarps, g = mw >> 2, ra = 64 * g + 16 * (mw & 3) + (lane >> 2), cq = 2 * (lane & 3);
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int4 ti = __ldg(p.tinfo + tile);
             float acc[16];
             int isum[16];
 #pragma unroll
-            for (int n = 0; n < 16; n++) { acc[n] = 0.f; isum[n] = 0; }
-            for (int st = 0; st < nst; st++, it++) {
-                const int buf = it & 1, hh = st & 1;
-                const bool tr = p.trace && blockIdx.x == 0 && ew == 0 && lane == 0 && tile == 0 && st < 96;
-                if (tr) p.trace[(2 * 96 + st) * 4 + 0] = clock64();
-                bar_wait(smem_u32(&misc.tmem_full[buf]), (it >> 1) & 1);
-                if (tr) p.trace[(2 * 96 + st) * 4 + 1] = clock64();
-                tc_fence_after();
-                const uint4 hd = misc.hdr[hs][row];
-                const uint32_t hw[4] = {hd.x, hd.y, hd.z, hd.w};
-                const uint32_t d = tbase + buf * 256;
+            for (int i = 0; i < 16; i++) { acc[i] = 0.f; isum[i] = 0; }
+            for (int st = 0; st < nst; st++) {
+                const int hh = st & 1;
+                const bool tr = p.trace && blockIdx.x == 0 && mw == 0 && lane == 0 && tile == 0 && st < 96;
+                if (tr) p.trace[(1 * 96 + st) * 4 + 0] = clock64();
+                bar_wait(smem_u32(&misc.ab_full[stage]), sphase);
+                if (tr) p.trace[(1 * 96 + st) * 4 + 1] = clock64();
+                const uint32_t a = base + stage * kGA + g * (kGA / 2), b = base + kOffB + stage * kGB;
+                uint32_t hw[2][4];
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const uint4 hd = misc.hdr[hs][ra + 8 * h];
+                    hw[h][0] = hd.x; hw[h][1] = hd.y; hw[h][2] = hd.z; hw[h][3] = hd.w;
+                }
                 if (FMT == 0) {
-                    int sc[4], mn;
-                    if (hh == 0) {
+                    int sc[2][4], mn;
 #pragma unroll
-                        for (int c = 0; c < 4; c++) q4k_scale_min(hw, c, sc[c], mn);
-                    } else {
+                    for (int h = 0; h < 2; h++) {   // (compile-time byte indices: no local-memory copy of the header)
+                        if (hh == 0) {
 #pragma unroll
-                        for (int c = 0; c < 4; c++) q4k_scale_min(hw, 4 + c, sc[c], mn);
+                            for (int c = 0; c < 4; c++) q4k_scale_min(hw[h], c, sc[h][c], mn);
+                        } else {
+#pragma unroll
+                            for (int c = 0; c < 4; c++) q4k_scale_min(hw[h], 4 + c, sc[h][c], mn);
+                        }
                     }
 #pragma unroll
                     for (int c = 0; c < 4; c += 2) {
                         uint32_t v0[16], v1[16];
-                        tmem_ld16(d + 32 * c, v0);
-                        tmem_ld16(d + 32 * c + 32, v1);
-                        tmem_wait_ld();
+                        fence();
+                        mma_u8s8_m64n32(v0, smem_desc(a + c * 32, 16, 1024, kLayoutSw128), smem_desc(b + c * 32, 16, 1024, kLayoutSw128), 0);
+                        mma_u8s8_m64n32(v1, smem_desc(a + c * 32 + 32, 16, 1024, kLayoutSw128), smem_desc(b + c * 32 + 32, 16, 1024, kLayoutSw128), 0);
+                        commit();
+                        wait<0>();
+                        fence_regs(v0);
+                        fence_regs(v1);
 #pragma unroll
-                        for (int n = 0; n < 16; n++) isum[n] += sc[c] * (int)v0[n] + sc[c + 1] * (int)v1[n];
+                        for (int i = 0; i < 16; i++) isum[i] += sc[(i >> 1) & 1][c] * (int)v0[i] + sc[(i >> 1) & 1][c + 1] * (int)v1[i];
                     }
                     if (hh == 1) {
-                        uint32_t ms[16];
-                        tmem_ld16(d + 128, ms);
-                        const __half2 dm = *reinterpret_cast<const __half2*>(&hw[0]);
-                        const float dw = __low2float(dm), dmin = __high2float(dm);
-                        tmem_wait_ld();
+                        float ms[16];
+                        fence();
+                        mma_f16_m64n32(ms, smem_desc(base + kOffA2 + stage * kGA2 + g * (kGA2 / 2), 128, 256, kLayoutNone),
+                                       smem_desc(base + kOffB2 + stage * kGB2, 128, 256, kLayoutNone), 0);
+                        commit();
+                        wait<0>();
+                        fence_regs(ms);
 #pragma unroll
-                        for (int n = 0; n < 16; n++) {
-                            const float dx = misc.dxs[hs][16 * ch + n];
-                            acc[n] += (dw * dx) * (float)isum[n] - (dmin * dx) * __uint_as_float(ms[n]);
-                            isum[n] = 0;
+                        for (int i = 0; i < 16; i++) {
+                            const __half2 dm = *reinterpret_cast<const __half2*>(&hw[(i >> 1) & 1][0]);
+                            const float dw = __low2float(dm), dmin = __high2float(dm);
+                            const float dx = misc.dxs[hs][8 * (i >> 2) + cq + (i & 1)];
+                            acc[i] += (dw * dx) * (float)isum[i] - (dmin * dx) * ms[i];
+                            isum[i] = 0;
                         }
                     }
                 } else {
 #pragma unroll
                     for (int c = 0; c < 4; c++) {
-                        uint32_t ve[16], vo[16];
-                        tmem_ld16(d + 64 * c, ve);
-                        tmem_ld16(d + 64 * c + 32, vo);
-                        const int se = sb8(hw, 2 * c), so = sb8(hw, 2 * c + 1);
-                        tmem_wait_ld();
+                        uint32_t v[32];
+                        fence();
+                        mma_s8s8_m64n64(v, smem_desc(a + c * 32, 16, 1024, kLayoutSw128), smem_desc(b + c * 32, 16, 1024, kLayoutSw128), 0);
+                        commit();
+                        wait<0>();
+                        fence_regs(v);
+                        // columns 0-31: the tokens against the even sub-block 2 c, columns 32-63: against the odd one
 #pragma unroll
-                        for (int n = 0; n < 16; n++) isum[n] += se * (int)ve[n] + so * (int)vo[n];
+                        for (int i = 0; i < 32; i++) isum[i & 15] += sb8(hw[(i >> 1) & 1], 2 * c + (i >> 4)) * (int)v[i];
                     }
                     if (hh == 1) {
-                        const float dw = __uint_as_float(hw[2]);
 #pragma unroll
-                        for (int n = 0; n < 16; n++) {
-                            acc[n] += (dw * misc.dxs[hs][16 * ch + n]) * (float)isum[n];
-                            isum[n] = 0;
+                        for (int i = 0; i < 16; i++) {
+                            acc[i] += (__uint_as_float(hw[(i >> 1) & 1][2]) * misc.dxs[hs][8 * (i >> 2) + cq + (i & 1)]) * (float)isum[i];
+                            isum[i] = 0;
                         }
                     }
                 }
-                tc_fence_before();
+                if (tr) p.trace[(1 * 96 + st) * 4 + 2] = clock64();
                 __syncwarp();
-                if (lane == 0) { bar_arrive(smem_u32(&misc.tmem_free[buf])); bar_arrive(smem_u32(&misc.hdr_free[hs])); }
-                if (tr) p.trace[(2 * 96 + st) * 4 + 3] = clock64();
+                if (lane == 0) { bar_arrive(smem_u32(&misc.smem_free[stage])); bar_arrive(smem_u32(&misc.hdr_free[hs])); }
+                if (tr) p.trace[(1 * 96 + st) * 4 + 3] = clock64();
+                if (++stage == kGStages) { stage = 0; sphase ^= 1; }
                 if (++hs == kGHdr) { hs = 0; hphase ^= 1; }
             }
 #pragma unroll
-            for (int n = 0; n < 16; n++)
-                if (16 * ch + n < ti.w) p.out[(long)(ti.z + 16 * ch + n) * p.R + ti.y + row] = acc[n];
+            for (int i = 0; i < 16; i++) {
+                const int n = 8 * (i >> 2) + cq + (i & 1);
+                if (n < ti.w) p.out[(long)(ti.z + n) * p.R + ti.y + ra + 8 * ((i >> 1) & 1)] = acc[i];
+            }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kGProdWarps) {
-        tc_fence_after();
-        tmem_dealloc(tmem, 512);
     }
 }
 

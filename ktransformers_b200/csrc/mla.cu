@@ -1,4 +1,4 @@
-// Absorbed-MLA paged decode attention on the Blackwell tensor path (tcgen05 + TMEM + TMA) and the paged latent KV write.
+// Absorbed-MLA paged decode attention on the Hopper tensor path (wgmma + TMA) and the paged latent KV write.
 //
 // Replaces MLAWrapper.run / flashinfer BatchMLAPagedAttentionWrapper
 // (archive/ktransformers/operators/flashinfer_wrapper.py:117-161, attention.py:419-447) and the Triton split-KV decode
@@ -7,60 +7,46 @@
 //     p      = softmax_t(s)   fp32, online; P is cast to bf16 before P.V            (triton_attention.py:137-141)
 //     out[h] = sum_t p[h,t] * ckv[t,:]                                             512 wide
 //
-// Work decomposition: CTA = (KV split, group of 64 heads, sequence); 6 warps with fixed roles
-//     warp 0      TMA producer: paged KV tiles of 32 tokens x 576 columns, 9 boxes of [32 rows x 64 columns] per tile
+// Work decomposition: CTA = (KV split, group of 64 heads, sequence); 3 warpgroups
+//     warp 8      TMA producer (the rest of its warpgroup only hands its registers to the other two): paged KV tiles of 32 tokens x 576 columns, 9 boxes of [32 rows x 64 columns] per tile
 //                 (cp.async.bulk.tensor, 128-byte swizzle) into a 4-stage ring, one mbarrier per stage
-//     warp 1      tensor-core issuer (one lane): S = Q.K^T and O^T = V^T.P^T as tcgen05.mma with TMEM accumulators
-//     warps 2..5  softmax / rescale / epilogue: tcgen05.ld of S, online softmax (thread = head), P -> shared memory
-// Both products read the SAME shared-memory tile: for S it is the K-major B operand [32 tokens x 576], for O^T its first
-// 512 columns are the MN-major A operand [latent x tokens] (the swizzle is a function of the shared-memory address only).
-// The output is accumulated TRANSPOSED — O^T[latent 512][head 64] = 4 blocks of 128 TMEM lanes x 64 columns — because a
-// [head][latent] accumulator for 64 heads would need 512 columns in the M=64 tcgen05 layout (half the lanes idle): the
-// whole tensor memory.  TMEM map (512 columns allocated): [0,256) O^T, [256,384) / [384,512) the two S buffers, each FOUR
-// partial accumulators of 32 columns: a 64 x 32 x 16 MMA is 16 cycles of work behind a pipeline several times as deep, so
-// 36 of them chained through ONE accumulator run at the latency, not the throughput (measured: ~75 cycles each); the 36
-// k-steps are dealt round-robin to four independent accumulators and the softmax warps add the four partial scores.
+//     warps 0..7  two warpgroups; warpgroup g owns latent columns [256 g, 256 g + 256) of the output.  Each computes
+//                 S = Q.K^T (64 heads x 32 tokens, wgmma from shared memory), the online softmax in registers, and
+//                 O[:, 256 g ..] += P.V with P straight from registers (the accumulator layout of S is the A-fragment
+//                 layout of P.V) and V read MN-major from the same tile (the swizzle is a function of the address only).
+// Both warpgroups compute the same S: the alternative, one S shared through shared memory, costs a CTA-wide hand-off per
+// tile, while the second S is 36 small MMAs on a tile whose load dominates the time.  The O accumulator (64 x 256 fp32 per
+// warpgroup) stays in registers for the whole split.
 //
-// Online softmax with a LAZY reference maximum: p = 2^(x - m_ref), m_ref is only raised (and O^T rescaled in TMEM, all
-// four warps) when some head's running maximum exceeds it by more than 8 — p stays <= 256, exact in bf16/fp32 terms —
-// so the steady-state tile costs no TMEM round trip of the accumulator.  Split-KV partials (fp32 O, base-2 LSE) are
-// merged by mla_merge_kernel.
+// Online softmax with a LAZY reference maximum: p = 2^(x - m_ref), m_ref is only raised (and the head's O row rescaled)
+// when the head's running maximum exceeds it by more than 8 — p stays <= 256, exact in bf16/fp32 terms.  Split-KV
+// partials (fp32 O, base-2 LSE) are merged by mla_merge_kernel.
 #include <cuda_bf16.h>
 
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace ktb {
 
-using namespace umma;
+using namespace wg;
 
 constexpr int kDK = 576;             // 512 latent + 64 rope
 constexpr int kDV = 512;
-constexpr int kHG = 64;              // heads per CTA (UMMA M of S)
-constexpr int kLT = 32;              // kv tokens per tile (UMMA N of S, K of O^T)
+constexpr int kHG = 64;              // heads per CTA (wgmma M)
+constexpr int kLT = 32;              // kv tokens per tile (N of S, K of P.V)
 constexpr int kStages = 4;
 constexpr int kChunks = kDK / 64;    // 9 column chunks of 64 bf16 = 128 B (one swizzle row)
-constexpr int kMlaThreads = 192;
+constexpr int kMlaConsumerWarps = 8, kMlaThreads = kMlaConsumerWarps * 32 + 128;
 constexpr int kStageBytes = kLT * kDK * 2;         // 36,864 = 9 regions of 32 rows x 128 B
 constexpr int kKRegion = kLT * 128;                // 4,096
 constexpr int kQRegion = kHG * 128;                // 8,192
 constexpr int kQBytes = kHG * kDK * 2;             // 73,728
-constexpr int kPBytes = kHG * kLT * 2;             // 4,096: [8 head groups][4 token groups][8 heads][8 tokens]
 constexpr int kOffQ = kStages * kStageBytes;       // 147,456
-constexpr int kOffP = kOffQ + kQBytes;             // 221,184
-constexpr int kOffMisc = kOffP + 2 * kPBytes;      // 229,376 (P is double-buffered)
-constexpr int kTmemCols = 512;
-constexpr int kColO = 0, kColS = 256;
-constexpr int kSChains = 4;          // independent partial-score accumulators per S buffer
+constexpr int kOffMisc = kOffQ + kQBytes;          // 221,184
 constexpr float kRescaleThreshold = 8.f;
 
 struct MlaMisc {
-    unsigned long long k_full[kStages], k_empty[kStages], s_full[2], s_empty[2], p_full, p_free[2];
-    uint32_t tmem_base;
-    int need[2][4];
-    float alpha[kHG];     // per head: 2^(m_ref_old - m_ref_new) of the current rescale
-    float l[kHG];         // final row sums
-    float m[kHG];         // final reference maxima
+    unsigned long long k_full[kStages], k_empty[kStages];
 };
 constexpr int kMlaSmem = kOffMisc + (int)sizeof(MlaMisc) + 1024;   // + slack to align the base to 1024 B
 static_assert(kMlaSmem <= 232448, "shared memory budget");
@@ -74,18 +60,13 @@ struct MlaKParams {
     float scale_log2;              // sm_scale * log2(e)
     float* o_part;                 // [B][splits][Hq][512]
     float* lse_part;               // [B][splits][Hq]  (base-2)
-    float* debug;                  // optional: S of the first tile [64][32], P bytes, see ktb200_debug_mla
+    float* debug;                  // optional: S of the first tile [64][32], see ktb200_debug_mla
 };
 
 __device__ __forceinline__ float ex2(float x) {   // 2^x, one MUFU (x = -inf -> 0)
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
-}
-__device__ __forceinline__ unsigned long long gtime() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
 }
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
     const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
@@ -119,46 +100,35 @@ __global__ void __launch_bounds__(kMlaThreads, 1) mla_decode_tc_kernel(const __g
         return;
     }
 
-    const bool dbg_cta = p.debug && tid == 0 && split == 0 && hg == 0 && b == 0;
-    if (dbg_cta) {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        reinterpret_cast<unsigned long long*>(p.debug + 2048)[0] = t;
-    }
     // ---- one-time setup -----------------------------------------------------------------------------------------
-    if (warp == 0 && lane == 0) {
+    auto issue_tile = [&](int j, int s) {
+        const int t_base = (tile0 + j) * kLT;
+        const int page = p.page_table[(long)b * p.max_pages + t_base / p.page_size];
+        const int row = page * p.page_size + t_base % p.page_size;
+        const uint32_t bar = smem_u32(&misc.k_full[s]);
+        bar_expect_tx(bar, kStageBytes);
+#pragma unroll
+        for (int c = 0; c < kChunks; c++) tma_load_2d(base + s * kStageBytes + c * kKRegion, &kv_map, bar, c * 64, row);
+    };
+    if (warp == kMlaConsumerWarps && lane == 0) {
         tma_prefetch_desc(&kv_map);
-        for (int s = 0; s < kStages; s++) { bar_init(smem_u32(&misc.k_full[s]), 1); bar_init(smem_u32(&misc.k_empty[s]), 1); }
-        for (int s = 0; s < 2; s++) { bar_init(smem_u32(&misc.s_full[s]), 1); bar_init(smem_u32(&misc.s_empty[s]), 4); }
-        bar_init(smem_u32(&misc.p_full), 4);
-        bar_init(smem_u32(&misc.p_free[0]), 1);
-        bar_init(smem_u32(&misc.p_free[1]), 1);
+        for (int s = 0; s < kStages; s++) { bar_init(smem_u32(&misc.k_full[s]), 1); bar_init(smem_u32(&misc.k_empty[s]), kMlaConsumerWarps); }
         bar_fence_init();
         // the first tiles do not depend on anything set up below: request them now
-        for (int j = 0; j < n && j < kStages; j++) {
-            const int t_base = (tile0 + j) * kLT;
-            const int page = p.page_table[(long)b * p.max_pages + t_base / p.page_size];
-            const int row = page * p.page_size + t_base % p.page_size;
-            const uint32_t bar = smem_u32(&misc.k_full[j]);
-            bar_expect_tx(bar, kStageBytes);
-#pragma unroll
-            for (int c = 0; c < kChunks; c++) tma_load_2d(base + j * kStageBytes + c * kKRegion, &kv_map, bar, c * 64, row);
-            if (p.debug && split == 0 && hg == 0 && b == 0) reinterpret_cast<unsigned long long*>(p.debug + 2048)[192 + j] = gtime();
-        }
+        for (int j = 0; j < n && j < kStages; j++) issue_tile(j, j);
     }
-    if (warp == 1) tmem_alloc(smem_u32(&misc.tmem_base), kTmemCols);
     // Q (64 heads x 576) -> shared memory in the K-major 128-byte-swizzle layout: chunk region c (64 columns) holds 64
     // rows of 128 B; the 16-byte piece j of row r sits at piece (j ^ (r & 7)).  Rows beyond num_heads are zero.
     {
-        constexpr int kPieces = kHG * (kDK / 8), kIter = kPieces / kMlaThreads;   // 4608 = 24 x 192
+        constexpr int kPieces = kHG * (kDK / 8), kIter = kPieces / kMlaThreads;   // 4608 = 12 x 384
         static_assert(kPieces % kMlaThreads == 0, "Q pieces");
-        constexpr int kB = 12;
+        constexpr int kB = 6;
         static_assert(kIter % kB == 0, "Q batches");
 #pragma unroll
         for (int i0 = 0; i0 < kIter; i0 += kB) {
             uint4 v[kB];
 #pragma unroll
-            for (int u = 0; u < kB; u++) {   // 12 independent 16-byte loads in flight per thread
+            for (int u = 0; u < kB; u++) {   // 6 independent 16-byte loads in flight per thread
                 const int i = tid + (i0 + u) * kMlaThreads, r = i / (kDK / 8), j = i - r * (kDK / 8);
                 v[u] = make_uint4(0, 0, 0, 0);
                 if (h0 + r < p.num_heads) {
@@ -175,225 +145,113 @@ __global__ void __launch_bounds__(kMlaThreads, 1) mla_decode_tc_kernel(const __g
         }
     }
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = misc.tmem_base;
-    if (dbg_cta) {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        reinterpret_cast<unsigned long long*>(p.debug + 2048)[1] = t;
-    }
 
-    if (warp == 0) {
+    if (warp >= kMlaConsumerWarps) {
         // ================================================================ TMA producer
-        if (lane == 0) {
+        regs_dec<40>();
+        if (warp == kMlaConsumerWarps && lane == 0) {
             for (int j = kStages; j < n; j++) {
                 const int s = j % kStages;
                 bar_wait(smem_u32(&misc.k_empty[s]), ((j / kStages) & 1) ^ 1);
-                const int t_base = (tile0 + j) * kLT;
-                const int page = p.page_table[(long)b * p.max_pages + t_base / p.page_size];
-                const int row = page * p.page_size + t_base % p.page_size;
-                const uint32_t bar = smem_u32(&misc.k_full[s]);
-                bar_expect_tx(bar, kStageBytes);
-#pragma unroll
-                for (int c = 0; c < kChunks; c++) tma_load_2d(base + s * kStageBytes + c * kKRegion, &kv_map, bar, c * 64, row);
-                if (p.debug && split == 0 && hg == 0 && b == 0 && j < 60) reinterpret_cast<unsigned long long*>(p.debug + 2048)[192 + j] = gtime();
+                issue_tile(j, s);
             }
         }
-        __syncwarp();
-    } else if (warp == 1) {
-        // ================================================================ tensor-core issuer (converged warp, see mma_f16)
-        {
-            constexpr uint32_t idesc_qk = instr_desc(1, 1, 1, 0, 0, kHG, kLT);    // f32 += bf16 . bf16, A K-major, B K-major, 64 x 32
-            constexpr uint32_t idesc_pv = instr_desc(1, 1, 1, 1, 0, 128, kHG);    // A MN-major (V^T from the [token][latent] tile), 128 x 64
-            auto issue_qk = [&](int j) {
-                const int s = j % kStages, buf = j & 1;
-                bar_wait(smem_u32(&misc.s_empty[buf]), ((j >> 1) & 1) ^ 1);
-                bar_wait(smem_u32(&misc.k_full[s]), (j / kStages) & 1);
-                tc_fence_after();
-                const uint32_t kb = base + s * kStageBytes, qb = base + kOffQ;
+        return;
+    }
+    // ==================================================================== the two warpgroups
+    regs_inc<232>();   // 128 x 40 + 256 x 232 <= 64 K registers
+    // thread = rows (heads) ra = 16 (warp % 4) + lane / 4 and ra + 8; accumulator register 4 jb + 2 h + e holds row ra + 8 h,
+    // column 8 jb + 2 (lane % 4) + e
+    const int g = warp >> 2, wt = tid & 127, ra = 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+    const uint32_t qb = base + kOffQ;
+    float o[128];
 #pragma unroll
-                for (int c = 0; c < kChunks; c++)
+    for (int i = 0; i < 128; i++) o[i] = 0.f;
+    float m_ref[2] = {-INFINITY, -INFINITY}, m_run[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};   // l: this thread's share of the row sum
+    for (int j = 0; j < n; j++) {
+        const int s = j % kStages;
+        const uint32_t kb = base + s * kStageBytes;
+        bar_wait(smem_u32(&misc.k_full[s]), (j / kStages) & 1);
+        float sv[16];
+        fence();
 #pragma unroll
-                    for (int k = 0; k < 4; k++)
-                        mma_f16(tmem + kColS + (buf * kSChains + (k & (kSChains - 1))) * kLT, smem_desc(qb + c * kQRegion + k * 32, 16, 1024, kLayoutSw128),
-                                smem_desc(kb + c * kKRegion + k * 32, 16, 1024, kLayoutSw128), idesc_qk, c != 0);
-                mma_commit(smem_u32(&misc.s_full[buf]));
-            };
-            issue_qk(0);
-            for (int j = 0; j < n; j++) {
-                if (j + 1 < n) issue_qk(j + 1);
-                bar_wait(smem_u32(&misc.p_full), j & 1);
-                tc_fence_after();
-                const int s = j % kStages;
-                const uint32_t kb = base + s * kStageBytes, pb = base + kOffP + (j & 1) * kPBytes;
+        for (int c = 0; c < kChunks; c++)
 #pragma unroll
-                for (int m = 0; m < 4; m++)
+            for (int k = 0; k < 4; k++)
+                mma_bf16_m64n32(sv, smem_desc(qb + c * kQRegion + k * 32, 16, 1024, kLayoutSw128), smem_desc(kb + c * kKRegion + k * 32, 16, 1024, kLayoutSw128),
+                                (c | k) != 0);
+        commit();
+        wait<0>();
+        fence_regs(sv);
+        if (p.debug && j == 0 && g == 0 && split == 0 && hg == 0 && b == 0)
 #pragma unroll
-                    for (int k = 0; k < 2; k++)
-                        mma_f16(tmem + kColO + m * kHG, smem_desc(kb + 2 * m * kKRegion + k * 2048, kKRegion, 1024, kLayoutSw128),
-                                smem_desc(pb + k * 256, 128, 512, kLayoutNone), idesc_pv, (j | k) != 0);
-                mma_commit(smem_u32(&misc.k_empty[s]));
-                mma_commit(smem_u32(&misc.p_free[j & 1]));
-                if (p.debug && lane == 0 && split == 0 && hg == 0 && b == 0 && j < 60) reinterpret_cast<unsigned long long*>(p.debug + 2048)[128 + j] = gtime();
+            for (int i = 0; i < 16; i++) p.debug[(ra + 8 * ((i >> 1) & 1)) * kLT + 8 * (i >> 2) + cq + (i & 1)] = sv[i];
+        const int t_base = (tile0 + j) * kLT;
+        float x[16], mt[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int i = 0; i < 16; i++) {
+            x[i] = (t_base + 8 * (i >> 2) + cq + (i & 1) < L) ? sv[i] * p.scale_log2 : -INFINITY;
+            mt[(i >> 1) & 1] = fmaxf(mt[(i >> 1) & 1], x[i]);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            mt[h] = fmaxf(mt[h], __shfl_xor_sync(0xffffffffu, mt[h], 1));
+            mt[h] = fmaxf(mt[h], __shfl_xor_sync(0xffffffffu, mt[h], 2));
+            m_run[h] = fmaxf(m_run[h], mt[h]);
+            // raise the reference maximum of this head? (never on the first tile: O is still zero)
+            if (j == 0) m_ref[h] = m_run[h];
+            else if (m_run[h] - m_ref[h] > kRescaleThreshold) {
+                const float a = ex2(m_ref[h] - m_run[h]);
+                l[h] *= a;
+                m_ref[h] = m_run[h];
+#pragma unroll
+                for (int jb = 0; jb < 32; jb++) { o[4 * jb + 2 * h] *= a; o[4 * jb + 2 * h + 1] *= a; }
             }
         }
-        __syncwarp();
-    } else {
-        // ================================================================ softmax / rescale / epilogue (4 warps)
-        // S rows of a sub-partition live in its TMEM lanes 0..15 (M = 64 layout): lane l < 16 loads the 32 scores of head
-        // 16 sp + l and hands tokens 16..31 to lane l + 16, so that all 32 lanes work: lane = (head, half of the tile).
-        const int sp = warp & 3;                       // TMEM sub-partition of this warp
-        const uint32_t lane_base = (uint32_t)(32 * sp) << 16;
-        const int upper = lane >> 4;
-        const int head = 16 * sp + (lane & 15);
-        const int st = tid - 64;                       // 0..127 among the softmax threads
-        float m_ref = -INFINITY, m_run = -INFINITY, l = 0.f;   // l: this lane's half of the row sum
-        for (int j = 0; j < n; j++) {
-            const int buf = j & 1;
-            bar_wait(smem_u32(&misc.s_full[buf]), (j >> 1) & 1);
-            tc_fence_after();
-            if (p.debug && st == 0 && split == 0 && hg == 0 && b == 0 && j < 60) reinterpret_cast<unsigned long long*>(p.debug + 2048)[64 + j] = gtime();
-            uint32_t sv[32];
-            {   // S = sum of the four partial accumulators
-                uint32_t t1[32], t2[32];
-                const uint32_t sa = tmem + lane_base + kColS + buf * kSChains * kLT;
-                tmem_ld32(sa, sv);
-                tmem_ld32(sa + kLT, t1);
-                tmem_wait_ld();
+        // P in bf16 as the A fragments of the two K = 16 steps: a[kk][i] = (p[8 kk + 2 i], p[8 kk + 2 i + 1])
+        uint32_t pa[2][4];
 #pragma unroll
-                for (int i = 0; i < 32; i++) sv[i] = __float_as_uint(__uint_as_float(sv[i]) + __uint_as_float(t1[i]));
-                tmem_ld32(sa + 2 * kLT, t1);
-                tmem_ld32(sa + 3 * kLT, t2);
-                tmem_wait_ld();
-#pragma unroll
-                for (int i = 0; i < 32; i++) sv[i] = __float_as_uint(__uint_as_float(sv[i]) + (__uint_as_float(t1[i]) + __uint_as_float(t2[i])));
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) bar_arrive(smem_u32(&misc.s_empty[buf]));
-            if (p.debug && j == 0 && !upper && split == 0 && hg == 0 && b == 0)
-                for (int i = 0; i < 32; i++) p.debug[head * 32 + i] = __uint_as_float(sv[i]);
-            const int t_base = (tile0 + j) * kLT + 16 * upper;
-            float x[16];
-            float mt = -INFINITY;
-#pragma unroll
-            for (int i = 0; i < 16; i++) {
-                const uint32_t hi = __shfl_sync(0xffffffffu, sv[16 + i], lane & 15);
-                const float v = __uint_as_float(upper ? hi : sv[i]);
-                x[i] = (t_base + i < L) ? v * p.scale_log2 : -INFINITY;
-                mt = fmaxf(mt, x[i]);
-            }
-            mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 16));
-            m_run = fmaxf(m_run, mt);
-            // does any head need its reference raised?  (never on the first tile: O^T is overwritten by the first PV)
-            bool need = false;
-            if (j == 0) m_ref = m_run;
-            else need = m_run - m_ref > kRescaleThreshold;
-            const unsigned any_w = __ballot_sync(0xffffffffu, need);
-            if (lane == 0) misc.need[buf][warp - 2] = any_w != 0;
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            const bool any = misc.need[buf][0] | misc.need[buf][1] | misc.need[buf][2] | misc.need[buf][3];
-            if (any) {
-                // O^T must be quiescent: the previous PV has to be complete (it also frees the other P buffer)
-                bar_wait(smem_u32(&misc.p_free[(j - 1) & 1]), ((j - 1) >> 1) & 1);
-                tc_fence_after();
-                const float a = need ? ex2(m_ref - m_run) : 1.f;
-                if (!upper) misc.alpha[head] = a;
-                if (need) { l *= a; m_ref = m_run; }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-#pragma unroll 1
-                for (int q = 0; q < 8; q++) {   // 4 latent blocks x 2 halves of the 64 head columns
-                    uint32_t ov[32];
-                    const uint32_t ta = tmem + lane_base + kColO + q * 32;
-                    tmem_ld32(ta, ov);
-                    tmem_wait_ld();
-#pragma unroll
-                    for (int i = 0; i < 32; i++) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * misc.alpha[(q & 1) * 32 + i]);
-                    tmem_st32(ta, ov);
-                }
-                tmem_wait_st();
-                tc_fence_before();
-                asm volatile("bar.sync 1, 128;" ::: "memory");   // alpha[] / need[] may be rewritten only after everyone used them
-            }
-            // this tile's P buffer was last read by PV(j - 2)
-            if (j >= 2) bar_wait(smem_u32(&misc.p_free[buf]), ((j >> 1) & 1) ^ 1);
-            {
-                float ps = 0.f;
-                uint32_t pk[8];
-#pragma unroll
-                for (int i = 0; i < 16; i += 2) {
-                    const float p0 = ex2(x[i] - m_ref), p1 = ex2(x[i + 1] - m_ref);
-                    ps += p0 + p1;
-                    pk[i >> 1] = pack_bf16(p0, p1);
-                }
-                l += ps;
-                // P[head][token] as the K-major no-swizzle B operand: core matrix (8 heads x 8 tokens) = 128 contiguous bytes
-                uint8_t* prow = smem + kOffP + buf * kPBytes + (head >> 3) * 512 + (head & 7) * 16 + upper * 256;
-                *reinterpret_cast<uint4*>(prow) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                *reinterpret_cast<uint4*>(prow + 128) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-            }
-            // rows of the tile beyond kv_len hold whatever the page contains: P is 0 there, but 0 * NaN is NaN -> zero the V rows
-            if ((tile0 + j) * kLT + kLT > L) {
-                const int valid = L - (tile0 + j) * kLT;
-                uint8_t* kb = smem + (j % kStages) * kStageBytes;
-                for (int i = st; i < (kLT - valid) * 64; i += 128) {      // 64 pieces of 16 B per row over the 8 latent chunks
-                    const int r = valid + i / 64, pc = i % 64;
-                    *reinterpret_cast<uint4*>(kb + (pc >> 3) * kKRegion + r * 128 + (pc & 7) * 16) = make_uint4(0, 0, 0, 0);
-                }
+        for (int i = 0; i < 16; i += 2) {
+            const int h = (i >> 1) & 1;
+            const float p0 = ex2(x[i] - m_ref[h]), p1 = ex2(x[i + 1] - m_ref[h]);
+            l[h] += p0 + p1;
+            pa[i >> 3][(i >> 1) & 3] = pack_bf16(p0, p1);
+        }
+        // rows of the tile beyond kv_len hold whatever the page contains: P is 0 there, but 0 * NaN is NaN -> zero the V rows
+        // of this warpgroup's latent half (the other half is only read by the other warpgroup, S never uses these rows)
+        if (t_base + kLT > L) {
+            const int valid = L - t_base;
+            uint8_t* kt = smem + s * kStageBytes + 4 * g * kKRegion;
+            for (int i = wt; i < (kLT - valid) * 32; i += 128) {      // 32 pieces of 16 B per row over the 4 latent chunks
+                const int r = valid + i / 32, pc = i % 32;
+                *reinterpret_cast<uint4*>(kt + (pc >> 3) * kKRegion + r * 128 + (pc & 7) * 16) = make_uint4(0, 0, 0, 0);
             }
             fence_async_smem();
-            __syncwarp();
-            if (lane == 0) bar_arrive(smem_u32(&misc.p_full));
-            if (p.debug && st == 0 && split == 0 && hg == 0 && b == 0 && j < 60) {
-                unsigned long long t;
-                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-                reinterpret_cast<unsigned long long*>(p.debug + 2048)[4 + j] = t;
-            }
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");
         }
-        // ---- epilogue: O^T / l -> fp32 partial output, base-2 LSE ---------------------------------------------------
-        l += __shfl_xor_sync(0xffffffffu, l, 16);
-        if (!upper) { misc.l[head] = l; misc.m[head] = m_ref; }
-        bar_wait(smem_u32(&misc.p_free[(n - 1) & 1]), ((n - 1) >> 1) & 1);   // the last PV (and with it every earlier one) is complete
-        tc_fence_after();
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (p.debug && st == 0 && split == 0 && hg == 0 && b == 0) {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-            reinterpret_cast<unsigned long long*>(p.debug + 2048)[2] = t;
-        }
-        if (st < kHG && h0 + st < p.num_heads) lse_out[st] = misc.m[st] + log2f(misc.l[st]);
-        if (st < kHG) misc.alpha[st] = 1.f / misc.l[st];
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-#pragma unroll 1
-        for (int half = 0; half < 2; half++) {
-            float inv[32];
+        fence();
 #pragma unroll
-            for (int i = 0; i < 32; i++) inv[i] = misc.alpha[half * 32 + i];
-            const int nh = min(32, p.num_heads - h0 - half * 32);   // valid heads of this half
-#pragma unroll 1
-            for (int blk = 0; blk < 4; blk++) {
-                uint32_t ov[32];
-                tmem_ld32(tmem + lane_base + kColO + blk * kHG + half * 32, ov);
-                tmem_wait_ld();
-                float* dst = o_out + (long)(half * 32) * kDV + blk * 128 + 32 * sp + lane;
-#pragma unroll
-                for (int i = 0; i < 32; i++)
-                    if (i < nh) dst[(long)i * kDV] = __uint_as_float(ov[i]) * inv[i];
-            }
-        }
-        tc_fence_before();
-        if (p.debug && st == 0 && split == 0 && hg == 0 && b == 0) {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-            reinterpret_cast<unsigned long long*>(p.debug + 2048)[3] = t;
-        }
+        for (int kk = 0; kk < 2; kk++)
+            mma_bf16_rs_m64n256_bt(o, pa[kk], smem_desc(kb + 4 * g * kKRegion + kk * 2048, kKRegion, 1024, kLayoutSw128), 1);
+        commit();
+        wait<0>();
+        fence_regs(o);
+        __syncwarp();
+        if (lane == 0) bar_arrive(smem_u32(&misc.k_empty[s]));
     }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem, kTmemCols);
+    // ---- epilogue: O / l -> fp32 partial output, base-2 LSE ---------------------------------------------------------
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+        l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+        const int r = ra + 8 * h;
+        if (h0 + r >= p.num_heads) continue;
+        if (g == 0 && (lane & 3) == 0) lse_out[r] = m_ref[h] + log2f(l[h]);
+        const float inv = 1.f / l[h];
+        float* dst = o_out + (long)r * kDV + 256 * g + cq;
+#pragma unroll
+        for (int jb = 0; jb < 32; jb++) *reinterpret_cast<float2*>(dst + 8 * jb) = make_float2(o[4 * jb + 2 * h] * inv, o[4 * jb + 2 * h + 1] * inv);
     }
 }
 
@@ -546,10 +404,7 @@ int ktb200_mla_decode(const ktb200_mla_params* q, void* stream) {
 }
 
 // Diagnostics: while set, CTA (split 0, head group 0, sequence 0) of ktb200_mla_decode writes the raw fp32 scores of its
-// first tile (S[64 heads][32 tokens], before scaling) to debug_dev[0..2048) and %globaltimer stamps (uint64) to
-// debug_dev + 2048: [0] kernel start, [1] setup done, [2] last PV complete, [3] epilogue stored, [4 + j] tile j's P ready
-// [64 + j] tile j's S seen
-// by the softmax warps, [128 + j] PV(j) issued, [192 + j] tile j's TMA issued (debug_dev must hold >= 2048 floats + 256 uint64).
+// first tile (S[64 heads][32 tokens], before scaling) to debug_dev[0..2048).
 void ktb200_debug_mla(float* debug_dev) { ktb::g_mla_debug = debug_dev; }
 
 int ktb200_mla_kv_write(void* kv_cache, int page_size, const void* ckv, const void* k_pe, const int* page_idx,

@@ -4,10 +4,10 @@
 // self.gate(x)` (models/modeling_deepseek_v3.py:430-481), `y = self.experts(x, topk_idx, topk_weight)` (the CPU MOE,
 // operators/llamafile/moe.cpp:146-245) and `y += self.shared_experts(identity)`.
 //
-// Why one kernel: a launch that streams ~100-150 MB lasts 25-30 us on a B200 of which ~6 us are fixed cost (launch
-// gap, pipeline ramp, activation prologue, tail) — profiles/probe_bulk.txt: the bare copy ring needs 27.3 us for the
-// gate/up bytes that take 21 us at the sustained rate.  Three launches per layer pay that three times.  Here the 148
-// CTAs (one per SM, cooperative launch, 12 warps, 168 registers) stay resident for the whole layer and separate the
+// Why one kernel: a launch that streams ~100-150 MB pays a fixed cost (launch gap, pipeline ramp, activation prologue,
+// tail) on top of the time its bytes take at the sustained rate (profiles/probe_bulk.py measures both for the bare copy
+// ring).  Three launches per layer pay that three times.  Here one CTA per SM (cooperative launch, 12 warps, 168
+// registers) stays resident for the whole layer and separates the
 // phases with two grid-wide barriers.  What overlaps what was decided with profiles/block_trace.py (%globaltimer at the
 // phase boundaries of every CTA):
 //   * a barrier is split into arrive / wait; weights that do not depend on the other CTAs are requested in between
@@ -1239,8 +1239,8 @@ extern "C" int ktb200_moe_ep_block_forward(const ktb200_gate_config* gc, ktb200_
 
 // Prefetch hint: while this handle's block kernel streams its down projection, pull up to three byte ranges into L2 — the
 // caller passes what the NEXT layer's launch reads first (its router weight, its shared expert's gate / up tensors).
-// Measured at DeepSeek-V3 shapes (profiles/r02_block_experiments.md): no gain while the down stream already saturates HBM
-// (the prefetch competes with it), so bench.py leaves it off; kept for callers whose next layer is not back to back.
+// While the down stream already saturates HBM the prefetch competes with it, so bench.py leaves it off (KTB200_BENCH_PREFETCH);
+// kept for callers whose next layer is not back to back.
 extern "C" int ktb200_moe_block_prefetch_hint(ktb200_moe* m, const void* const* ptrs, const size_t* bytes, int n) {
     if (!m || n < 0 || n > 3 || (n && (!ptrs || !bytes))) { set_error("prefetch_hint: up to 3 ranges"); return KTB200_EINVAL; }
     for (int r = 0; r < 3; r++) {
@@ -1280,5 +1280,5 @@ extern "C" int ktb200_moe_block_forward_host(const ktb200_gate_config* gc, ktb20
 }
 
 // Diagnostics (profiles/block_trace.py): when set, thread 0 of every CTA of the following ktb200_moe_block_forward
-// launches writes %globaltimer at the phase boundaries into trace[cta][16] (device memory, >= 148*16 u64).
+// launches writes %globaltimer at the phase boundaries into trace[cta][16] (device memory, >= num_SMs*16 u64).
 extern "C" void ktb200_debug_block_trace(unsigned long long* trace_dev) { g_btrace = trace_dev; }

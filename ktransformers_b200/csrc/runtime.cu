@@ -29,7 +29,7 @@ int num_sms(int device) {
     if (device < 0 || device >= 64) device = 0;
     if (!cached[device]) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || n <= 0) n = 132;
         cached[device] = n;
     }
     return cached[device];
@@ -39,7 +39,7 @@ int num_sms(int device) {
 
 extern "C" {
 const char* ktb200_last_error(void) { return ktb::g_err; }
-const char* ktb200_version(void) { return "ktb200 0.1 (sm_100a)"; }
+const char* ktb200_version(void) { return "ktb200 0.1 (sm_90a)"; }
 long ktb200_type_size(int t) { return ktb::type_size(t); }
 long ktb200_blck_size(int t) { return ktb::blck_size(t); }
 unsigned long long ktb200_launch_count(void) { return ktb::g_launches.load(); }

@@ -1,0 +1,145 @@
+// Hopper (sm_90a) tensor-path primitives as inline PTX: mbarrier, TMA tensor loads, shared-memory matrix descriptors and
+// warpgroup MMAs (wgmma.mma_async).  No CUTLASS: the descriptor bits are the documented format (PTX ISA "Matrix Descriptor
+// Format" for wgmma: start_address [0,14), leading_byte_offset [16,30), stride_byte_offset [32,46), base_offset [49,52),
+// layout_type [62,64)).  A wgmma is issued by all 128 threads of a warpgroup (4 consecutive warps, the first a multiple of 4);
+// the accumulator lives in their registers:  warp w of the group holds rows 16 w + lane / 4 and 16 w + lane / 4 + 8, and for
+// every 8 columns j registers [4 j, 4 j + 4) = (row, 8 j + 2 (lane % 4) + {0, 1}), (row + 8, the same two columns).
+#pragma once
+#include <cuda.h>   // CUtensorMap (types only: the driver entry point is resolved at run time, libcuda is not linked)
+#include <stdint.h>
+
+namespace ktb {
+namespace wg {
+
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// ---------------------------------------------------------------------------------------------- mbarrier
+__device__ __forceinline__ void bar_init(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void bar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void bar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ void bar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+// blocks until the phase with the given parity has completed (a fresh barrier passes parity 1 at once)
+__device__ __forceinline__ void bar_wait(uint32_t bar, uint32_t parity) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "WAIT_LOOP:\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+        "@p bra WAIT_DONE;\n"
+        "bra WAIT_LOOP;\n"
+        "WAIT_DONE:\n"
+        "}\n" ::"r"(bar), "r"(parity)
+        : "memory");
+}
+// generic-proxy writes to shared memory (st.shared) -> visible to the async proxy (TMA, wgmma operand reads)
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// ---------------------------------------------------------------------------------------------- TMA
+__device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
+}
+// 2-D tiled load: box (c0 .. c0+box0, c1 .. c1+box1) -> shared memory, completion (bytes) on `bar`
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
+                 "l"(m), "r"(bar), "r"(c0), "r"(c1)
+                 : "memory");
+}
+
+// ---------------------------------------------------------------------------------------------- descriptors
+enum : uint64_t { kLayoutNone = 0, kLayoutSw128 = 1, kLayoutSw64 = 2, kLayoutSw32 = 3 };
+
+// Shared-memory matrix descriptor.  `addr` is a shared::cta byte address (16-byte aligned, swizzled tiles 1024-byte
+// aligned), lbo / sbo in bytes.
+//   K-major,  swizzle 128B : rows of 128 B (64 bf16 / 128 8-bit values along K), 8-row groups `sbo` = 1024 B apart; lbo
+//                            unused; the k-th 32-byte step along K is addr + 32 k
+//   K-major,  no swizzle   : core matrix = 8 rows x 16 B contiguous; next core matrix along K at `lbo`, next 8 rows at `sbo`
+//   MN-major, swizzle 128B : 128 B (64 bf16) contiguous along MN, 8 K-rows per 1024-B atom; next MN atom at `lbo`,
+//                            next 8 K-rows at `sbo`
+__device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo, uint32_t sbo, uint64_t layout) {
+    return (uint64_t)((addr >> 4) & 0x3fffu) | ((uint64_t)((lbo >> 4) & 0x3fffu) << 16) | ((uint64_t)((sbo >> 4) & 0x3fffu) << 32) |
+           (layout << 62);
+}
+
+// ---------------------------------------------------------------------------------------------- wgmma
+// Order of use in a warpgroup: fence() -> mma_* ... -> commit() -> wait<N>() -> fence_regs(accumulator) before reading it.
+__device__ __forceinline__ void fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs that own the registers
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int N>
+__device__ __forceinline__ void fence_regs(uint32_t (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; i++) asm volatile("" : "+r"(d[i])::"memory");
+}
+
+// Per-thread register budget of the calling warpgroup (all of its warps execute it): a producer warpgroup gives registers
+// back so that the MMA warpgroups of the CTA can hold larger accumulators.
+template <int N>
+__device__ __forceinline__ void regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// D (+)= A . B; `accumulate` == 0 overwrites D.
+// fp32 += f16 (A: registers, accumulator-shaped fragment) . f16 (B: shared memory, K-major), 64 x 16 x 16
+__device__ __forceinline__ void mma_f16_rs_m64n16(float (&d)[8], const uint32_t (&a)[4], uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));
+}
+// fp32 += bf16 . bf16, A and B K-major from shared memory, 64 x 32 x 16
+__device__ __forceinline__ void mma_bf16_m64n32(float (&d)[16], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+// fp32 += f16 . f16, A and B K-major from shared memory, 64 x 32 x 16
+__device__ __forceinline__ void mma_f16_m64n32(float (&d)[16], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+// s32 += u8 . s8, K-major, 64 x 32 x 32
+__device__ __forceinline__ void mma_u8s8_m64n32(uint32_t (&d)[16], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+// s32 += s8 . s8, K-major, 64 x 64 x 32
+__device__ __forceinline__ void mma_s8s8_m64n64(uint32_t (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+// fp32 += bf16 (A: registers, accumulator-shaped fragment) . bf16 (B: shared memory, MN-major), 64 x 256 x 16
+__device__ __forceinline__ void mma_bf16_rs_m64n256_bt(float (&d)[128], const uint32_t (&a)[4], uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %133, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, {%128, %129, %130, %131}, %132, p, 1, 1, 1;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));
+}
+
+}  // namespace wg
+}  // namespace ktb

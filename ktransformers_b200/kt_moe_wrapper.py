@@ -1,4 +1,4 @@
-"""`KTMoEWrapper` front door for the B200 experts (SURVEY §8f rank 1).
+"""`KTMoEWrapper` front door for the H100 experts (SURVEY §8f rank 1).
 
 API mirror of kt-kernel's factory (kt-kernel/python/experts.py:72-262) and its inference base class
 (kt-kernel/python/experts_base.py:227-544): same constructor arguments, `load_weights(physical_to_logical_map_cpu)`,
@@ -6,7 +6,7 @@ API mirror of kt-kernel's factory (kt-kernel/python/experts.py:72-262) and its i
 cuda_stream)`, the capture-batch-size helpers.  What changes underneath:
 
   * `method="B200_GGUF"`: the layer's GGUF expert tensors (`blk.L.ffn_{gate,up,down}_exps.weight`, any K-quant the
-    sm_100a kernels take) are uploaded as raw blocks and consumed on the GPU through the C-ABI (`ktb200_moe_*`);
+    sm_90a kernels take) are uploaded as raw blocks and consumed on the GPU through the C-ABI (`ktb200_moe_*`);
     there is no CPU worker pool, so `cpuinfer_threads`, `threadpool_count`, `numa_nodes`, `cpu_save` are accepted and
     ignored, and `submit_forward` launches on `cuda_stream` while `sync_forward` only hands back the (stream-ordered)
     output buffer — the two names keep their meaning for callers such as SGLang's KTEPWrapperMethod.
@@ -42,11 +42,11 @@ class KTMoEWrapper:
                  numa_nodes: Optional[List[int]] = None, mode: str = "inference", device: str = "cuda",
                  key_template: str = "model.layers.{layer}.mlp.experts", dtype: torch.dtype = torch.bfloat16, **kwargs):
         if mode != "inference":
-            raise NotImplementedError("KTMoEWrapper (B200): only mode='inference' (SFT is out of scope, DESIGN.md §6)")
+            raise NotImplementedError("KTMoEWrapper (H100): only mode='inference' (SFT is out of scope, DESIGN.md §6)")
         if method not in B200_METHODS:
             raise NotImplementedError(f"Unsupported method: {method}. Supported methods: {sorted(B200_METHODS)}")
         if max_deferred_experts_per_token:
-            raise ValueError("deferred experts overlap a CPU backend with the GPU; the B200 backend has nothing to defer")
+            raise ValueError("deferred experts overlap a CPU backend with the GPU; the H100 backend has nothing to defer")
         if num_experts <= 0 or num_experts_per_tok <= 0 or num_experts_per_tok > num_experts:
             raise ValueError("num_experts / num_experts_per_tok out of range")
         self.layer_idx, self.num_experts, self.num_experts_per_tok = layer_idx, num_experts, num_experts_per_tok
@@ -97,7 +97,7 @@ class KTMoEWrapper:
     def _load(self, raw, types, p2l):
         for t in types.values():
             if GGML_NAMES.get(t) not in B200_WEIGHT_TYPES:
-                raise ValueError(f"ggml type {GGML_NAMES.get(t, t)} is not supported by the sm_100a kernels")
+                raise ValueError(f"ggml type {GGML_NAMES.get(t, t)} is not supported by the sm_90a kernels")
         w = {n: self._permute(raw[n], self.num_experts, p2l) for n in ("gate", "up", "down")}
         w.update(gate_type=types["gate"], up_type=types["up"], down_type=types["down"])
         self.moe.load(w, device=self.device)

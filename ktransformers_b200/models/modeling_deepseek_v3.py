@@ -1,4 +1,4 @@
-"""Minimal DeepSeek-V3 MoE block definitions — the injection targets of the B200 rule files.
+"""Minimal DeepSeek-V3 MoE block definitions — the injection targets of the H100 rule files.
 
 Only the classes the hot path's YAML rules match against are defined here (the reference carries the
 whole HF model, archive/ktransformers/models/modeling_deepseek_v3.py; everything outside the MoE block

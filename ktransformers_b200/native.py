@@ -116,7 +116,7 @@ class EpComm(C.Structure):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile libktb200.so for sm_100a with nvcc (cross-compiles without a GPU)."""
+    """Compile libktb200.so for sm_90a with nvcc (cross-compiles without a GPU)."""
     out = None if verbose else subprocess.DEVNULL
     subprocess.check_call(["make", "-C", CSRC, "-j", "4"], stdout=out)
     return LIB_PATH
@@ -130,7 +130,7 @@ def lib() -> C.CDLL:
             if _lib is None:
                 if not os.path.exists(LIB_PATH):
                     raise RuntimeError(
-                        f"{LIB_PATH} is missing: the B200 path has no CPU fallback. Build it with "
+                        f"{LIB_PATH} is missing: the H100 path has no CPU fallback. Build it with "
                         "`python -c 'import __graft_entry__ as g; g.build()'` or `make -C ktransformers_b200/csrc`.")
                 l = C.CDLL(LIB_PATH)
                 for name, (res, args) in SYMBOLS.items():

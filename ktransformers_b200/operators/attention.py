@@ -2,8 +2,8 @@
 
 Mirrors archive/ktransformers/operators/attention.py:49-75 (`get_absorbed`) and :349-478 (`forward_linux_flashinfer`,
 decode branch): q projections -> RoPE -> paged latent-cache update -> q_nope . W_UK (batched matmul) -> MLA paged decode
-over the 576-wide latents -> . W_UV^T -> o_proj.  The attention itself is `MLAWrapper.run` = ktb200_mla_decode (tcgen05 +
-TMEM + TMA, csrc/mla.cu); the cache write is ktb200_mla_kv_write; the projections are whatever modules the rules injected
+over the 576-wide latents -> . W_UV^T -> o_proj.  The attention itself is `MLAWrapper.run` = ktb200_mla_decode (wgmma +
+TMA, csrc/mla.cu); the cache write is ktb200_mla_kv_write; the projections are whatever modules the rules injected
 (KLinearB200 on raw GGUF blocks, or nn.Linear); the two absorb products are ktb200_mla_absorb_q / _o (HBM-bound batched
 GEMVs over the bf16 halves of kv_b_proj; torch.matmul for other dtypes).  Prefill (q_len > 1 without absorb) is outside this path and raises."""
 from __future__ import annotations
@@ -40,7 +40,7 @@ class KDeepseekV2Attention(BaseInjectedModule, DeepseekV3Attention):
                 use_cache: bool = False, cache_position: Optional[torch.Tensor] = None, **kwargs):
         bsz, q_len, _ = hidden_states.size()
         if q_len != 1 and not self.absorb_for_prefill:
-            raise NotImplementedError("KDeepseekV2Attention: the B200 path covers absorbed decode (q_len == 1)")
+            raise NotImplementedError("KDeepseekV2Attention: the H100 path covers absorbed decode (q_len == 1)")
         assert past_key_value is not None, "decode needs the paged latent cache (models/custom_cache.StaticCache)"
         q = self.q_proj(hidden_states) if self.q_lora_rank is None else self.q_b_proj(self.q_a_layernorm(self.q_a_proj(hidden_states)))
         q = q.view(bsz, q_len, self.num_heads, self.q_head_dim)

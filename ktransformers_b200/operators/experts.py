@@ -2,7 +2,7 @@
 
     KExpertsBase          :68-140    ctor/load/unload/forward/load_weights contract
     KExpertsB200          replaces KExpertsCPU (:143-435) / KExpertsMarlin (:437-559): the raw GGUF expert
-                          blocks live in HBM and are consumed by the sm_100a kernels through the C-ABI
+                          blocks live in HBM and are consumed by the sm_90a kernels through the C-ABI
                           (include/ktb200.h: ktb200_moe_*).  No CPU hand-off: submit_for_one_decode /
                           sync_for_one_decode keep their names and stream-ordered semantics (:293-318) but
                           launch the kernels directly on torch's current stream.
@@ -77,7 +77,7 @@ class KExpertsBase(ABC):
 
 
 class KExpertsB200(KExpertsBase):
-    """GPU-resident GGUF experts on the hand-written sm_100a kernels."""
+    """GPU-resident GGUF experts on the hand-written sm_90a kernels."""
 
     # graph-safe output buffers per device, like KExpertsCPU.output_gpu_map (experts.py:147)
     output_gpu_map: dict = {}
@@ -110,7 +110,7 @@ class KExpertsB200(KExpertsBase):
         self.gate_type, self.up_type, self.down_type = int(w["gate_type"]), int(w["up_type"]), int(w["down_type"])
         for t in (self.gate_type, self.up_type, self.down_type):
             if GGML_NAMES.get(t) not in B200_WEIGHT_TYPES:
-                raise ValueError(f"KExpertsB200: ggml type {GGML_NAMES.get(t, t)} is not supported by the sm_100a kernels")
+                raise ValueError(f"KExpertsB200: ggml type {GGML_NAMES.get(t, t)} is not supported by the sm_90a kernels")
         E = self.n_routed_experts
         per, lo = E // self.ep_size, (E // self.ep_size) * self.ep_rank
 

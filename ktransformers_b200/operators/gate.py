@@ -2,7 +2,7 @@
 
     KMoEGateBase  :23-89   load_weights(weight, e_score_correction_bias) contract
     KMoEGate      :91-127  the reference delegates to the torch MoEGate.forward (≈10 ATen kernels)
-    KMoEGateB200  the same routing as two sm_100a kernels (ktb200_moe_gate_forward): fp32 GEMV +
+    KMoEGateB200  the same routing as two sm_90a kernels (ktb200_moe_gate_forward): fp32 GEMV +
                   warp-shuffle grouped top-k; ids are bit-exact vs torch up to fp32 summation-order ties.
 """
 from __future__ import annotations

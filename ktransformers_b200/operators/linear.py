@@ -2,7 +2,7 @@
 
     KLinearBase          :57-155   ctor / load_weight / load / unload contract
     KLinearB200          replaces KLinearMarlin (:595-721): the raw GGUF blocks stay in HBM and are
-                         consumed directly by the sm_100a integer GEMV (no dequant -> 4-bit g64
+                         consumed directly by the sm_90a integer GEMV (no dequant -> 4-bit g64
                          re-quantisation, linear.py:664-666); arithmetic equals the reference's CPU
                          Linear (operators/llamafile/linear.cpp:37-63).
     KLinearTorch         :158-216  dequantised weight + torch matmul
@@ -131,7 +131,7 @@ class KLinearB200(KLinearBase):
                 self.bias = w[2].to(device=device, dtype=torch.float32).contiguous()
                 self.has_bias = True
         if GGML_NAMES.get(ggml_type) not in B200_WEIGHT_TYPES:
-            raise ValueError(f"KLinearB200: ggml type {GGML_NAMES.get(ggml_type, ggml_type)} is not supported by the sm_100a kernels")
+            raise ValueError(f"KLinearB200: ggml type {GGML_NAMES.get(ggml_type, ggml_type)} is not supported by the sm_90a kernels")
         raw = raw if isinstance(raw, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(np.asarray(raw)).view(np.uint8).reshape(-1))
         self.weight = raw.reshape(-1).to(device).contiguous()
         self.ggml_type = ggml_type
@@ -175,7 +175,7 @@ class KLinearFP8(KLinearBase):
     """DeepSeek-V3's native FP8 checkpoints: e4m3 weight [out][in] + fp32 `weight_scale_inv` per 128 x 128 block, activations
     quantised per token and 128 values inside the kernel.  Same contract as the reference's KLinearFP8 (operators/linear.py:388-435:
     `load(w=(weight, weight_scale_inv))`, `forward(x, bsz_tensor)`), which runs Triton's act_quant + fp8_gemm; here one launch of
-    `ktb200_fp8_linear_forward` (TMA -> tcgen05.mma.kind::f8f6f4 -> TMEM, csrc/fp8_linear.cu)."""
+    `ktb200_fp8_linear_forward` (TMA -> e4m3 widened to fp16 in registers -> fp16 wgmma, csrc/fp8_linear.cu)."""
 
     def __init__(self, key, gguf_loader, config, orig_module=None, device: str = "cuda", block_size: int = 128, **kwargs):
         super().__init__(key, gguf_loader, config, orig_module, device, **kwargs)

@@ -63,7 +63,7 @@ GGML_TYPES = {t.name: int(t) for t in GGMLQuantizationType}
 GGML_ELEMENTS_PER_BLOCK = {t.name: GGML_QUANT_SIZES[t][0] for t in GGML_QUANT_SIZES}
 GGML_BLOCK_SIZES = {t.name: GGML_QUANT_SIZES[t][1] for t in GGML_QUANT_SIZES}
 
-# types the sm_100a kernels consume / dequantise directly
+# types the sm_90a kernels consume / dequantise directly
 B200_WEIGHT_TYPES = {"Q2_K", "Q3_K", "Q4_K", "Q5_K", "Q6_K", "IQ4_XS"}
 B200_DEQUANT_TYPES = B200_WEIGHT_TYPES | {"Q8_0", "F32", "F16", "BF16"}
 

@@ -149,7 +149,7 @@ class GGUFLoader(ModelLoader):
         ggml_name = GGML_NAMES[ggml_type]
         if "cuda" in str(device).lower():
             if ggml_name not in B200_DEQUANT_TYPES:
-                raise NotImplementedError(f"ggml_type {ggml_name} has no sm_100a dequantiser")
+                raise NotImplementedError(f"ggml_type {ggml_name} has no sm_90a dequantiser")
             from .. import native
             out_dtype = target_dtype if target_dtype in _TORCH_TO_GGML_OUT else torch.float32
             raw = torch.from_numpy(np.ascontiguousarray(data).view(np.uint8)).to(device)

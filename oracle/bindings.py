@@ -156,7 +156,7 @@ class Ref(_Common):
     def __init__(self):
         path = ref_library_path()
         if path is None:
-            raise RuntimeError("oracle/_ref is not built (run `make -C oracle ref` where /root/reference exists)")
+            raise RuntimeError("oracle/_ref is not built (run `make -C oracle ref` with REF pointing at the reference sources, see oracle/Makefile)")
         self.path = path
         self.lib = C.CDLL(path)
         for n in ("type_size", "blck_size"):
@@ -240,7 +240,7 @@ def f32_to_bf16_bits(x: np.ndarray) -> np.ndarray:
 
 
 class AmxRef:
-    """The reference's AMX MoE backend (kt_kernel_ext.moe.AMXInt4_MOE) compiled UNMODIFIED from /root/reference through the
+    """The reference's AMX MoE backend (kt_kernel_ext.moe.AMXInt4_MOE) compiled UNMODIFIED from the reference sources (REF in oracle/Makefile) through the
     single-node numa/hwloc shim (oracle/amx_shim.cpp, oracle/amx_shim/*.h): the "CPU-AMX" baseline of BASELINE.json.
     A SHIMMED build; runs only on hosts whose /proc/cpuinfo shows amx_tile + amx_int8."""
 
@@ -257,7 +257,7 @@ class AmxRef:
     @classmethod
     def why_unavailable(cls) -> str:
         if not os.path.exists(cls.path()):
-            return "oracle/_ref/libktamx.so not built (needs /root/reference)"
+            return "oracle/_ref/libktamx.so not built (needs the reference sources, see REF in oracle/Makefile)"
         return "host CPU has no AMX (amx_tile / amx_int8 / amx_bf16 absent from /proc/cpuinfo)"
 
     @classmethod

@@ -10,7 +10,7 @@ for _p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100: pytest -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -37,10 +37,3 @@ def oracle():
     from oracle.bindings import Oracle
     return Oracle()
 
-
-@pytest.fixture(scope="session")
-def ref():
-    from oracle.bindings import Ref
-    if not Ref.available():
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
-    return Ref.get(min(os.cpu_count() or 1, 16))

@@ -5,8 +5,9 @@ reference's Python.  Run in the build container only:
     make -C oracle ref && python tests/golden/make_golden.py
 
 Outputs (small, committed):
-    moe_small.npz        E=4 k=2 H=512 I=256, Q4_K/Q4_K/Q6_K + a Q5_K/Q5_K/Q4_K variant: quantised weights
-                         (reference from_float), inputs, MOE::forward outputs for qlen 1,3,12 (fp32 and bf16)
+    moe_small_{a,b}.npz  E=4 k=2 H=512 I=256, Q4_K/Q4_K/Q6_K (a) and Q5_K/Q5_K/Q4_K (b): quantised weights (reference
+                         from_float), inputs, MOE::forward outputs for qlen 1,3,12 (fp32 and bf16); stored for the 3 experts
+                         that keep the most tokens and the tokens routed only to them (sample_moe_case)
     act_quant.npz        Q8_K / Q8_0 activation blocks for fp32 and bf16-valued rows (tie-heavy)
     dequant.npz          16 blocks per weight type: raw bytes + to_float values
     linear_mlp.npz       Linear / MLP forward outputs
@@ -48,10 +49,33 @@ def moe_case(rng, E, k, H, I, gt, ut, dt, qlens):
     return out
 
 
+def sample_moe_case(c, keep=3):
+    """Keeps `keep` of the case's experts (the subset that keeps the most tokens) and the tokens routed only to them, ids
+    renumbered: a token's output depends on its own experts alone, and the weights of all experts would not fit 1 MB."""
+    import itertools
+    E, qls = int(c["E"]), [int(k[2:]) for k in c if k.startswith("x_")]
+    sub = max(itertools.combinations(range(E), keep), key=lambda s: (sum(int(np.isin(c[f"ids_{q}"], s).all(1).sum()) for q in qls),
+                                                                    min(int(np.isin(c[f"ids_{q}"], s).all(1).sum()) for q in qls)))
+    out = {k: v for k, v in c.items() if k in ("k", "H", "I", "gate_type", "up_type", "down_type")}
+    out["E"] = np.int64(keep)
+    for w in ("gate", "up", "down"):
+        per = np.asarray(c[w]).reshape(E, -1)
+        out[w] = np.ascontiguousarray(per[list(sub)]).reshape(-1)
+    remap = np.full(E, -1, np.int64)
+    remap[list(sub)] = np.arange(keep)
+    for q in qls:
+        sel = np.isin(c[f"ids_{q}"], sub).all(1)
+        for n in ("x", "w", "out_f32", "out_bf16"):
+            out[f"{n}_{q}"] = np.asarray(c[f"{n}_{q}"])[sel]
+        out[f"ids_{q}"] = remap[np.asarray(c[f"ids_{q}"])[sel]]
+    return out
+
+
 rng = np.random.default_rng(20260922)
 a = moe_case(rng, 4, 2, 512, 256, Q4_K, Q4_K, Q6_K, (1, 3, 12))
 b = moe_case(rng, 4, 2, 512, 256, Q5_K, Q5_K, Q4_K, (1, 12))
-np.savez_compressed(os.path.join(OUT, "moe_small.npz"), **{f"a_{k}": v for k, v in a.items()}, **{f"b_{k}": v for k, v in b.items()})
+for name, c in (("a", a), ("b", b)):
+    np.savez_compressed(os.path.join(OUT, f"moe_small_{name}.npz"), **{f"{name}_{k}": v for k, v in sample_moe_case(c).items()})
 
 # activation quantisation
 rows = []

@@ -1,5 +1,5 @@
 """GPU tests of the Python operator layer (the reference-facing injection API) on a tiny GGUF file:
-`optimize_and_load_gguf` with the shipped B200 rule file -> KDeepseekV3MoE / KTransformersExperts(KExpertsB200) /
+`optimize_and_load_gguf` with the shipped H100 rule file -> KDeepseekV3MoE / KTransformersExperts(KExpertsB200) /
 KMoEGateB200 / KTransformersLinear(KLinearB200), decode through the single-launch block call and through the
 three-step path (reference control flow, experts.py:972-1012), both against a dense fp32 restatement."""
 import os
@@ -186,7 +186,7 @@ def test_pybind_extension_runs_the_reference_submit_sync_sequence(oracle):
 @pytest.mark.parametrize("heads,bsz", [(16, 1), (128, 2)])
 def test_kdeepseek_v2_attention_absorbed_paged_decode_matches_plain_attention(heads, bsz):
     """KDeepseekV2Attention (operators/attention.py; reference attention.py:349-478): q/kv projections, RoPE, paged latent
-    cache write (ktb200_mla_kv_write), W_UK absorb, ktb200_mla_decode (tcgen05), W_UV, o_proj — token by token against the
+    cache write (ktb200_mla_kv_write), W_UK absorb, ktb200_mla_decode (wgmma), W_UV, o_proj — token by token against the
     plain non-absorbed attention of the same module (fp32 softmax over explicit latents)."""
     from ktransformers_b200.models.custom_cache import StaticCache
     from ktransformers_b200.models.modeling_deepseek_v3 import DeepseekV3Attention, DeepseekV3Config

@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol():
     assert lib.ktb200_type_size(12) == 144 and lib.ktb200_blck_size(12) == 256
     assert lib.ktb200_type_size(14) == 210 and lib.ktb200_type_size(15) == 292
     assert lib.ktb200_type_size(99) == 0
-    assert b"sm_100a" in lib.ktb200_version()
+    assert b"sm_90a" in lib.ktb200_version()
 
 
 def test_missing_library_fails_loudly(monkeypatch):
@@ -233,7 +233,7 @@ def test_b200_ops_are_registered_and_refuse_cpu():
 
 
 def test_kt_moe_wrapper_front_door_contract():
-    """KTMoEWrapper (kt-kernel/python/experts.py:72-262) for the B200 backend: constructor checks, mask handling and the
+    """KTMoEWrapper (kt-kernel/python/experts.py:72-262) for the H100 backend: constructor checks, mask handling and the
     EPLB permutation are host logic; the compute goes through KExpertsB200 (GPU tests)."""
     from ktransformers_b200.kt_moe_wrapper import KTMoEWrapper
     with pytest.raises(NotImplementedError):
@@ -287,7 +287,7 @@ def test_pybind_module_exposes_the_reference_extension_surface():
     import sys
     sys.path.insert(0, os.path.join(ROOT, "ktransformers_b200"))
     ext = importlib.import_module("kt_kernel_ext_b200")
-    assert "sm_100a" in ext.version()
+    assert "sm_90a" in ext.version()
     cfg = ext.moe.MOEConfig(8, 2, 512, 256)
     for f in ("expert_num", "num_experts_per_tok", "hidden_size", "intermediate_size", "layer_idx", "max_len", "group_min_len",
               "group_max_len", "gate_type", "up_type", "down_type", "hidden_type", "gate_proj", "up_proj", "down_proj",

@@ -1,6 +1,5 @@
 """CPU: pins the oracle (oracle/ktoracle.c, oracle/gate_oracle.py) against the committed golden vectors that
-were generated from the unmodified reference, and — where oracle/_ref is present — against the reference
-itself on fresh random inputs."""
+were generated from the unmodified reference."""
 import json
 import os
 
@@ -40,7 +39,7 @@ def test_dequantisation_matches_reference(oracle, golden_dir):
 
 @pytest.mark.parametrize("case", ["a", "b"])
 def test_moe_forward_matches_golden(oracle, golden_dir, case):
-    g = np.load(os.path.join(golden_dir, "moe_small.npz"))
+    g = np.load(os.path.join(golden_dir, f"moe_small_{case}.npz"))
     E, k, H, I = (int(g[f"{case}_{n}"]) for n in ("E", "k", "H", "I"))
     gt, ut, dt = (int(g[f"{case}_{n}"]) for n in ("gate_type", "up_type", "down_type"))
     for qlen in (1, 3, 12):
@@ -89,33 +88,46 @@ def test_name_translation_matches_reference(golden_dir):
         assert translate_name_to_gguf(src) == dst, src
 
 
-# ---- live checks against the compiled reference (build container / any box that has oracle/_ref) ------------
+# ---- the oracle's dot products and MoE against the reference's own quantised data and outputs ----------------
 @pytest.mark.parametrize("wtype", [Q2_K, Q3_K, Q4_K, Q5_K, Q6_K, IQ4_XS, Q8_0])
-def test_vec_dot_against_ref(oracle, ref, wtype):
-    rng = np.random.default_rng(wtype)
-    n = 256 * 12
-    wq = ref.from_float(rng.standard_normal(n).astype(np.float32), wtype)
-    x = (rng.standard_normal(n) / 7).astype(np.float32)
+def test_vec_dot_against_ref(oracle, golden_dir, wtype):
+    """Weights the reference quantised (dequant.npz raw_*) against activation rows the reference quantised (act_quant.npz):
+    the oracle's activation quantiser must reproduce the reference's bytes, its dequantiser the reference's values, and its
+    integer dot must equal the dot of the reference's dequantised weights and activations up to fp32 rounding."""
+    dq, aq = np.load(os.path.join(golden_dir, "dequant.npz")), np.load(os.path.join(golden_dir, "act_quant.npz"))
+    name = TYPE_NAMES[wtype]
+    wq, wval = dq[f"raw_{name}"], dq[f"val_{name}"].astype(np.float64)
+    n = wval.size
+    rows = n // aq["x"].shape[1]
+    x = aq["x"][:rows].reshape(-1)
     vdt = Q8_0 if wtype == Q8_0 else Q8_K
-    xq = ref.from_float(x, vdt)
+    xq = np.ascontiguousarray(aq["q8_0" if wtype == Q8_0 else "q8k"][:rows]).reshape(-1)
     assert np.array_equal(oracle.from_float(x, vdt), xq)
-    a, b = oracle.vec_dot(wtype, n, wq, xq), ref.vec_dot(wtype, n, wq, xq)
+    # the reference's activation blocks, dequantised: Q8_K = f32 d | 256 int8 | 16 int16 sums, Q8_0 = f16 d | 32 int8
+    if vdt == Q8_K:
+        blk = xq.reshape(-1, 292)
+        xv = blk[:, :4].copy().view(np.float32).astype(np.float64) * blk[:, 4:260].view(np.int8).astype(np.float64)
+    else:
+        blk = xq.reshape(-1, 34)
+        xv = blk[:, :2].copy().view(np.float16).astype(np.float64) * blk[:, 2:].view(np.int8).astype(np.float64)
+    a, b = oracle.vec_dot(wtype, n, wq, xq), float(np.dot(wval, xv.reshape(-1)))
     assert abs(a - b) <= 2e-5 * max(abs(b), 1.0)
-    np.testing.assert_allclose(oracle.to_float(wq, wtype, n), ref.to_float(wq, wtype, n), rtol=0, atol=1e-6)
+    np.testing.assert_allclose(oracle.to_float(wq, wtype, n), dq[f"val_{name}"], rtol=0, atol=1e-6)
 
 
 @pytest.mark.parametrize("qlen", [1, 5, 24])
-def test_moe_against_ref_fresh(oracle, ref, qlen):
-    rng = np.random.default_rng(100 + qlen)
-    E, k, H, I = 8, 4, 1024, 512
-    gq = ref.from_float(rng.standard_normal((E, I, H)).astype(np.float32), Q4_K)
-    uq = ref.from_float(rng.standard_normal((E, I, H)).astype(np.float32), Q4_K)
-    dq = ref.from_float(rng.standard_normal((E, H, I)).astype(np.float32), Q6_K)
-    x = f32_to_bf16_bits((rng.standard_normal((qlen, H)) / 100).astype(np.float32))
-    ids = np.stack([rng.permutation(E)[:k] for _ in range(qlen)]).astype(np.int64)
-    w = rng.random((qlen, k)).astype(np.float32)
-    a = bf16_to_f32(oracle.moe_forward(E, H, I, gq, uq, dq, Q4_K, Q4_K, Q6_K, BF16, ids, w, x))
-    b = bf16_to_f32(ref.moe_forward(E, H, I, gq, uq, dq, Q4_K, Q4_K, Q6_K, BF16, ids, w, x))
+def test_moe_against_ref_fresh(oracle, golden_dir, qlen):
+    """The oracle's MoE (bf16 hidden) against the reference's MOE::forward outputs (moe_small_a.npz: weights the reference
+    quantised, Q4_K / Q4_K / Q6_K).  A token's output depends on its own experts alone, so batches of any length are drawn
+    from the stored tokens."""
+    g = np.load(os.path.join(golden_dir, "moe_small_a.npz"))
+    E, k, H, I = (int(g[f"a_{n}"]) for n in ("E", "k", "H", "I"))
+    qls = sorted(int(n[len("a_x_"):]) for n in g.files if n.startswith("a_x_"))
+    x, ids, w, want = (np.concatenate([g[f"a_{n}_{q}"] for q in qls]) for n in ("x", "ids", "w", "out_bf16"))
+    rep = np.arange(qlen) % len(x)
+    a = bf16_to_f32(oracle.moe_forward(E, H, I, g["a_gate"], g["a_up"], g["a_down"], Q4_K, Q4_K, Q6_K, BF16, ids[rep], w[rep],
+                                       f32_to_bf16_bits(x[rep])))
+    b = bf16_to_f32(want[rep])
     # a one-LSB flip of an int8 activation (knife-edge rounding under fp32 re-association) moves outputs by
     # up to ~2e-3 of the row norm; anything larger is a real divergence
     # ... on top of the 1-ulp (2^-8 relative) granularity of the bf16 output itself

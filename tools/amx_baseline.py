@@ -1,5 +1,5 @@
 """Times the reference's AMX INT4 MoE (shimmed build, oracle/_ref/libktamx.so) at DeepSeek-V3 expert shapes on THIS host:
-8-of-N resident experts per layer-forward, one token, thread ladder.  Prints one JSON object (committed under profiles/)."""
+8-of-N resident experts per layer-forward, one token, thread ladder.  Prints one JSON object."""
 import json
 import os
 import sys

@@ -36,7 +36,7 @@ if os.environ.get("TRACE"):
     t = tr.cpu().numpy().reshape(2, 3, 96, 4)
     for kname, kk in (("gate (Q4_K)", 0), ("down (Q6_K)", 1)):
         t0 = t[kk, 0, 0, 0]
-        print(f"--- {kname}: cycles since the producer's first stage; P = wait_group done / smem_free seen / arrived, M = ab_full seen / tmem_free seen / committed, E = tmem_full seen / arrived")
+        print(f"--- {kname}: cycles since the producer's first stage; P = wait_group done / smem_free seen / arrived, M = before ab_full / ab_full seen / MMAs + scale-and-add done / arrived")
         for st in range(0, 40):
-            P, M, E = t[kk, 0, st] - t0, t[kk, 1, st] - t0, t[kk, 2, st] - t0
-            print(f"st {st:2d}  P {P[0]:6d} {P[1]:6d} {P[2]:6d} {P[3]:6d} | M {M[0]:6d} {M[1]:6d} {M[2]:6d} {M[3]:6d} | E {E[0]:6d} {E[1]:6d} {E[3]:6d}")
+            P, M = t[kk, 0, st] - t0, t[kk, 1, st] - t0
+            print(f"st {st:2d}  P {P[0]:6d} {P[1]:6d} {P[2]:6d} {P[3]:6d} | M {M[0]:6d} {M[1]:6d} {M[2]:6d} {M[3]:6d}")

@@ -1,4 +1,4 @@
-"""GPU probe for ktb200_mla_decode (tcgen05 path): stage-by-stage numerics (raw scores of the first tile through
+"""GPU probe for ktb200_mla_decode (wgmma path): stage-by-stage numerics (raw scores of the first tile through
 ktb200_debug_mla, then output / LSE against the numpy oracle) and timing over context lengths.
     python tools/mla_probe.py [--time]
 """
@@ -49,13 +49,6 @@ def numerics():
         mag = np.abs(want).max()
         print(f"B={B} Hq={Hq} page={page} lens={lens} splits={splits}: S err {np.abs(s_got - s_ref).max():.3e} (|S| {np.abs(s_ref).max():.2f}) "
               f"out err {np.abs(out - want).max() / mag:.3e} lse err {np.abs(lse - want_lse).max():.3e} finite={np.isfinite(out).all()}", flush=True)
-        ts = dbg.cpu().numpy()[2048:2048 + 512].view(np.uint64)
-        if ts[0]:
-            tl = [(int(t) - int(ts[0])) / 1e3 for t in ts[1:4]]
-            tiles = [(int(t) - int(ts[0])) / 1e3 for t in ts[4:64] if t]
-            print(f"   timeline us (CTA 0): setup {tl[0]:.1f} | last PV done {tl[1]:.1f} | stored {tl[2]:.1f} | P ready per tile: {[round(v, 1) for v in tiles[:16]]}", flush=True)
-            for nm, o in (("S seen", 64), ("PV issued", 128), ("TMA issued", 192)):
-                print(f"      {nm}: {[round((int(t) - int(ts[0])) / 1e3, 1) for t in ts[o:o + 16] if t]}", flush=True)
         if np.abs(s_got - s_ref).max() > 1e-2 * np.abs(s_ref).max():
             bad = np.argwhere(np.abs(s_got - s_ref) > 1e-2 * np.abs(s_ref).max())
             print("   first bad S entries (head, token):", bad[:8].tolist(), "got", s_got[tuple(bad[0])], "want", s_ref[tuple(bad[0])])
