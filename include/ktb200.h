@@ -35,7 +35,15 @@ extern "C" {
 enum ktb200_ggml_type {
     KTB200_TYPE_F32 = 0, KTB200_TYPE_F16 = 1, KTB200_TYPE_Q8_0 = 8, KTB200_TYPE_Q2_K = 10,
     KTB200_TYPE_Q3_K = 11, KTB200_TYPE_Q4_K = 12, KTB200_TYPE_Q5_K = 13, KTB200_TYPE_Q6_K = 14,
-    KTB200_TYPE_Q8_K = 15, KTB200_TYPE_IQ4_XS = 23, KTB200_TYPE_BF16 = 30
+    KTB200_TYPE_Q8_K = 15, KTB200_TYPE_IQ4_XS = 23, KTB200_TYPE_BF16 = 30,
+    /* Not a ggml type: ggml's ids stay below 64, so 256 cannot collide with one.
+     * Symmetric INT4 in groups of 32 with bf16 scales (compressed-tensors "pack-quantized", kt-kernel's RAWINT4; Kimi-K2's
+     * routed experts), in the device layout ktb200_rawint4_pack writes: 144 B per 256 values of a row,
+     *   bytes 0..15          eight bf16 group scales
+     *   bytes 16+16j..31+16j group j = four 32-bit words, word w holds columns 8w..8w+7 of the group, column 8w+i in
+     *                        bits 4i..4i+3 as u = q + 8 (the compressed-tensors words unchanged)
+     * value = (u - 8) * scale.  Routed experts only (ktb200_moe_*): linears and MLP handles reject it. */
+    KTB200_TYPE_RAWINT4_G32 = 256
 };
 
 const char* ktb200_last_error(void);
@@ -97,7 +105,8 @@ int ktb200_moe_warm_up(ktb200_moe* moe, void* stream);
  *     graph serves a variable batch; rows >= *bsz are left untouched.
  * Arithmetic: identical to the reference CPU path — activations quantised to the weight type's
  * vec_dot_type (Q8_K / Q8_0) with the reference's rounding, integer dot products, fp32 scales,
- * fp32 accumulation over experts in expert_ids order, output rounded like ggml from_float. */
+ * fp32 accumulation over experts in expert_ids order, output rounded like ggml from_float.
+ * RAWINT4_G32 experts are W4A16 instead: fp32 activations against (u - 8) * scale, fp32 sums (DESIGN.md §2). */
 int ktb200_moe_forward(ktb200_moe* moe, int qlen, int k, const int64_t* expert_ids_dev,
                        const float* weights_dev, const void* input_dev, void* output_dev,
                        const int* bsz_tensor_dev, void* stream);
@@ -184,6 +193,15 @@ int ktb200_quantize_activations(const void* x_dev, int hidden_type, long n_rows,
  * ------------------------------------------------------------------------------------------ */
 int ktb200_dequantize(const void* src_dev, int ggml_type, long n_elements, void* out_dev, int out_type,
                       void* stream);
+
+/* Load-time conversion of compressed-tensors pack-quantized INT4 (num_bits 4, group 32, symmetric) into the
+ * KTB200_TYPE_RAWINT4_G32 device layout (see the type enum):
+ *   packed_dev    int32 [n_rows][n_cols/8]  (`weight_packed`: value i of a word in bits 4i..4i+3, stored as q + 8)
+ *   scale_bf16_dev bf16  [n_rows][n_cols/32] (`weight_scale`)
+ *   out_dev       caller-owned, n_rows * n_cols / 256 * 144 bytes, 16-byte aligned.
+ * Stacked experts are more rows.  KTB200_EINVAL when n_cols % 256 != 0.  Stream-ordered, no allocation. */
+int ktb200_rawint4_pack(const int32_t* packed_dev, const uint16_t* scale_bf16_dev, long n_rows, long n_cols, void* out_dev,
+                        void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Router.  Replaces MoEGate.forward (archive/ktransformers/models/modeling_deepseek_v3.py:430-481,

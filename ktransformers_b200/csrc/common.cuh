@@ -16,6 +16,7 @@
 #define SZ_Q6_K 210
 #define SZ_Q8_K 292
 #define SZ_IQ4_XS 136
+#define SZ_RAWINT4 144   // 8 bf16 scales + 256 nibbles (rawint4.cuh)
 
 namespace ktb {
 
@@ -69,6 +70,7 @@ __host__ __device__ inline long type_size(int t) {
         case KTB200_TYPE_Q6_K: return SZ_Q6_K;
         case KTB200_TYPE_Q8_K: return SZ_Q8_K;
         case KTB200_TYPE_IQ4_XS: return SZ_IQ4_XS;
+        case KTB200_TYPE_RAWINT4_G32: return SZ_RAWINT4;
         default: return 0;
     }
 }
@@ -77,7 +79,7 @@ __host__ __device__ inline long blck_size(int t) {
         case KTB200_TYPE_F32: case KTB200_TYPE_F16: case KTB200_TYPE_BF16: return 1;
         case KTB200_TYPE_Q8_0: return 32;
         case KTB200_TYPE_Q2_K: case KTB200_TYPE_Q3_K: case KTB200_TYPE_Q4_K: case KTB200_TYPE_Q5_K:
-        case KTB200_TYPE_Q6_K: case KTB200_TYPE_Q8_K: case KTB200_TYPE_IQ4_XS: return QK_K;
+        case KTB200_TYPE_Q6_K: case KTB200_TYPE_Q8_K: case KTB200_TYPE_IQ4_XS: case KTB200_TYPE_RAWINT4_G32: return QK_K;
         default: return 0;
     }
 }
@@ -85,6 +87,8 @@ __host__ __device__ inline bool is_kquant(int t) {
     return t == KTB200_TYPE_Q2_K || t == KTB200_TYPE_Q3_K || t == KTB200_TYPE_Q4_K || t == KTB200_TYPE_Q5_K ||
            t == KTB200_TYPE_Q6_K || t == KTB200_TYPE_IQ4_XS;
 }
+// not a K-quant: it has its own kernels (rawint4.cuh) and no path through the generic K-quant ones
+__host__ __device__ inline bool is_rawint4(int t) { return t == KTB200_TYPE_RAWINT4_G32; }
 __host__ __device__ inline bool is_hidden_type(int t) {
     return t == KTB200_TYPE_F32 || t == KTB200_TYPE_F16 || t == KTB200_TYPE_BF16;
 }

@@ -40,6 +40,19 @@ __global__ void __launch_bounds__(256) dequant_q8_0_kernel(const uint8_t* src, l
     }
 }
 
+// RAWINT4_G32 device blocks (rawint4.cuh): thread = one 32-bit word = 8 values, value = (u - 8) * s in fp32, then cast
+template <typename OutT>
+__global__ void __launch_bounds__(256) dequant_rawint4_kernel(const uint8_t* src, long n_words, OutT* out) {
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n_words; i += (long)gridDim.x * blockDim.x) {
+        const uint8_t* blk = src + (i >> 5) * SZ_RAWINT4;
+        const int wi = (int)(i & 31);                     // word of the block; group wi / 4
+        const uint32_t w = *reinterpret_cast<const uint32_t*>(blk + 16 + 4 * wi);
+        const float s = __uint_as_float((uint32_t)reinterpret_cast<const uint16_t*>(blk)[wi >> 2] << 16);
+#pragma unroll
+        for (int v = 0; v < 8; v++) out[i * 8 + v] = cast_out<OutT>((float)((int)((w >> (4 * v)) & 15u) - 8) * s);
+    }
+}
+
 template <typename InT, typename OutT>
 __global__ void __launch_bounds__(256) convert_kernel(const InT* src, long n, OutT* out) {
     for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
@@ -60,6 +73,10 @@ static int dequant_to(const void* src, int type, long n, OutT* out, cudaStream_t
         long blocks = (ng + 255) / 256;
         if (blocks > max_blocks) blocks = max_blocks;
         dequant_k_kernel<OutT><<<(unsigned)blocks, 256, 0, s>>>(reinterpret_cast<const uint8_t*>(src), type, (int)type_size(type), ng, out);
+    } else if (is_rawint4(type)) {
+        long blocks = (n / 8 + 255) / 256;
+        if (blocks > max_blocks) blocks = max_blocks;
+        dequant_rawint4_kernel<OutT><<<(unsigned)blocks, 256, 0, s>>>(reinterpret_cast<const uint8_t*>(src), n / 8, out);
     } else if (type == KTB200_TYPE_F32 || type == KTB200_TYPE_F16 || type == KTB200_TYPE_BF16) {
         long blocks = (n + 255) / 256;
         if (blocks > max_blocks) blocks = max_blocks;

@@ -4,7 +4,7 @@
 #include "common.cuh"
 
 namespace ktb {
-enum FmtId { FMT_Q4K, FMT_Q5K, FMT_Q6K8, FMT_Q6K4T, FMT_GENK, FMT_NONE };
+enum FmtId { FMT_Q4K, FMT_Q5K, FMT_Q6K8, FMT_Q6K4T, FMT_GENK, FMT_RAWINT4, FMT_NONE };
 // how a Q6_K tensor was re-laid at load time
 enum Q6Layout { LAYOUT_RAW = 0, LAYOUT_SOA8 = 1, LAYOUT_T4 = 2 };
 
@@ -14,6 +14,7 @@ static inline FmtId pick_fmt(int type, int layout) {
     if (type == KTB200_TYPE_Q6_K && layout == LAYOUT_SOA8) return FMT_Q6K8;
     if (type == KTB200_TYPE_Q6_K && layout == LAYOUT_T4) return FMT_Q6K4T;
     if (is_kquant(type)) return FMT_GENK;
+    if (is_rawint4(type)) return FMT_RAWINT4;
     return FMT_NONE;
 }
 }  // namespace ktb

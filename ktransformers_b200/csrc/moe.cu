@@ -7,6 +7,7 @@
 
 #include "gemv_bulk.cuh"
 #include "dense_bulk.cuh"
+#include "rawint4.cuh"
 #include "handles.cuh"
 
 namespace ktb {
@@ -274,10 +275,41 @@ static int launch_dense_q4k(const RowsParams& p, int T, int device, cudaStream_t
     return KTB200_OK;
 }
 
+// RAWINT4 gate/up pairs (rows_bulk_i4_kernel): the only kernel for the format, so a shape it cannot take is an error.
+// Ring of 2 slots per warp (one (gate row | up row) pair in flight while one is computed); tokens per chunk: as many
+// (<= 8) as leave room for >= 8 warps.
+static int launch_rows_i4(const RowsParams& p, int T, int device, cudaStream_t stream) {
+    constexpr int S = 2;
+    const int nblk = p.ncols / QK_K;
+    const size_t slot = (size_t)2 * nblk * SZ_RAWINT4;
+    const size_t act_tok = (size_t)nblk * kI4ActStride;
+    const long total = (long)p.slots * p.rows;
+    if (p.x0 || p.shared_token >= 0 || p.slots > 200 || total >= (1L << 26)) { set_error("RAWINT4 gate/up: unsupported launch"); return KTB200_EINVAL; }
+    auto head = [&](int tc) { return ((size_t)tc * act_tok + (size_t)tc * p.slots * 4 + 15) & ~(size_t)15; };
+    int tc = T < kI4MaxChunkTokens ? T : kI4MaxChunkTokens;
+    while (tc > 1 && head(tc) + 64 + (size_t)8 * S * (slot + 8) > kSmemCap) tc--;
+    if (head(tc) + 64 >= kSmemCap) { set_error("RAWINT4 gate/up: hidden_size %d does not fit shared memory", p.ncols); return KTB200_EINVAL; }
+    int W = (int)((kSmemCap - head(tc) - 16) / (S * (slot + 8)));
+    if (W > cfg_bulk_warps()) W = cfg_bulk_warps();
+    if (W < 1) { set_error("RAWINT4 gate/up: hidden_size %d does not fit shared memory", p.ncols); return KTB200_EINVAL; }
+    const size_t smem = head(tc) + (((size_t)W * S * 8 + 15) & ~(size_t)15) + (size_t)W * S * slot;
+    int gx = num_sms(device);
+    if (gx > total) gx = (int)total;
+    if (gx < 1) gx = 1;
+    KTB_CUDA_CHECK(cudaFuncSetAttribute(rows_bulk_i4_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    rows_bulk_i4_kernel<S><<<gx, W * 32, smem, stream>>>(p, tc);
+    KTB_LAUNCH_CHECK();
+    return KTB200_OK;
+}
+
 template <bool PAIR>
 static int launch_rows(FmtId f, const RowsParams& p_in, int T, int device, cudaStream_t stream) {
     RowsParams p = p_in;
     p.ntokens = T;
+    if (f == FMT_RAWINT4) {
+        if (!PAIR) { set_error("RAWINT4: routed experts only"); return KTB200_EINVAL; }
+        return launch_rows_i4(p, T, device, stream);
+    }
     if (!PAIR && f == FMT_Q4K) {
         const int rcd = launch_dense_q4k(p, T, device, stream);
         if (rcd != 1) return rcd;
@@ -429,9 +461,55 @@ static bool q6k4t_eligible(int rows, int ncols, int ns_max, int device) {
     return reduce_bulk_plan<BulkQ6K4T>(rows, ncols, ns_max, 3, device, nullptr, nullptr, nullptr) >= 4;
 }
 
+// Shared-memory plan of reduce_bulk_i4_kernel<S> for `pcap` staged pairs: returns the warp count (0 = does not fit)
+static int reduce_i4_plan(int rows, int ncols, int pcap, int S, int device, int* gx_out, int* nrows_max_out, size_t* smem_out) {
+    const int nb = ncols / QK_K;
+    if (rows % 4 || nb < 1 || pcap > 200) return 0;
+    const size_t item = (size_t)4 * nb * SZ_RAWINT4;
+    const int quads = rows / 4;
+    int gx = num_sms(device);
+    if (gx > quads) gx = quads;
+    if (gx < 1) gx = 1;
+    const int nrows_max = ((quads + gx - 1) / gx) * 4;
+    size_t base = (size_t)pcap * nb * kI4ActStride + (size_t)nrows_max * pcap * 4 + (size_t)pcap * 4;
+    base = (base + 15) & ~(size_t)15;
+    if (base + 16 >= kSmemCap) return 0;
+    int W = (int)((kSmemCap - base - 16) / ((size_t)S * (item + 8)));
+    if (W > cfg_bulk_warps()) W = cfg_bulk_warps();
+    if (W > kBulkMaxWarpsDown) W = kBulkMaxWarpsDown;
+    if (W < 1) return 0;
+    if (gx_out) *gx_out = gx;
+    if (nrows_max_out) *nrows_max_out = nrows_max;
+    if (smem_out) *smem_out = base + (((size_t)W * S * 8 + 15) & ~(size_t)15) + (size_t)W * S * item;
+    return W;
+}
+
+// RAWINT4 down projection (reduce_bulk_i4_kernel): pair capacity of a token chunk as in launch_reduce_bulk.
+static int launch_reduce_i4(const ReduceParams& p, int T, int device, cudaStream_t stream) {
+    constexpr int S = 2;
+    if (p.xw) { set_error("RAWINT4 down: the shared expert cannot ride in the routed launch"); return KTB200_EINVAL; }
+    const int ns = p.slots;
+    int pcap = ns;
+    if (T > 1) {
+        int want = 2 * ns < 18 ? 2 * ns : (ns > 18 ? ns : 18);
+        if ((long)T * ns < want) want = T * ns;
+        while (want > ns && reduce_i4_plan(p.rows, p.ncols, want, S, device, nullptr, nullptr, nullptr) < 10) want--;
+        pcap = want;
+    }
+    int gx = 0, nrows_max = 0;
+    size_t smem = 0;
+    const int W = reduce_i4_plan(p.rows, p.ncols, pcap, S, device, &gx, &nrows_max, &smem);
+    if (!W) { set_error("RAWINT4 down: k=%d x intermediate_size=%d does not fit shared memory", ns, p.ncols); return KTB200_EINVAL; }
+    KTB_CUDA_CHECK(cudaFuncSetAttribute(reduce_bulk_i4_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    reduce_bulk_i4_kernel<S><<<gx, W * 32, smem, stream>>>(p, nrows_max, pcap);
+    KTB_LAUNCH_CHECK();
+    return KTB200_OK;
+}
+
 static int launch_reduce(FmtId f, const ReduceParams& p_in, int T, int device, cudaStream_t stream) {
     ReduceParams p = p_in;
     p.ntokens = T;
+    if (f == FMT_RAWINT4) return launch_reduce_i4(p, T, device, stream);
     if (f == FMT_Q6K4T) {
         const int rc = launch_reduce_bulk<BulkQ6K4T>(p, T, device, stream);
         if (rc == 1) { set_error("Q6_K tile layout: k=%d x ncols=%d does not fit the bulk kernel", p.slots, p.ncols); return KTB200_EINVAL; }
@@ -489,7 +567,12 @@ int ktb200_moe_create(const ktb200_moe_config* c, int device, ktb200_moe** out) 
     if (!c || !out) { set_error("null argument"); return KTB200_EINVAL; }
     if (c->expert_num <= 0 || c->routed_expert_num <= 0 || c->hidden_size <= 0 || c->intermediate_size <= 0 ||
         c->group_max_len <= 0) { set_error("MOEConfig: non-positive dimension"); return KTB200_EINVAL; }
-    if (!weight_type_ok(c->gate_type) || !weight_type_ok(c->up_type) || !weight_type_ok(c->down_type)) {
+    const int n_i4 = is_rawint4(c->gate_type) + is_rawint4(c->up_type) + is_rawint4(c->down_type);
+    if (n_i4 != 0 && n_i4 != 3) {
+        set_error("MOEConfig: RAWINT4_G32 must be the type of all three tensors (gate %d up %d down %d)", c->gate_type, c->up_type, c->down_type);
+        return KTB200_EINVAL;
+    }
+    if (!n_i4 && (!weight_type_ok(c->gate_type) || !weight_type_ok(c->up_type) || !weight_type_ok(c->down_type))) {
         set_error("MOEConfig: unsupported ggml weight type (gate %d up %d down %d)", c->gate_type, c->up_type, c->down_type);
         return KTB200_EINVAL;
     }
@@ -641,6 +724,7 @@ int ktb200_moe_forward_ep(ktb200_moe* m, ktb200_mlp* shared, int qlen, int k, co
                           const void* input, void* partial_out, int own_token, void* shared_out, const int* bsz, void* stream) {
     if (!shared || !shared_out || own_token < 0 || own_token >= qlen) { set_error("moe_forward_ep: shared handle, shared_out and 0 <= own_token < qlen are required"); return KTB200_EINVAL; }
     if (!shared->loaded) { set_error("shared expert: Not Loaded"); return KTB200_ESTATE; }
+    if (m && is_rawint4(m->cfg.gate_type)) { set_error("moe_forward_ep: RAWINT4_G32 experts are not supported (their kernels have no shared-expert slot)"); return KTB200_EINVAL; }
     // shared_out rows are indexed like the tokens: point the kernels at a virtual base so that row `own_token` is shared_out
     uint8_t* base = reinterpret_cast<uint8_t*>(shared_out) - (size_t)own_token * shared->H * type_size(shared->hidden_type);
     return moe_forward_impl(m, qlen, k, ids, weights, input, partial_out, bsz, (cudaStream_t)stream, nullptr, shared, own_token, base);
@@ -838,6 +922,23 @@ int ktb200_mlp_forward(ktb200_mlp* m, int qlen, const void* input, void* output,
     dp.w = m->down; dp.type = m->down_type; dp.n_experts = 1; dp.rows = m->H; dp.ncols = m->I; dp.slots = 1; dp.ids = nullptr;
     dp.weights = nullptr; dp.a = m->inter; dp.out = output; dp.hidden_type = m->hidden_type; dp.accumulate = accumulate; dp.bsz = bsz;
     return launch_reduce(pick_fmt(m->down_type, m->down_layout), dp, qlen, m->device, s);
+}
+
+// ------------------------------------------------------------------------------------------ RAWINT4 pack
+int ktb200_rawint4_pack(const int32_t* packed, const uint16_t* scale, long n_rows, long n_cols, void* out, void* stream) {
+    if (!packed || !scale || !out) { set_error("rawint4_pack: null pointer"); return KTB200_EINVAL; }
+    if (n_rows < 0 || n_cols <= 0 || n_cols % QK_K) { set_error("rawint4_pack: n_cols=%ld must be a positive multiple of 256", n_cols); return KTB200_EINVAL; }
+    if ((uintptr_t)out & 15) { set_error("rawint4_pack: out must be 16-byte aligned"); return KTB200_EINVAL; }
+    const long n_sb = n_rows * (n_cols / QK_K);
+    if (n_sb == 0) return KTB200_OK;
+    int dev = 0;
+    KTB_CUDA_CHECK(cudaGetDevice(&dev));
+    long blocks = (n_sb * 9 + 255) / 256;
+    if (blocks > (long)num_sms(dev) * 16) blocks = (long)num_sms(dev) * 16;
+    rawint4_pack_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const uint32_t*>(packed), scale, n_sb,
+                                                                             (int)(n_cols / QK_K), reinterpret_cast<uint4*>(out));
+    KTB_LAUNCH_CHECK();
+    return KTB200_OK;
 }
 
 // ------------------------------------------------------------------------------------------ quantize API

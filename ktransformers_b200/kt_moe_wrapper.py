@@ -14,6 +14,10 @@ cuda_stream)`, the capture-batch-size helpers.  What changes underneath:
     skipped (the reference's should_skip_expert, operators/common.hpp:255-258).
   * `physical_to_logical_map_cpu[p]` = logical expert stored in physical slot p (EPLB): the upload permutes the experts
     accordingly, exactly like `load_weights_task(physical_to_logical_map_ptr)` (ext_bindings.cpp:447-471).
+  * `method="B200_RAWINT4"`: kt-kernel's RAWINT4 — the compressed-tensors "pack-quantized" experts Kimi-K2 ships
+    (symmetric INT4, group 32, bf16 scales, `<key>.{e}.{gate,up,down}_proj.{weight_packed,weight_scale,weight_shape}` in a
+    safetensors directory).  The packed words and scales are uploaded and converted once on the GPU
+    (`ktb200_rawint4_pack`); decode runs W4A16 on the sm_90a kernels (no activation quantisation).
   * deferred experts (`max_deferred_experts_per_token`) have no purpose without a CPU/GPU overlap: must be 0 / None.
 """
 from __future__ import annotations
@@ -24,11 +28,12 @@ from typing import List, Optional
 import numpy as np
 import torch
 
+from .native import RAWINT4_G32
 from .operators.experts import KExpertsB200
 from .util.custom_gguf import GGML_NAMES, B200_WEIGHT_TYPES
 from .util.custom_loader import ModelLoaderFactory
 
-B200_METHODS = frozenset(["B200_GGUF"])
+B200_METHODS = frozenset(["B200_GGUF", "B200_RAWINT4"])
 
 
 class KTMoEWrapper:
@@ -82,17 +87,48 @@ class KTMoEWrapper:
         ld = KTMoEWrapper._loaders.get(self.weight_path)
         if ld is None:
             ld = KTMoEWrapper._loaders[self.weight_path] = ModelLoaderFactory.create_loader(self.weight_path)
+        if self.method == "B200_RAWINT4":
+            if not hasattr(ld, "load_experts"):
+                raise ValueError(f"B200_RAWINT4 reads compressed-tensors safetensors; {self.weight_path} is not a safetensors directory")
+            w = ld.load_experts(self.key)
+            if w.get("gate_type") != RAWINT4_G32:
+                raise ValueError(f"B200_RAWINT4: the experts of {self.key} are not compressed-tensors INT4 tensors")
+            self._load_rawint4(w, physical_to_logical_map_cpu)
+            return
         names = {n: f"{self.key}.ffn_{n}_exps.weight" for n in ("gate", "up", "down")}
         types = {n: int(ld.get_ggml_type(names[n])) for n in names}
         self._load({n: ld.get_mmap_tensor(names[n]) for n in names}, types, physical_to_logical_map_cpu)
 
-    def load_weights_from_tensors(self, gate_proj, up_proj, down_proj, physical_to_logical_map_cpu=None, ggml_types=None):
-        """The reference quantises bf16/fp16 tensors online here; this backend takes tensors that ARE ggml blocks already
-        (uint8, `[E, rows, blocks * block_bytes]`) together with `ggml_types=(gate, up, down)`."""
+    def load_weights_from_tensors(self, gate_proj, up_proj, down_proj, physical_to_logical_map_cpu=None, ggml_types=None,
+                                  gate_scale=None, up_scale=None, down_scale=None):
+        """The reference quantises bf16/fp16 tensors online here; this backend takes tensors that ARE quantised already:
+        B200_GGUF: ggml blocks (uint8, `[E, rows, blocks * block_bytes]`) together with `ggml_types=(gate, up, down)`;
+        B200_RAWINT4: compressed-tensors `weight_packed` (int32 `[E, rows, cols/8]`) as gate/up/down_proj and
+        `weight_scale` (bfloat16 `[E, rows, cols/32]`) as gate/up/down_scale."""
+        if self.method == "B200_RAWINT4":
+            if gate_scale is None or up_scale is None or down_scale is None:
+                raise ValueError("B200_RAWINT4: gate_scale, up_scale and down_scale (bfloat16 weight_scale tensors) are required")
+            if ggml_types is not None:
+                raise ValueError("B200_RAWINT4: ggml_types does not apply to compressed-tensors INT4 weights")
+            self._load_rawint4({"gate": gate_proj, "up": up_proj, "down": down_proj, "gate_scale": gate_scale, "up_scale": up_scale,
+                                "down_scale": down_scale}, physical_to_logical_map_cpu)
+            return
+        if any(t is not None for t in (gate_scale, up_scale, down_scale)):
+            raise ValueError("gate/up/down_scale belong to method='B200_RAWINT4'")
         if ggml_types is None or any(t.dtype != torch.uint8 for t in (gate_proj, up_proj, down_proj)):
             raise NotImplementedError("online quantisation to K-quants is not built: pass raw ggml blocks (uint8) and ggml_types=(g, u, d)")
         self._load({"gate": gate_proj, "up": up_proj, "down": down_proj},
                    dict(zip(("gate", "up", "down"), (int(t) for t in ggml_types))), physical_to_logical_map_cpu)
+
+    def _load_rawint4(self, t, p2l):
+        w = {}
+        for n in ("gate", "up", "down", "gate_scale", "up_scale", "down_scale"):
+            a = torch.as_tensor(t[n])
+            if a.dim() != 3 or a.shape[0] != self.num_experts:
+                raise ValueError(f"B200_RAWINT4: {n} must be [num_experts={self.num_experts}, rows, cols], got {tuple(a.shape)}")
+            w[n] = self._permute(a, self.num_experts, p2l).reshape(a.shape)
+        w.update(gate_type=RAWINT4_G32, up_type=RAWINT4_G32, down_type=RAWINT4_G32)
+        self._finish_load(w)
 
     def _load(self, raw, types, p2l):
         for t in types.values():
@@ -100,6 +136,9 @@ class KTMoEWrapper:
                 raise ValueError(f"ggml type {GGML_NAMES.get(t, t)} is not supported by the sm_90a kernels")
         w = {n: self._permute(raw[n], self.num_experts, p2l) for n in ("gate", "up", "down")}
         w.update(gate_type=types["gate"], up_type=types["up"], down_type=types["down"])
+        self._finish_load(w)
+
+    def _finish_load(self, w):
         self.moe.load(w, device=self.device)
         dt = {0: torch.float32, 1: torch.float16, 30: torch.bfloat16}[self.moe.hidden_type]
         self._out = torch.zeros((self.moe.max_tokens, self.hidden_size), dtype=dt, device=self.device)

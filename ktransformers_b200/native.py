@@ -20,6 +20,8 @@ OK, EINVAL, ECUDA, ESTATE, ENOMEM = 0, -1, -2, -3, -4
 # ggml type ids (third_party/llama.cpp/ggml.h:349-380)
 GGML_F32, GGML_F16, GGML_Q8_0, GGML_Q2_K, GGML_Q3_K, GGML_Q4_K, GGML_Q5_K, GGML_Q6_K, GGML_Q8_K = 0, 1, 8, 10, 11, 12, 13, 14, 15
 GGML_IQ4_XS, GGML_BF16 = 23, 30
+# not a ggml id (include/ktb200.h): symmetric INT4, group 32, bf16 scales, in the layout ktb200_rawint4_pack writes
+RAWINT4_G32 = 256
 
 
 class MoeConfig(C.Structure):
@@ -78,6 +80,7 @@ SYMBOLS = {
     "ktb200_moe_forward_shared": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
     "ktb200_quantize_activations": (_I, [_VP, _I, _L, _L, _I, _VP, _VP]),
     "ktb200_dequantize": (_I, [_VP, _I, _L, _VP, _I, _VP]),
+    "ktb200_rawint4_pack": (_I, [_VP, _VP, _L, _L, _VP, _VP]),
     "ktb200_moe_gate_forward": (_I, [C.POINTER(GateConfig), _I, _VP, _VP, _VP, _VP, _VP, _VP]),
     "ktb200_moe_block_forward": (_I, [C.POINTER(GateConfig), _VP, _VP, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
     "ktb200_moe_block_forward_host": (_I, [C.POINTER(GateConfig), _VP, _VP, _I, _VP, _VP, _VP, _VP, _VP]),
@@ -159,3 +162,8 @@ def check(rc: int) -> None:
 
 def launch_count() -> int:
     return int(lib().ktb200_launch_count())
+
+
+def type_size(ggml_type: int) -> int:
+    """Bytes per block of a weight type (ktb200_type_size; 144 for RAWINT4_G32), 0 when unsupported."""
+    return int(lib().ktb200_type_size(int(ggml_type)))

@@ -62,6 +62,14 @@ class PeerExchange:
 
 def attach_expert_parallel(model: torch.nn.Module, hidden_size: int, hidden_type: int, device, group=None) -> PeerExchange:
     """Give every injected MoE block of `model` whose experts are sharded the same PeerExchange."""
+    from ..native import RAWINT4_G32
+    for m in model.modules():
+        gen = getattr(getattr(m, "experts", None), "generate_experts", None)
+        if hasattr(m, "_block_handles") and getattr(gen, "gate_type", None) == RAWINT4_G32:
+            # the single-launch NVLink kernel does not take INT4 experts, and without it a sharded block would return its
+            # shard's partial sums as the layer output
+            raise ValueError(f"attach_expert_parallel: {getattr(m, 'key', type(m).__name__)} has RAWINT4_G32 experts, "
+                             "which the expert-parallel kernel does not support")
     ex = PeerExchange(hidden_size, hidden_type, device, group)
     for m in model.modules():
         if hasattr(m, "_block_handles"):

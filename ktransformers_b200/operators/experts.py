@@ -108,11 +108,32 @@ class KExpertsB200(KExpertsBase):
         if w is None:
             w = self.load_weights()[self.key]
         self.gate_type, self.up_type, self.down_type = int(w["gate_type"]), int(w["up_type"]), int(w["down_type"])
-        for t in (self.gate_type, self.up_type, self.down_type):
+        n_i4 = sum(t == native.RAWINT4_G32 for t in (self.gate_type, self.up_type, self.down_type))
+        if n_i4 not in (0, 3):
+            raise ValueError("KExpertsB200: RAWINT4_G32 must be the type of all three expert tensors")
+        for t in (self.gate_type, self.up_type, self.down_type) if not n_i4 else ():
             if GGML_NAMES.get(t) not in B200_WEIGHT_TYPES:
                 raise ValueError(f"KExpertsB200: ggml type {GGML_NAMES.get(t, t)} is not supported by the sm_90a kernels")
         E = self.n_routed_experts
         per, lo = E // self.ep_size, (E // self.ep_size) * self.ep_rank
+        dev = torch.device(device)
+        H, I = self.config.hidden_size, self.config.moe_intermediate_size
+
+        def pack_rawint4(name, rows, cols):
+            # compressed-tensors weight_packed int32 [E][rows][cols/8] + weight_scale bf16 [E][rows][cols/32]: the shard's
+            # experts go up as staging copies and are converted into a fresh buffer; the caller's tensors are not touched
+            p, s = torch.as_tensor(w[name]), torch.as_tensor(w[name + "_scale"])
+            if p.dtype != torch.int32 or s.dtype != torch.bfloat16:
+                raise ValueError(f"KExpertsB200: RAWINT4 {name} needs int32 weight_packed and bfloat16 weight_scale, got {p.dtype} / {s.dtype}")
+            if tuple(p.shape) != (E, rows, cols // 8) or tuple(s.shape) != (E, rows, cols // 32):
+                raise ValueError(f"KExpertsB200: RAWINT4 {name} shapes {tuple(p.shape)} / {tuple(s.shape)}, expected "
+                                 f"{(E, rows, cols // 8)} / {(E, rows, cols // 32)}")
+            p_d = p[lo:lo + per].to(dev).contiguous()
+            s_d = s[lo:lo + per].to(dev).contiguous()
+            out = torch.empty(per * rows * cols // 256 * 144, dtype=torch.uint8, device=dev)
+            with torch.cuda.device(dev):
+                native.check(lib.ktb200_rawint4_pack(p_d.data_ptr(), s_d.data_ptr(), per * rows, cols, out.data_ptr(), _stream(dev)))
+            return out
 
         def upload(a):
             a = a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(np.asarray(a)).view(np.uint8).reshape(-1))
@@ -122,8 +143,10 @@ class KExpertsB200(KExpertsBase):
             # load_weights re-tiles Q6_K bytes IN PLACE: never hand it memory the caller still owns
             return sl.clone() if sl.device == torch.device(device) else sl.to(device).contiguous()
 
-        self.gate, self.up, self.down = upload(w["gate"]), upload(w["up"]), upload(w["down"])
-        dev = torch.device(device)
+        if n_i4:
+            self.gate, self.up, self.down = pack_rawint4("gate", I, H), pack_rawint4("up", I, H), pack_rawint4("down", H, I)
+        else:
+            self.gate, self.up, self.down = upload(w["gate"]), upload(w["up"]), upload(w["down"])
         self.dev_index = dev.index if dev.index is not None else torch.cuda.current_device()
         want_dtype = self.hidden_dtype or torch.get_default_dtype()
         hidden_type = TORCH_TO_GGML_HIDDEN[want_dtype] if want_dtype in TORCH_TO_GGML_HIDDEN else 30

@@ -11,6 +11,7 @@
 """
 from __future__ import annotations
 
+import json
 import math
 import os
 import struct
@@ -224,6 +225,7 @@ class SafeTensorLoader(ModelLoader):
         self.tensor_device_map: dict = {}        # filled by optimize.inject, like GGUFLoader's
         self.tensor_info: dict = {}
         root = os.path.dirname(file_path) if os.path.isfile(file_path) else file_path
+        self.root = root
         found = False
         for cur, _, files in os.walk(root):
             for fn in sorted(files):
@@ -275,8 +277,34 @@ class SafeTensorLoader(ModelLoader):
             raise NotImplementedError(f"{name}: quantised tensors of a safetensors file are consumed raw (get_mmap_tensor / KLinearFP8), not dequantised")
         return t.to(target_dtype) if target_dtype is not None else t
 
+    def _check_int4_quantization_config(self):
+        """config.json's compressed-tensors `quantization_config`, when present, must describe the INT4 format the
+        RAWINT4 kernels compute: every config group's weights are num_bits 4, group_size 32, symmetric, type int, strategy group."""
+        path = os.path.join(self.root, "config.json")
+        if not os.path.isfile(path):
+            return
+        with open(path) as f:
+            qc = json.load(f).get("quantization_config")
+        if qc is None:
+            return
+        groups = qc.get("config_groups")
+        if not isinstance(groups, dict) or not groups:
+            raise ValueError("quantization_config: config_groups is missing; expected compressed-tensors INT4 weights")
+        want = {"num_bits": 4, "group_size": 32, "symmetric": True, "type": "int", "strategy": "group"}
+        for gname, g in groups.items():
+            wq = (g or {}).get("weights") or {}
+            for field, val in want.items():
+                if wq.get(field) != val:
+                    raise ValueError(f"quantization_config: config_groups.{gname}.weights.{field} = {wq.get(field)!r}, "
+                                     f"the RAWINT4 kernels need {val!r}")
+
     def load_experts(self, key: str, device: str = "cpu") -> dict:
-        """custom_loader.py:114-148 (hybrid branch): {gate, up, down: raw ggml bytes, *_type: ggml type}"""
+        """custom_loader.py:114-148 (hybrid branch): {gate, up, down: raw ggml bytes, *_type: ggml type}.
+        Per-expert compressed-tensors INT4 tensors (`{key}.{e}.{gate,up,down}_proj.{weight_packed,weight_scale,weight_shape}`,
+        Kimi-K2) are stacked instead: {gate, up, down: int32 [E, rows, cols/8], *_scale: bf16 [E, rows, cols/32],
+        *_type: RAWINT4_G32}."""
+        if f"{key}.0.gate_proj.weight_packed" in self.tensor_file_map:
+            return self._load_int4_experts(key)
         base = translate_name_to_gguf(key)
         if not self.has_tensor(base + ".ffn_gate_exps.weight"):
             raise ValueError(f"No experts found for key {key}")
@@ -284,6 +312,36 @@ class SafeTensorLoader(ModelLoader):
         for n in ("gate", "up", "down"):
             out[n] = self.get_mmap_tensor(f"{base}.ffn_{n}_exps.weight")
             out[n + "_type"] = self.get_ggml_type(f"{base}.ffn_{n}_exps.weight")
+        return out
+
+    def _load_int4_experts(self, key: str) -> dict:
+        from ..native import RAWINT4_G32
+        self._check_int4_quantization_config()
+        E = 0
+        while f"{key}.{E}.gate_proj.weight_packed" in self.tensor_file_map:
+            E += 1
+        out = {}
+        for n in ("gate", "up", "down"):
+            packed, scales, shape = [], [], None
+            for e in range(E):
+                p = f"{key}.{e}.{n}_proj"
+                for suffix in ("weight_packed", "weight_scale", "weight_shape"):
+                    if f"{p}.{suffix}" not in self.tensor_file_map:
+                        raise ValueError(f"{p}.{suffix} is missing")
+                w, s = self.load_tensor(f"{p}.weight_packed"), self.load_tensor(f"{p}.weight_scale")
+                ws = tuple(int(v) for v in self.load_tensor(f"{p}.weight_shape").reshape(-1).tolist())
+                if w.dtype != torch.int32 or s.dtype != torch.bfloat16:
+                    raise ValueError(f"{p}: weight_packed must be int32 and weight_scale bfloat16, got {w.dtype} / {s.dtype}")
+                if len(ws) != 2 or ws[1] % 256:
+                    raise ValueError(f"{p}.weight_shape {ws}: expected [rows, cols] with cols a multiple of 256")
+                if tuple(w.shape) != (ws[0], ws[1] // 8) or tuple(s.shape) != (ws[0], ws[1] // 32):
+                    raise ValueError(f"{p}: weight_packed {tuple(w.shape)} / weight_scale {tuple(s.shape)} do not match weight_shape {ws}")
+                if shape is not None and ws != shape:
+                    raise ValueError(f"{p}.weight_shape {ws} differs from expert 0's {shape}")
+                shape = ws
+                packed.append(w)
+                scales.append(s)
+            out[n], out[n + "_scale"], out[n + "_type"] = torch.stack(packed), torch.stack(scales), RAWINT4_G32
         return out
 
     def load_gate(self, key: str, device: str = "cpu") -> dict:
