@@ -376,6 +376,10 @@ int ktb200_debug_stream_read(const void* src_dev, long bytes, int mode, int unro
  * Phase trace of ktb200_moe_block_forward (profiles/block_trace.py): while trace_dev != NULL, thread 0 of every CTA
  * writes %globaltimer at the phase boundaries into trace_dev[cta][16] (uint64, >= num_SMs * 16 entries). */
 void ktb200_debug_block_trace(unsigned long long* trace_dev);
+/* The synchronisation words of the handle's MoE-block launches, copied to host memory after a device synchronise: grid
+ * barrier words [0..3], the timeout status word [4], then the per-Q8_K-block readiness words.  Every word is 0 between
+ * launches.  Copies min(n, total) words to host_out (may be NULL) and returns the total, or -1 on error. */
+long ktb200_debug_block_sync_words(ktb200_moe* moe, unsigned* host_out, long n);
 
 #ifdef __cplusplus
 }

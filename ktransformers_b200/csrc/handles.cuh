@@ -40,14 +40,29 @@ struct ktb200_moe {
     float* w_d;
     void* in_d;
     void* out_d;
-    // scratch of the persistent MoE-block kernel (moe_block.cu): router partial sums [8 tokens][8 splits][512 experts]
-    // and two pairs of grid-barrier words used alternately (zero between launches)
+    // scratch of the persistent MoE-block kernel (moe_block.cu): router partial sums [8 tokens][8 splits][512 experts];
+    // blk_sync: two pairs of grid-barrier words, a status word, then two sets of per-Q8_K-block readiness words
+    // (blk_ready_words each), pairs and sets used alternately (zero between launches); blk_inter: the kernel's fp32
+    // intermediate [8 tokens][top-k + 1][I], all ones between launches (moe_block.cu: kInterEmpty); blk_stage: it
+    // quantised, [blk_ready_words] x (QK_K int8 | 16 int16 block sums | fp32 scale), as three arrays
     float* blk_partial;
     unsigned* blk_sync;
     unsigned blk_flip;
+    float* blk_inter;
+    uint8_t* blk_stage;
     const void* pf[3];       // ktb200_moe_block_prefetch_hint: ranges the block kernel pulls into L2 during its down phase
     size_t pf_bytes[3];
 };
+
+namespace ktb {
+constexpr int kBlockMaxTokens = 8;   // tokens one persistent MoE-block launch takes
+constexpr int kBlkStatusWord = 4, kBlkReadyWord = 8;   // offsets in ktb200_moe::blk_sync
+// readiness words of one set: [tokens][slots: top-k + the shared expert][Q8_K blocks of I]
+static inline size_t blk_ready_words(const ktb200_moe_config& c) {
+    const int t = c.group_max_len < kBlockMaxTokens ? c.group_max_len : kBlockMaxTokens;
+    return (size_t)t * (c.routed_expert_num + 1) * (c.intermediate_size / QK_K);
+}
+}  // namespace ktb
 
 struct DeviceGuard {
     int prev;

@@ -593,7 +593,7 @@ int ktb200_moe_create(const ktb200_moe_config* c, int device, ktb200_moe** out) 
     m->gu_soa = false;
     m->down_layout = LAYOUT_RAW;
     m->inter = nullptr; m->ids_d = nullptr; m->w_d = nullptr; m->in_d = nullptr; m->out_d = nullptr;
-    m->blk_partial = nullptr; m->blk_sync = nullptr; m->blk_flip = 0;
+    m->blk_partial = nullptr; m->blk_sync = nullptr; m->blk_flip = 0; m->blk_inter = nullptr; m->blk_stage = nullptr;
     for (int r = 0; r < 3; r++) { m->pf[r] = nullptr; m->pf_bytes[r] = 0; }
     const size_t slots = (size_t)c->group_max_len * c->routed_expert_num;
     const size_t hid = (size_t)c->group_max_len * c->hidden_size * type_size(c->hidden_type);
@@ -604,8 +604,12 @@ int ktb200_moe_create(const ktb200_moe_config* c, int device, ktb200_moe** out) 
     if (e == cudaSuccess) e = cudaMalloc(&m->in_d, hid);
     if (e == cudaSuccess) e = cudaMalloc(&m->out_d, hid);
     if (e == cudaSuccess) e = cudaMalloc(&m->blk_partial, (size_t)8 * 8 * 512 * sizeof(float));
-    if (e == cudaSuccess) e = cudaMalloc(&m->blk_sync, 4 * sizeof(unsigned));
-    if (e == cudaSuccess) e = cudaMemset(m->blk_sync, 0, 4 * sizeof(unsigned));
+    const size_t sync_words = kBlkReadyWord + 2 * blk_ready_words(*c);
+    if (e == cudaSuccess) e = cudaMalloc(&m->blk_sync, sync_words * sizeof(unsigned));
+    if (e == cudaSuccess) e = cudaMemset(m->blk_sync, 0, sync_words * sizeof(unsigned));
+    if (e == cudaSuccess) e = cudaMalloc(&m->blk_inter, blk_ready_words(*c) * QK_K * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemset(m->blk_inter, 0xff, blk_ready_words(*c) * QK_K * sizeof(float));
+    if (e == cudaSuccess) e = cudaMalloc(&m->blk_stage, blk_ready_words(*c) * (QK_K + 32 + 4));
     if (e != cudaSuccess) {
         set_error("cudaMalloc failed: %s", cudaGetErrorString(e));
         ktb200_moe_destroy(m);
@@ -619,7 +623,7 @@ void ktb200_moe_destroy(ktb200_moe* m) {
     if (!m) return;
     DeviceGuard g(m->device);
     cudaFree(m->inter); cudaFree(m->ids_d); cudaFree(m->w_d); cudaFree(m->in_d); cudaFree(m->out_d);
-    cudaFree(m->blk_partial); cudaFree(m->blk_sync);
+    cudaFree(m->blk_partial); cudaFree(m->blk_sync); cudaFree(m->blk_inter); cudaFree(m->blk_stage);
     delete m;
 }
 

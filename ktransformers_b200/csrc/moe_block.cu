@@ -7,14 +7,20 @@
 // Why one kernel: a launch that streams ~100-150 MB pays a fixed cost (launch gap, pipeline ramp, activation prologue,
 // tail) on top of the time its bytes take at the sustained rate (profiles/probe_bulk.py measures both for the bare copy
 // ring).  Three launches per layer pay that three times.  Here one CTA per SM (cooperative launch, 12 warps, 168
-// registers) stays resident for the whole layer and separates the
-// phases with two grid-wide barriers.  What overlaps what was decided with profiles/block_trace.py (%globaltimer at the
-// phase boundaries of every CTA):
-//   * a barrier is split into arrive / wait; weights that do not depend on the other CTAs are requested in between
-//     (the shared expert's rows behind barrier 1, the first down tiles — they need the expert ids only — behind
-//     barrier 2), never before the arrive: a fence issued with bulk copies in flight waits for them;
-//   * x is quantised under barrier 1 (the router reads x itself); the shared expert's gate/up rows are consumed by
+// registers) stays resident for the whole layer.  One grid-wide barrier separates the router from the top-k; gate/up
+// hands its output to down through per-Q8_K-block readiness instead.  What overlaps what was decided with
+// profiles/block_trace.py (%globaltimer at the phase boundaries of every CTA):
+//   * the barrier is split into arrive / wait; the shared expert's first rows are requested in between, never before
+//     the arrive: a fence issued with bulk copies in flight waits for them (measured again on H100: one gpu-scope fence
+//     per CTA and Q8_K block inside the gate/up stream cost ~10 us per layer);
+//   * x is quantised under the barrier (the router reads x itself); the shared expert's gate/up rows are consumed by
 //     warps 4.. while warps 0..3 run the top-k;
+//   * gate/up is entry-major: every CTA computes a slice of every entry, in work-list order, so the entries complete
+//     one after another across the grid.  The producers only store (`inter` starts out as kInterEmpty: a consumer sees
+//     each value arrive, no fence or count is needed).  Each Q8_K block is quantised once, by the first CTA to claim
+//     it, into a global staging buffer; a CTA's down tiles of entry j start as soon as entry j is staged, while other
+//     CTAs may still be computing later entries.  The claims and their fences run on one warp per CTA that streams no
+//     down tiles;
 //   * the selection runs redundantly in every CTA (128 threads, from the same partial sums in the same order): no
 //     second barrier and no global round trip for the ids;
 //   * programmatic dependent launch: the router's weight loads are issued before griddepcontrol.wait, so the next
@@ -32,7 +38,6 @@ namespace ktb {
 
 constexpr int kBlockWarps = 15;    // 480 threads -> 128 registers; 15 x 13440-byte rings + staging = 227 KB
 constexpr int kBlockWarpsLo = 12;  // 384 threads -> 168 registers (KTB200_BLK_WARPS <= 12)
-constexpr int kBlockMaxTokens = 8;
 
 struct BlockParams {
     GateParams g;                        // router (W, bias, partial scratch, idx / w / logits outputs, x)
@@ -41,13 +46,20 @@ struct BlockParams {
     int n_local, id_offset;              // this shard owns expert ids [id_offset, id_offset + n_local)
     int H, I, k;
     int hidden_type, use_silu;
-    float* inter;                        // [T][ns][I] fp32
+    float* inter;                        // [T][ns][I] fp32 (moe_block_kernel: kInterEmpty where not written yet)
     void* out;                           // [T][H]
     unsigned* sync;                      // [0] barrier counter, [1] exit counter; both zero between launches
+    // moe_block_kernel: ready[(t * ns + slot) * nb + b] of Q8_K block b of `inter`: 1 = a CTA is quantising it into the
+    // stage_* buffers, 2 = staged; zero between launches
+    unsigned* ready;
+    unsigned* status;                    // set to 1 when a readiness wait timed out (the results of that launch are invalid)
+    uint8_t* stage_q;                    // [T][ns][nb][QK_K] int8 quants, same values as the shared-memory `aq` staging
+    int16_t* stage_bs;                   // [T][ns][nb][KBS] block sums (`abs_`)
+    float* stage_d;                      // [T][ns][nb] scales (`adx`)
     int nrows_max;                       // output rows per CTA (stride of the `partial` staging)
     int region_a;                        // bytes of the aliased activation staging
     int ring_bytes;                      // per-warp ring
-    int prime_u, prime_d;                // rows / tiles every warp requests BEFORE the router's / the second grid barrier
+    int prime_u, prime_d;                // rows / tiles every warp requests BEFORE the router's / the second grid barrier (EP)
     unsigned long long* trace;           // debug: [grid][16] globaltimer stamps of the phase boundaries (null: off)
     const uint8_t* pf[3];                // ranges to pull into L2 while the down phase streams (the NEXT layer's router rows and
     unsigned pf_bytes[3];                // shared-expert gate/up rows: ktb200_moe_block_prefetch_hint); null: none
@@ -57,6 +69,31 @@ __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
     unsigned v;
     asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     return v;
+}
+__device__ __forceinline__ unsigned ld_acquire_sys_u32(const unsigned* p) {
+    unsigned v;
+    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ unsigned long long ep_now() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+constexpr unsigned long long kEpTimeoutNs = 4000000000ull;
+// spin until *p - target >= 0 (wrap-safe), acquiring at system (peer memory) or GPU scope; gives up after kEpTimeoutNs
+// and records it in `status`
+template <bool SYS>
+__device__ __forceinline__ void wait_ge(const unsigned* p, unsigned target, unsigned* status) {
+    unsigned long long t0 = 0;
+    unsigned spins = 0;
+    while ((int)((SYS ? ld_acquire_sys_u32(p) : ld_acquire_u32(p)) - target) < 0) {
+        if ((++spins & 1023u) == 0) {
+            const unsigned long long t = ep_now();
+            if (!t0) t0 = t;
+            else if (t - t0 > kEpTimeoutNs) { *status = 1; break; }
+        }
+    }
 }
 
 // Grid-wide barrier over the (co-resident) CTAs, split in two so that work which does not depend on the other CTAs —
@@ -81,12 +118,11 @@ __device__ __forceinline__ void grid_wait(unsigned* counter, unsigned gen) {
 // Programmatic dependent launch: the next layer's launch is processed, and its CTAs start on SMs as they free up,
 // while the tail of this one still runs; everything that depends on the previous kernel comes after griddep_wait().
 
+__device__ __forceinline__ void trace_stamp(const BlockParams& p, int i) {   // from the calling thread
+    if (p.trace) p.trace[blockIdx.x * 16 + i] = ep_now();
+}
 __device__ __forceinline__ void block_stamp(const BlockParams& p, int i) {
-    if (p.trace && threadIdx.x == 0) {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        p.trace[blockIdx.x * 16 + i] = t;
-    }
+    if (threadIdx.x == 0) trace_stamp(p, i);
 }
 
 __device__ __forceinline__ float4 load_x4(const void* x, long i4, int type) {
@@ -114,6 +150,8 @@ struct BlockShared {
     int vs[36];      // work list: slot indices this shard computes (the shared expert, slot k, first)
     int nv;
     unsigned skip;   // bit j: routed slot j is not owned by this shard
+    int ent_state[36];   // down: 0 = entry i's `a` not in shared memory, 1 = a warp is copying it, 2 = there
+    int last_cta;        // this CTA is the last to leave the launch: it zeroes the barrier and readiness words
 };
 constexpr int kBlockSharedBytes = (sizeof(BlockShared) + 15) & ~15;
 
@@ -237,41 +275,120 @@ __device__ __forceinline__ void blk_select(int t) {
     __syncthreads();
 }
 
-// a (fp32 phase-1 output, written by all CTAs) -> Q8_K
+// Rows of entry `ie` (index into the work list) this CTA computes in gate/up: slice (blockIdx + ie) mod G of the G equal
+// slices of I.  Rotating the slice per entry keeps every CTA's total within one row of I * entries / G.
+__device__ __forceinline__ void entry_slice(int I, int ie, int& r0, int& len) {
+    const unsigned s = (blockIdx.x + (unsigned)ie) % gridDim.x;
+    r0 = (int)((unsigned long long)I * s / gridDim.x);
+    len = (int)((unsigned long long)I * (s + 1) / gridDim.x) - r0;
+}
+
+// `inter` of the block kernel (ktb200_moe::blk_inter) holds kInterEmpty wherever gate/up has not stored a value yet: a
+// consumer sees each value arrive on its own, so the producers store without any fence or count.  The bits are a NaN
+// that arithmetic never produces (a NaN result is the canonical 0x7fffffff).
+constexpr unsigned kInterEmpty = 0xffffffffu;
+__device__ __forceinline__ void st_relaxed_f32(float* p, float v) {
+    asm volatile("st.relaxed.gpu.global.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
+}
+__device__ __forceinline__ uint4 ld_relaxed_u4(const void* p) {
+    uint4 v;
+    asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
+    return v;
+}
+
+// Q8_K block `gb` (readiness word index), already claimed by this warp (ready 0 -> 1): wait until its QK_K values in
+// `src` have all arrived, quantise them in exactly the layout of the shared-memory staging, empty them again for the next
+// launch and publish the result (ready 2).  Whole warp.
 template <int KBS>
-__device__ __forceinline__ void blk_quantize_a(int t) {
-    extern __shared__ __align__(16) uint8_t smem[];
-    const BlockShared& sh = *reinterpret_cast<const BlockShared*>(smem);
-    const BlockParams& p = sh.prm;
-    const BlockLay L = block_layout<KBS>(p, smem);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, W = blockDim.x >> 5;
-    const int k = p.k, nb = p.I / QK_K, ns = k + (p.s_gate ? 1 : 0);
-    const unsigned skip = sh.skip;
-    const int totalb = ns * nb;
-    // block gb = (slot r, block b of its row); `inter` was written by other SMs in this launch: read at L2
-    auto fetch = [&](int gb, float (&x)[8]) -> bool {
-        const int r = gb / nb, b = gb - r * nb;
-        if (r != k && ((skip >> r) & 1u)) return false;
-        const float4* src = reinterpret_cast<const float4*>(p.inter + ((long)t * ns + r) * p.I + (long)b * QK_K + lane * 8);
-        const float4 v0 = __ldcg(src), v1 = __ldcg(src + 1);
-        x[0] = v0.x; x[1] = v0.y; x[2] = v0.z; x[3] = v0.w; x[4] = v1.x; x[5] = v1.y; x[6] = v1.z; x[7] = v1.w;
-        return true;
-    };
-    float cur[8], nxt[8];
-    int gb = warp;
-    bool live = gb < totalb && fetch(gb, cur);
-#pragma unroll 1
-    while (gb < totalb) {
-        const int gn = gb + W;
-        const bool nlive = gn < totalb && fetch(gn, nxt);
-        if (live)
-            warp_quantize_q8k_block(cur, lane, reinterpret_cast<uint32_t*>(L.aq + (size_t)gb * kActBlkStride), L.adx + gb,
-                                    KBS == 16 ? L.abs_ + gb * 16 : nullptr, KBS == 8 ? L.abs_ + gb * 8 : nullptr);
-#pragma unroll
-        for (int i = 0; i < 8; i++) cur[i] = nxt[i];
-        gb = gn;
-        live = nlive;
+__device__ __forceinline__ void quantise_block(const BlockParams& p, long gb, float* src) {
+    const int lane = threadIdx.x & 31;
+    uint4 v0, v1;
+    unsigned long long t0 = 0;
+    for (unsigned spins = 1;; spins++) {
+        v0 = ld_relaxed_u4(src + lane * 8);
+        v1 = ld_relaxed_u4(src + lane * 8 + 4);
+        const bool here = v0.x != kInterEmpty && v0.y != kInterEmpty && v0.z != kInterEmpty && v0.w != kInterEmpty &&
+                          v1.x != kInterEmpty && v1.y != kInterEmpty && v1.z != kInterEmpty && v1.w != kInterEmpty;
+        if (__all_sync(0xffffffffu, here)) break;
+        if ((spins & 255u) == 0) {   // bounded like wait_ge
+            const unsigned long long t = ep_now();
+            if (!t0) t0 = t;
+            else if (t - t0 > kEpTimeoutNs) { if (lane == 0) *p.status = 1; break; }
+        }
     }
+    const float x[8] = {__uint_as_float(v0.x), __uint_as_float(v0.y), __uint_as_float(v0.z), __uint_as_float(v0.w),
+                        __uint_as_float(v1.x), __uint_as_float(v1.y), __uint_as_float(v1.z), __uint_as_float(v1.w)};
+    warp_quantize_q8k_block(x, lane, reinterpret_cast<uint32_t*>(p.stage_q + gb * QK_K), p.stage_d + gb,
+                            KBS == 16 ? p.stage_bs + gb * 16 : nullptr, KBS == 8 ? p.stage_bs + gb * 8 : nullptr);
+    const uint4 empty = make_uint4(kInterEmpty, kInterEmpty, kInterEmpty, kInterEmpty);
+    reinterpret_cast<uint4*>(src + lane * 8)[0] = empty;
+    reinterpret_cast<uint4*>(src + lane * 8)[1] = empty;
+    __syncwarp();
+    if (lane == 0) {
+        __threadfence();
+        atomicExch(p.ready + gb, 2u);
+    }
+}
+
+// Every Q8_K block of (token t, slot) is quantised once per launch, by whichever CTA claims it first.  The warp claims the
+// blocks no CTA has claimed yet, one at a time, preferring a different block in every CTA so that the CTAs arriving
+// together quantise the blocks of an entry in parallel.  Returns when every block is claimed.  Whole warp.
+template <int KBS>
+__device__ __forceinline__ void claim_entry(const BlockParams& p, int t, int slot) {
+    const int lane = threadIdx.x & 31, ns = p.k + (p.s_gate ? 1 : 0), nb = p.I / QK_K;
+    const long g0 = ((long)t * ns + slot) * nb;
+    for (int c0 = 0; c0 < nb; c0 += 32) {
+        const int nc = min(32, nb - c0), rot = (int)(blockIdx.x % nc);
+        for (;;) {
+            const unsigned fr = __ballot_sync(0xffffffffu, lane < nc && ld_acquire_u32(p.ready + g0 + c0 + lane) == 0u);
+            if (!fr) break;
+            const unsigned pref = fr & (~0u << rot);
+            const int b = c0 + __ffs(pref ? pref : fr) - 1;
+            unsigned won = 0;
+            if (lane == 0) won = atomicCAS(p.ready + g0 + b, 0u, 1u) == 0u;
+            if (__shfl_sync(0xffffffffu, won, 0)) quantise_block<KBS>(p, g0 + b, p.inter + ((long)t * ns + slot) * p.I + (long)b * QK_K);
+        }
+    }
+}
+
+// Down: entry `ev`'s quantised `a` must be in region A before the first tile of it.  The first warp of the CTA to get here
+// waits until every block of the entry is staged and copies it (plain L2 loads: the staging was written in this
+// launch); with `need`, a warp that finds another warp doing it waits for that warp, without it returns at once (a
+// look-ahead).  Whole warp.
+template <int KBS>
+__device__ __forceinline__ void entry_to_smem(BlockShared& sh, const BlockLay& L, int t, int ev, bool need) {
+    const BlockParams& p = sh.prm;
+    const int lane = threadIdx.x & 31;
+    volatile int* state = &sh.ent_state[ev];
+    int s = lane == 0 ? *state : 0;
+    s = __shfl_sync(0xffffffffu, s, 0);
+    if (s == 0) {
+        if (lane == 0) s = atomicCAS(&sh.ent_state[ev], 0, 1) == 0 ? 3 : 1;
+        s = __shfl_sync(0xffffffffu, s, 0);
+    }
+    if (s == 3) {   // this warp claimed the copy
+        const int nb = p.I / QK_K, slot = sh.vs[ev];
+        const long g0 = ((long)t * (p.k + (p.s_gate ? 1 : 0)) + slot) * nb;
+        for (int b = lane; b < nb; b += 32) wait_ge<false>(p.ready + g0 + b, 2u, p.status);
+        __syncwarp();
+        const uint4* q = reinterpret_cast<const uint4*>(p.stage_q + g0 * QK_K);
+        for (int i = lane; i < nb * (QK_K / 16); i += 32)
+            *reinterpret_cast<uint4*>(L.aq + (size_t)(slot * nb + i / (QK_K / 16)) * kActBlkStride + (i % (QK_K / 16)) * 16) = __ldcg(q + i);
+        const uint4* bs = reinterpret_cast<const uint4*>(p.stage_bs + g0 * KBS);
+        for (int i = lane; i < nb * KBS / 8; i += 32) reinterpret_cast<uint4*>(L.abs_ + slot * nb * KBS)[i] = __ldcg(bs + i);
+        for (int i = lane; i < nb; i += 32) L.adx[slot * nb + i] = __ldcg(p.stage_d + g0 + i);
+        __syncwarp();
+        if (lane == 0) {
+            __threadfence_block();
+            *state = 2;
+            if (ev == 0) trace_stamp(p, 6);
+            if (ev == sh.nv - 1) trace_stamp(p, 7);
+        }
+    } else if (s == 1 && need && lane == 0) {
+        while (*state != 2) {}   // bounded: the copying warp's own waits are
+    }
+    if (lane == 0) __threadfence_block();
+    __syncwarp();
 }
 
 // weighted accumulation over the k experts IN expert_ids ORDER (moe.cpp:222-236), one FMA per expert; then the
@@ -337,20 +454,31 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
     __syncthreads();   // previous token: region A, partial and the work list are free (first token: barriers initialised)
     {
         // ------------------------------------------------------------ gate/up
-        // A warp walks a list of units (work-list entry, row) — 2 weight rows (gate, up) each.  Two lists per token:
-        //   S: the shared expert (entry 0), rows [ur0, ur0 + nr) of it, walked by warps 4.. WHILE warps 0..3 run the
-        //      top-k (the shared expert needs no routing);
-        //   R: the routed entries, all warps: the (entry, row) pairs of ALL routed entries form one global list that is
-        //      cut into equal contiguous ranges per CTA (+-1 unit) and dealt round-robin to the CTA's warps.
+        // A warp walks a list of units (work-list entry, row) — 2 weight rows (gate, up) each.  A CTA computes one slice of
+        // every entry (entry_slice); its list is the concatenation of those slices in entry order.  Two lists per token:
+        //   S: the shared expert (entry 0), its slice walked by warps 4.. WHILE warps 0..3 run the top-k (the shared
+        //      expert needs no routing);
+        //   R: the routed entries, all warps, dealt round-robin.  Every CTA walks the entries in the same order, so they
+        //      complete one after another across the grid and the down phase can start on the first while the last are
+        //      still being computed.
         const int nblk = p.H / QK_K, row_bytes = nblk * SZ_Q4_K;
         const int ns = k + (has_shared ? 1 : 0);
-        int ie = 0, ir = 0, ileft = 0, isub = 0;   // issue cursor (entry, row), units left to request, rows requested
-        int ce = 0, cr = 0, cleft = 0, csub = 0;   // consume cursor, units left to finish, rows consumed
-        int stride = W;
+        int ie = 0, ir = 0, ir0 = 0, ilen = 0, ileft = 0, isub = 0;   // issue cursor (entry, row, its slice), units left to request, rows requested
+        int ce = 0, cr = 0, cr0 = 0, clen = 0, cleft = 0, csub = 0;   // consume cursor, units left to finish, rows consumed
+        int stride = W, iend = 1;
         int slot_i = 0, slot_u = 0;
-        auto start_list = [&](int e0, int first_row, int count, int stride_) {   // first_row may exceed I: it wraps into the next entries
-            ie = e0 + first_row / p.I; ir = first_row - (first_row / p.I) * p.I;
-            ce = ie; cr = ir;
+        auto advance = [&](int& e, int& r, int& r0, int& len, int n) {   // n units further along the list
+            int off = r - r0 + n;
+            while (off >= len && e + 1 < iend) { off -= len; e++; entry_slice(p.I, e, r0, len); }
+            r = r0 + off;
+        };
+        auto start_list = [&](int e0, int e1, int first, int count, int stride_) {   // entries [e0, e1), from unit `first`
+            iend = e1;
+            ie = e0;
+            entry_slice(p.I, e0, ir0, ilen);
+            ir = ir0;
+            advance(ie, ir, ir0, ilen, first);
+            ce = ie; cr = ir; cr0 = ir0; clen = ilen;
             ileft = cleft = count > 0 ? count : 0;
             stride = stride_;
         };
@@ -373,20 +501,21 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
                 isub++;
                 if (!(isub & 1)) {
                     ileft--;
-                    ir += stride;
-                    while (ir >= p.I) { ir -= p.I; ie++; }
+                    advance(ie, ir, ir0, ilen, stride);
                 }
                 slot_i = (slot_i + 1 == SU) ? 0 : slot_i + 1;
             }
         };
+        if (threadIdx.x < 36) sh.ent_state[threadIdx.x] = 0;
         blk_router(t, waited);
         block_stamp(p, 2);
         grid_arrive(p.sync, gen);
         // while the barrier completes: request the shared expert's first rows, then quantise x (the router read x itself)
         if (has_shared && warp >= kGateWarps) {
-            const int ur0 = (int)((long)p.I * blockIdx.x / gridDim.x), nr = (int)((long)p.I * (blockIdx.x + 1) / gridDim.x) - ur0;
+            int r0, nr;
+            entry_slice(p.I, 0, r0, nr);
             const int first = warp - kGateWarps, st = W - kGateWarps;
-            start_list(0, ur0 + first, (nr - first + st - 1) / st, st);
+            start_list(0, 1, first, (nr - first + st - 1) / st, st);
         }
 #pragma unroll
         for (int s = 0; s < SU; s++)
@@ -403,10 +532,14 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
                 // list 0 (the shared expert) was consumed by warps 4.. while warps 0..3 run the top-k now
                 blk_select(t);
                 block_stamp(p, 4);
-                const int e0 = has_shared ? 1 : 0;
-                const long total = (long)(sh.nv - e0) * p.I;
-                const int u0 = (int)(total * blockIdx.x / gridDim.x), u1 = (int)(total * (blockIdx.x + 1) / gridDim.x);
-                start_list(e0, u0 + warp, (u1 - u0 - warp + W - 1) / W, W);
+                const int e0 = has_shared ? 1 : 0, nv = sh.nv;
+                int total = 0;
+                for (int e = e0; e < nv; e++) {
+                    int r0, len;
+                    entry_slice(p.I, e, r0, len);
+                    total += len;
+                }
+                start_list(e0, nv, warp, (total - warp + W - 1) / W, W);
 #pragma unroll
                 for (int s = 0; s < SU; s++) issue_u();
             }
@@ -430,13 +563,13 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
                     g += __shfl_xor_sync(0xffffffffu, g, o);
                     uu += __shfl_xor_sync(0xffffffffu, uu, o);
                 }
-                if (lane == 0) p.inter[((long)t * ns + sh.vs[ce]) * p.I + cr] = (p.use_silu ? act_silu(g) : act_relu(g)) * uu;
+                if (lane == 0) st_relaxed_f32(p.inter + ((long)t * ns + sh.vs[ce]) * p.I + cr, (p.use_silu ? act_silu(g) : act_relu(g)) * uu);
                 cleft--;
-                cr += stride;
-                while (cr >= p.I) { cr -= p.I; ce++; }
+                advance(ce, cr, cr0, clen, stride);
             }
         }
-        if (p.trace) { __syncthreads(); block_stamp(p, 5); }
+        __syncthreads();   // every warp's gate/up is done: region A (the x staging) is free for `a`
+        block_stamp(p, 5);
     }
     {
         // ------------------------------------------------------------ down: row quads [q0, q0 + nquads) of every entry
@@ -444,8 +577,9 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
         const int quads = p.H / RW;
         const int q0 = (int)((long)quads * blockIdx.x / gridDim.x), nquads = (int)((long)quads * (blockIdx.x + 1) / gridDim.x) - q0;
         const int nv = sh.nv;
-        int ni = nquads * nv - warp;
-        ni = ni > 0 ? (ni + W - 1) / W : 0;
+        const int Wd = W - 1;   // warps streaming tiles; warp W - 1 quantises this CTA's share of the Q8_K blocks
+        int ni = warp < Wd ? nquads * nv - warp : 0;
+        ni = ni > 0 ? (ni + Wd - 1) / Wd : 0;
         int dvi = 0, dq = 0, dss = 0, dcons = 0;   // issue cursor, tiles requested, tiles consumed
         if (ni > 0) { dvi = warp / nquads; dq = warp - dvi * nquads; }
         int evi = dvi, eq = dq;
@@ -463,21 +597,20 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
                     bulk_g2s(ring_u32 + dslot_i * item_bytes, wbase + (row >> 2) * item_bytes, (uint32_t)item_bytes, bar);
                 }
                 dss++;
-                dq += W;
+                dq += Wd;
                 while (dq >= nquads) { dq -= nquads; dvi++; }
                 dslot_i = (dslot_i + 1 == SD) ? 0 : dslot_i + 1;
             }
         };
-        grid_arrive(p.sync, gen);   // this CTA's rows of `inter` are written
-        // the first tiles depend on the expert ids only: they stream while the barrier completes and `a` is quantised
-#pragma unroll
-        for (int s = 0; s < SD; s++)
-            if (s < p.prime_d) issue_d();
-        grid_wait(p.sync, gen);     // every row of `inter` is written and visible
-        block_stamp(p, 6);
-        blk_quantize_a<DownFmt::kBs>(t);
+        // the tiles depend on the expert ids only: they stream while the first entry's `a` is fetched
 #pragma unroll
         for (int s = 0; s < SD; s++) issue_d();
+        const BlockLay L = block_layout<DownFmt::kBs>(p, smem);
+        if (warp == W - 1) {
+            // the quantisation this CTA contributes, in work-list order (this warp has no bulk copies in flight: its
+            // fences do not wait for any)
+            for (int ev = 0; ev < nv; ev++) claim_entry<DownFmt::kBs>(p, t, sh.vs[ev]);
+        }
         if (t == Teff - 1 && warp == W - 1) {
             // the next layer's first bytes (ktb200_moe_block_prefetch_hint) -> L2, this CTA's 1/grid slice of each range in
             // 4 KB pieces: no registers or shared memory held, the down stream keeps its ring
@@ -490,13 +623,14 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
                 }
             }
         }
-        __syncthreads();
-        block_stamp(p, 7);
 
-        const BlockLay L = block_layout<DownFmt::kBs>(p, smem);
         const uint8_t* ring = smem + (ring_u32 - (uint32_t)__cvta_generic_to_shared(smem));
         const int ns = k + (has_shared ? 1 : 0);
         for (int n = 0; n < ni; n++) {
+            if (eq < Wd) {   // this warp's first tile of entry evi; the next entry is copied ahead by whoever gets there first
+                entry_to_smem<DownFmt::kBs>(sh, L, t, evi, true);
+                if (evi + 1 < nv) entry_to_smem<DownFmt::kBs>(sh, L, t, evi + 1, false);
+            }
             mbar_wait(bar_u32 + 8 * dslot_u, (phase >> dslot_u) & 1u);
             phase ^= 1u << dslot_u;
             const uint8_t* sl = ring + dslot_u * item_bytes;
@@ -517,7 +651,7 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
             dcons++;
             issue_d();
             if ((lane & 7) == 0) L.partial[(eq * RW + (lane >> 3)) * ns + j] = res;
-            eq += W;
+            eq += Wd;
             while (eq >= nquads) { eq -= nquads; evi++; }
         }
         __syncthreads();
@@ -527,15 +661,19 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
     }
   }  // tokens
 
-    // leave the barrier words zeroed for the next launch / graph replay: the last CTA to get here resets them
+    // leave the barrier and readiness words zeroed for the next launch / graph replay: the last CTA to get here resets
+    // them (every other CTA has finished all its reads of them)
     __syncthreads();
-    if (threadIdx.x == 0) {
-        const unsigned prev = atomicAdd(p.sync + 1, 1u);
-        if (prev == gridDim.x - 1) {
+    if (threadIdx.x == 0) sh.last_cta = atomicAdd(p.sync + 1, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (sh.last_cta) {
+        const int nready = Teff * (k + (has_shared ? 1 : 0)) * (p.I / QK_K);
+        for (int i = threadIdx.x; i < nready; i += blockDim.x) p.ready[i] = 0;
+        if (threadIdx.x == 0) {
             p.sync[0] = 0;
             p.sync[1] = 0;
-            __threadfence();
         }
+        __threadfence();
     }
 }
 
@@ -559,7 +697,6 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
 // phase C, which needs every rank's phase-X stores, which come after that rank's reads of the messages.
 constexpr int kEpWorldMax = 8;
 constexpr int kEpPairsMax = 64;
-constexpr unsigned long long kEpTimeoutNs = 4000000000ull;
 
 struct EpExtra {
     int rank, world, phase_mask, pa;      // pa: entries per down chunk (activation staging capacity)
@@ -583,33 +720,11 @@ struct EpShared {
     int tok_slot[2];                      // which tokens' activations sit in the two x staging slots (phase X)
 };
 
-__device__ __forceinline__ unsigned ld_acquire_sys_u32(const unsigned* p) {
-    unsigned v;
-    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
 __device__ __forceinline__ void st_release_sys_u32(unsigned* p, unsigned v) {
     asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ void red_release_sys_add(unsigned* p, unsigned v) {
     asm volatile("red.release.sys.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ unsigned long long ep_now() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-// spin until *p - target >= 0 (wrap-safe); gives up after kEpTimeoutNs and records it in `status`
-__device__ __forceinline__ void ep_wait_ge(const unsigned* p, unsigned target, unsigned* status) {
-    unsigned long long t0 = 0;
-    unsigned spins = 0;
-    while ((int)(ld_acquire_sys_u32(p) - target) < 0) {
-        if ((++spins & 1023u) == 0) {
-            const unsigned long long t = ep_now();
-            if (!t0) t0 = t;
-            else if (t - t0 > kEpTimeoutNs) { *status = 1; break; }
-        }
-    }
 }
 
 // one token row (hidden type, read at L2: it was written by a peer) -> Q8_K in staging slot `slot`
@@ -804,7 +919,7 @@ __global__ void __launch_bounds__(kBlockWarpsLo * 32, 1) moe_ep_block_kernel(con
 
     // =============================================================================================== phase X
     if (mask & 2) {
-        if ((int)threadIdx.x < world) ep_wait_ge(my_flags + threadIdx.x, epoch, status);
+        if ((int)threadIdx.x < world) wait_ge<true>(my_flags + threadIdx.x, epoch, status);
         __syncthreads();
         block_stamp(p, 5);
         const uint8_t* mymsg = pp.x.msg[rank];
@@ -959,7 +1074,7 @@ __global__ void __launch_bounds__(kBlockWarpsLo * 32, 1) moe_ep_block_kernel(con
 
     // =============================================================================================== phase C
     if (mask & 4) {
-        if ((int)threadIdx.x < world) ep_wait_ge(my_flags + world + threadIdx.x, epoch * gridDim.x, status);
+        if ((int)threadIdx.x < world) wait_ge<true>(my_flags + world + threadIdx.x, epoch * gridDim.x, status);
         __syncthreads();
         block_stamp(p, 9);
         const float* mine = pp.x.part[rank];
@@ -1066,11 +1181,16 @@ extern "C" int ktb200_moe_block_forward(const ktb200_gate_config* gc, ktb200_moe
     p.s_gate = sh ? sh->gate : nullptr; p.s_up = sh ? sh->up : nullptr; p.s_down = sh ? sh->down : nullptr;
     p.n_local = c.expert_num; p.id_offset = c.expert_id_offset;
     p.H = c.hidden_size; p.I = c.intermediate_size; p.k = k; p.hidden_type = c.hidden_type; p.use_silu = c.use_silu;
-    p.inter = m->inter; p.out = output; p.sync = m->blk_sync + 2 * (m->blk_flip++ & 1u); p.trace = g_btrace;
+    const unsigned flip = m->blk_flip++ & 1u;
+    p.inter = m->blk_inter; p.out = output; p.sync = m->blk_sync + 2 * flip; p.trace = g_btrace;
+    p.status = m->blk_sync + kBlkStatusWord;
+    p.ready = m->blk_sync + kBlkReadyWord + flip * blk_ready_words(c);
+    p.stage_q = m->blk_stage;
+    p.stage_bs = reinterpret_cast<int16_t*>(m->blk_stage + blk_ready_words(c) * (size_t)QK_K);
+    p.stage_d = reinterpret_cast<float*>(m->blk_stage + blk_ready_words(c) * (size_t)(QK_K + 32));
     for (int r = 0; r < 3; r++) { p.pf[r] = (const uint8_t*)m->pf[r]; p.pf_bytes[r] = (unsigned)m->pf_bytes[r]; }
     static const int prime_u = [] { const char* e = getenv("KTB200_BLK_PRIME_U"); return e ? atoi(e) : 3; }();
-    static const int prime_d = [] { const char* e = getenv("KTB200_BLK_PRIME_D"); return e ? atoi(e) : 2; }();
-    p.prime_u = prime_u; p.prime_d = prime_d;
+    p.prime_u = prime_u;
 
     void* args[] = {&p};
     const void* fn;
@@ -1283,3 +1403,17 @@ extern "C" int ktb200_moe_block_forward_host(const ktb200_gate_config* gc, ktb20
 // Diagnostics (profiles/block_trace.py): when set, thread 0 of every CTA of the following ktb200_moe_block_forward
 // launches writes %globaltimer at the phase boundaries into trace[cta][16] (device memory, >= num_SMs*16 u64).
 extern "C" void ktb200_debug_block_trace(unsigned long long* trace_dev) { g_btrace = trace_dev; }
+
+extern "C" long ktb200_debug_block_sync_words(ktb200_moe* m, unsigned* host_out, long n) {
+    if (!m) { set_error("null handle"); return -1; }
+    const long total = (long)(kBlkReadyWord + 2 * blk_ready_words(m->cfg));
+    DeviceGuard guard(m->device);
+    if (host_out && n > 0) {
+        if (cudaDeviceSynchronize() != cudaSuccess ||
+            cudaMemcpy(host_out, m->blk_sync, (size_t)(n < total ? n : total) * sizeof(unsigned), cudaMemcpyDeviceToHost) != cudaSuccess) {
+            set_error("debug_block_sync_words: %s", cudaGetErrorString(cudaGetLastError()));
+            return -1;
+        }
+    }
+    return total;
+}

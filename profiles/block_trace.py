@@ -35,7 +35,7 @@ ids = torch.zeros(1, K, dtype=torch.int64, device="cuda"); wts = torch.zeros(1, 
 n_sm = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count   # one CTA per SM
 trace = torch.zeros(n_sm * 16, dtype=torch.int64, device="cuda")
 names = ["start", "x quantised (under barrier 1)", "router partials written", "grid barrier 1 passed", "top-k selected",
-         "gate/up done (CTA)", "grid barrier 2 passed", "a quantised", "down tiles done (CTA)", "combined + stored",
+         "gate/up done (CTA)", "entry 0 ready (its a in smem)", "last entry ready (its a in smem)", "down tiles done (CTA)", "combined + stored",
          "  (top-k done, before the work-list build)"]
 acc = []
 for rep in range(12):
