@@ -36,6 +36,14 @@ enum ktb200_ggml_type {
     KTB200_TYPE_F32 = 0, KTB200_TYPE_F16 = 1, KTB200_TYPE_Q8_0 = 8, KTB200_TYPE_Q2_K = 10,
     KTB200_TYPE_Q3_K = 11, KTB200_TYPE_Q4_K = 12, KTB200_TYPE_Q5_K = 13, KTB200_TYPE_Q6_K = 14,
     KTB200_TYPE_Q8_K = 15, KTB200_TYPE_IQ4_XS = 23, KTB200_TYPE_BF16 = 30,
+    /* ggml's codebook i-quants (DeepSeek-R1's 1.5-2-bit GGUF experts), raw ggml blocks of 256 values:
+     *   IQ2_XXS  66 B: fp16 d, then per 32-value sub-block two 32-bit words: four 8-bit indices into iq2xxs_grid, then
+     *            four 7-bit indices into ksigns_iq2xs and the 4-bit scale s in bits 28..31; value = d*(2s+1)/8 * grid * sign
+     *   IQ1_S    50 B: fp16 d, qs[32], qh uint16[8]; sub-block ib has ls = 2*((qh>>12)&7)+1, delta = qh bit 15 ? -1/8 : +1/8,
+     *            group l = iq1s_grid[qs[4ib+l] | ((qh >> 3l) & 7) << 8]; value = d*ls*(grid + delta)
+     * vec_dot_type Q8_K.  Routed experts only (ktb200_moe_create, any mix with the K-quants); linears, MLP handles and the
+     * expert-parallel entry points reject them.  The codebooks are ktransformers_b200/csrc/iq_tables.h. */
+    KTB200_TYPE_IQ2_XXS = 16, KTB200_TYPE_IQ1_S = 19,
     /* Not a ggml type: ggml's ids stay below 64, so 256 cannot collide with one.
      * Symmetric INT4 in groups of 32 with bf16 scales (compressed-tensors "pack-quantized", kt-kernel's RAWINT4; Kimi-K2's
      * routed experts), in the device layout ktb200_rawint4_pack writes: 144 B per 256 values of a row,

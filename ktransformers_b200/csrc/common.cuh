@@ -16,6 +16,8 @@
 #define SZ_Q6_K 210
 #define SZ_Q8_K 292
 #define SZ_IQ4_XS 136
+#define SZ_IQ2_XXS 66    // fp16 d + 8 x (4 grid indices | signs + scale) words
+#define SZ_IQ1_S 50      // fp16 d + qs[32] + qh[8] (uint16)
 #define SZ_RAWINT4 144   // 8 bf16 scales + 256 nibbles (rawint4.cuh)
 
 namespace ktb {
@@ -87,6 +89,16 @@ __host__ __device__ inline bool is_kquant(int t) {
     return t == KTB200_TYPE_Q2_K || t == KTB200_TYPE_Q3_K || t == KTB200_TYPE_Q4_K || t == KTB200_TYPE_Q5_K ||
            t == KTB200_TYPE_Q6_K || t == KTB200_TYPE_IQ4_XS;
 }
+// codebook i-quants: routed experts only (iq.cuh bulk kernels, generic per-pair fallback), no linear /
+// MLP / grouped / block / expert-parallel path
+__host__ __device__ inline bool is_iquant(int t) { return t == KTB200_TYPE_IQ2_XXS || t == KTB200_TYPE_IQ1_S; }
+static inline const char* iquant_name(int t) { return t == KTB200_TYPE_IQ1_S ? "IQ1_S" : t == KTB200_TYPE_IQ2_XXS ? "IQ2_XXS" : "?"; }
+// block geometry including the i-quants.  Kept apart from type_size / blck_size, which every kernel inlines for its hidden
+// type: a longer switch there would change the code of kernels that never see an i-quant.
+__host__ __device__ inline long weight_block_bytes(int t) {
+    return t == KTB200_TYPE_IQ2_XXS ? SZ_IQ2_XXS : t == KTB200_TYPE_IQ1_S ? SZ_IQ1_S : type_size(t);
+}
+__host__ __device__ inline long weight_block_elems(int t) { return is_iquant(t) ? QK_K : blck_size(t); }
 // not a K-quant: it has its own kernels (rawint4.cuh) and no path through the generic K-quant ones
 __host__ __device__ inline bool is_rawint4(int t) { return t == KTB200_TYPE_RAWINT4_G32; }
 __host__ __device__ inline bool is_hidden_type(int t) {

@@ -3,6 +3,7 @@
 // loads).  Here one thread owns one 16-element group, so a warp covers two super-blocks with
 // contiguous 32-byte stores per lane; value = fma(d*sc, q, -(dmin*m)) in fp32, then cast — the same
 // expression the reference kernels evaluate (dequant.cu:343-413 for Q4_K, 502-595 for Q6_K).
+#define KTB_IQ_CODEBOOKS
 #include "formats.cuh"
 
 namespace ktb {
@@ -68,11 +69,11 @@ static int dequant_to(const void* src, int type, long n, OutT* out, cudaStream_t
         long blocks = (n + 255) / 256;
         if (blocks > max_blocks) blocks = max_blocks;
         dequant_q8_0_kernel<OutT><<<(unsigned)blocks, 256, 0, s>>>(reinterpret_cast<const uint8_t*>(src), n, out);
-    } else if (is_kquant(type)) {
+    } else if (is_kquant(type) || is_iquant(type)) {
         const long ng = n / 16;
         long blocks = (ng + 255) / 256;
         if (blocks > max_blocks) blocks = max_blocks;
-        dequant_k_kernel<OutT><<<(unsigned)blocks, 256, 0, s>>>(reinterpret_cast<const uint8_t*>(src), type, (int)type_size(type), ng, out);
+        dequant_k_kernel<OutT><<<(unsigned)blocks, 256, 0, s>>>(reinterpret_cast<const uint8_t*>(src), type, (int)weight_block_bytes(type), ng, out);
     } else if (is_rawint4(type)) {
         long blocks = (n / 8 + 255) / 256;
         if (blocks > max_blocks) blocks = max_blocks;
@@ -97,7 +98,7 @@ extern "C" int ktb200_dequantize(const void* src, int type, long n, void* out, i
     using namespace ktb;
     if (!src || !out) { set_error("null pointer"); return KTB200_EINVAL; }
     if (n <= 0) return KTB200_OK;
-    const long blk = blck_size(type);
+    const long blk = weight_block_elems(type);
     if (blk == 0 || n % blk) { set_error("dequantize: n=%ld is not a multiple of the block size of type %d", n, type); return KTB200_EINVAL; }
     cudaStream_t s = (cudaStream_t)stream;
     switch (out_type) {

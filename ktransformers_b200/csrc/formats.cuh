@@ -13,9 +13,17 @@
 //   FmtQ4K    raw GGUF block_q4_K (144 B, already 16-byte aligned)   unit = 16 B of qs = 32 weights, 4 blocks/step
 //   FmtQ5K    raw GGUF block_q5_K (176 B, 16-byte aligned)           unit = 16 B qs + qh   = 32 weights, 4 blocks/step
 //   FmtQ6K8   block_q6_K re-laid as "8-row SoA" (moe.cu repack)      unit = 48 B           = 64 weights, 8 blocks/step
-//   FmtGenK   any raw K-quant / IQ4_XS through byte loads (fallback) unit = 16 weights,              2 blocks/step
+//   FmtGenK   any raw K-quant / IQ4_XS / IQ2_XXS / IQ1_S through byte loads (fallback)
+//                                                                    unit = 16 weights,              2 blocks/step
 #pragma once
 #include "common.cuh"
+
+// The IQ1_S / IQ2_XXS codebooks (device globals) only exist in the translation units that dispatch those types
+// (moe.cu, dequant.cu define KTB_IQ_CODEBOOKS); elsewhere unpack_group16 has no IQ cases and no table is emitted.
+#ifdef KTB_IQ_CODEBOOKS
+#define KTB_IQ_TABLE static __device__ const
+#include "iq_tables.h"
+#endif
 
 namespace ktb {
 
@@ -400,6 +408,38 @@ __device__ inline void unpack_group16(int type, const uint8_t* b, int g, GroupK&
             for (int l = 0; l < 16; l++) v[l] = c_kvalues_iq4nl[half ? (ldg_u8(qs + l) >> 4) : (ldg_u8(qs + l) & 0xf)];
             break;
         }
+#ifdef KTB_IQ_CODEBOOKS
+        case KTB200_TYPE_IQ1_S: {
+            // values held as 8*grid + delta (-9..9) with d/8: the dot's fp32 term is the reference's (d*dx)*(S/8) exactly
+            o.d = fp16_bits_to_f32(ldg_u16(b)) * 0.125f;
+            const int ib = g >> 1, l0 = 2 * (g & 1);
+            const uint32_t qh = ldg_u16(b + 34 + 2 * ib);
+            o.isc = 2 * (int)((qh >> 12) & 7) + 1;
+            const int delta = (qh & 0x8000u) ? -1 : 1;
+            for (int l = 0; l < 2; l++) {
+                const int idx = ldg_u8(b + 2 + 4 * ib + l0 + l) | (int)(((qh >> (3 * (l0 + l))) & 7) << 8);
+                for (int j = 0; j < 8; j++) v[8 * l + j] = (int8_t)(8 * (int)(int8_t)ldg_u8(&ktb_iq1s_grid[idx][j]) + delta);
+            }
+            break;
+        }
+        case KTB200_TYPE_IQ2_XXS: {
+            // d/8 and ls = 2s+1: the reference's final 0.125 folded into the scale (exact, a power of two)
+            o.d = fp16_bits_to_f32(ldg_u16(b)) * 0.125f;
+            const int ib = g >> 1, l0 = 2 * (g & 1);
+            const uint8_t* q = b + 2 + 8 * ib;
+            const uint32_t aux1 = (uint32_t)ldg_u16(q + 4) | ((uint32_t)ldg_u16(q + 6) << 16);
+            o.isc = 2 * (int)(aux1 >> 28) + 1;
+            for (int l = 0; l < 2; l++) {
+                const int idx = ldg_u8(q + l0 + l);
+                const uint32_t signs = ldg_u8(&ktb_ksigns_iq2xs[(aux1 >> (7 * (l0 + l))) & 127]);
+                for (int j = 0; j < 8; j++) {
+                    const int gv = ldg_u8(&ktb_iq2xxs_grid[idx][j]);
+                    v[8 * l + j] = (int8_t)(((signs >> j) & 1) ? -gv : gv);
+                }
+            }
+            break;
+        }
+#endif
         default:
             o.d = 0.f; o.isc = 0;
             for (int l = 0; l < 16; l++) v[l] = 0;
@@ -420,7 +460,7 @@ struct FmtGenK {
 
     __device__ static __forceinline__ Lane lane(int l) { return Lane{l >> 4, l & 15}; }
     __device__ static __forceinline__ Row row(const void* base, long row_idx, int ncols, int type) {
-        const int bsz = (int)type_size(type);
+        const int bsz = (int)weight_block_bytes(type);
         return Row{reinterpret_cast<const uint8_t*>(base) + row_idx * (long)(ncols / QK_K) * bsz, type, bsz};
     }
     __device__ static __forceinline__ void prefetch(const Row&, int) {}

@@ -253,6 +253,8 @@ __global__ void __launch_bounds__(kBulkMaxWarps * 32, 1) rows_bulk_q4k_kernel(co
 struct BulkQ4K {   // raw Q4_K rows: block f of the item at f*144
     static constexpr int kBlockBytes = SZ_Q4_K;
     static constexpr int kBs = 8;   // int16 activation sums per block (32-value groups)
+    static constexpr int kTableBytes = 0;   // static shared memory of the format's tables (iq.cuh)
+    __device__ static __forceinline__ void stage_tables() {}
     __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int /*nrb*/, const uint8_t* aq, const int16_t* bs, float dxb) {
         return q4k_block_dot(sl + f * SZ_Q4_K, aq, *reinterpret_cast<const uint4*>(bs), dxb);
     }
@@ -261,6 +263,8 @@ struct BulkQ4K {   // raw Q4_K rows: block f of the item at f*144
 struct BulkQ6K4T {   // chunk-major 4-row tiles (see the header comment)
     static constexpr int kBlockBytes = SZ_Q6_K;
     static constexpr int kBs = 16;  // int16 activation sums per block (16-value groups)
+    static constexpr int kTableBytes = 0;
+    __device__ static __forceinline__ void stage_tables() {}
     __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int nrb, const uint8_t* aq, const int16_t* bs, float dxb) {
         const uint8_t* ql = sl + f * 16;                  // chunk c at ql + c*nrb*16
         const uint8_t* qh = sl + nrb * 128 + f * 16;      // chunk c at qh + c*nrb*16
@@ -330,6 +334,7 @@ __global__ void __launch_bounds__(kBulkMaxWarpsDown * 32, 1) reduce_bulk_kernel(
     __shared__ int s_np, s_nt;
     __shared__ int s_first[kBulkMaxChunkTokens + 1];   // first pair of every token of the chunk (+ end)
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, W = blockDim.x >> 5;
+    Fmt::stage_tables();   // codebooks of the IQ formats; read only after the token loop's first __syncthreads
     int Teff = p.ntokens;
     if (p.bsz) Teff = min(Teff, *p.bsz);
     const int nb = p.ncols / QK_K;

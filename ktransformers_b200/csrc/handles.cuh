@@ -13,7 +13,7 @@ static inline FmtId pick_fmt(int type, int layout) {
     if (type == KTB200_TYPE_Q5_K) return FMT_Q5K;
     if (type == KTB200_TYPE_Q6_K && layout == LAYOUT_SOA8) return FMT_Q6K8;
     if (type == KTB200_TYPE_Q6_K && layout == LAYOUT_T4) return FMT_Q6K4T;
-    if (is_kquant(type)) return FMT_GENK;
+    if (is_kquant(type) || is_iquant(type)) return FMT_GENK;
     if (is_rawint4(type)) return FMT_RAWINT4;
     return FMT_NONE;
 }

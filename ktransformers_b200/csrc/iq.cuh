@@ -1,0 +1,250 @@
+// IQ1_S and IQ2_XXS routed experts on the bulk-copy ring (gemv_bulk.cuh): one lane per super-block, codebooks in shared
+// memory.
+//
+//   * down: item formats BulkIQ1S / BulkIQ2XXS of reduce_bulk_kernel — 4 rows x nb raw ggml blocks, one bulk copy
+//     (4 * nb * 50 B / 4 * nb * 66 B, a multiple of 16 when nb is even; 1600 B / 2112 B at I = 2048 = one block per lane);
+//   * gate/up: rows_bulk_iq_kernel.  A row is nblk * 50 B (IQ1_S) or nblk * 66 B (IQ2_XXS): 1400 B / 1848 B at H = 7168,
+//     not a multiple of 16, so a single row cannot be one bulk copy.  The unit is two consecutive rows (2800 B / 3696 B,
+//     16-byte aligned when nblk % 4 == 0): one ring slot holds the gate rows 2r, 2r+1 and the up rows 2r, 2r+1 (two copies
+//     on one mbarrier), so one read of x serves both matrices and the raw GGUF bytes are used as they are.
+//
+// Codebooks: IQ1_S's 2048 x 8 int8 grid as 16 KB of uint2 (one LDS.64 per 8 values, no unpacking); IQ2_XXS's 256 x 8
+// grid (2 KB) and its 128 sign patterns expanded to byte masks (1 KB: value = (g ^ m) - m per byte).  Both are copied from
+// the device tables of iq_tables.h once per CTA.
+//
+// Arithmetic (DESIGN.md §2): IQ1_S  S = sum_ib ls * (8 * sum grid * q8 + delta * bsum32) and term = ((d/8) * dx) * S;
+// IQ2_XXS  term = ((d/8) * dx) * sum_ib ls * sum (+-grid) * q8.  Both equal the reference's per-super-block fp32 terms.
+#pragma once
+#include "gemv_bulk.cuh"
+
+namespace ktb {
+
+__device__ __forceinline__ uint2* iq1s_grid_smem() { __shared__ uint2 t[2048]; return t; }
+__device__ __forceinline__ uint2* iq2xxs_grid_smem() { __shared__ uint2 t[256]; return t; }
+__device__ __forceinline__ uint2* iq2xxs_signs_smem() { __shared__ uint2 t[128]; return t; }
+
+// 32 bits from a 2-byte aligned shared-memory address
+__device__ __forceinline__ uint32_t lds_u32_a2(const uint8_t* p) {
+    const uint16_t* h = reinterpret_cast<const uint16_t*>(p);
+    return (uint32_t)h[0] | ((uint32_t)h[1] << 16);
+}
+
+struct BulkIQ1S {
+    static constexpr int kType = KTB200_TYPE_IQ1_S;
+    static constexpr int kBlockBytes = SZ_IQ1_S;
+    static constexpr int kBs = 8;            // int16 activation sums per block (32-value groups)
+    static constexpr int kTableBytes = 2048 * 8;
+    __device__ static __forceinline__ void stage_tables() {
+        uint2* g = iq1s_grid_smem();
+        for (int i = threadIdx.x; i < 2048; i += blockDim.x) g[i] = *reinterpret_cast<const uint2*>(ktb_iq1s_grid[i]);
+    }
+    // one super-block at `wb` (shared memory, 2-byte aligned) against one padded int8 activation block
+    __device__ static __forceinline__ float block_dot(const uint8_t* wb, const uint8_t* aq, const int16_t* bs32, float dxb) {
+        const uint2* grid = iq1s_grid_smem();
+        const float d = fp16_bits_to_f32(*reinterpret_cast<const uint16_t*>(wb)) * 0.125f;
+        int isum = 0;
+#pragma unroll
+        for (int ib = 0; ib < 8; ib++) {
+            const uint32_t qh = *reinterpret_cast<const uint16_t*>(wb + 34 + 2 * ib);
+            const uint32_t qs = lds_u32_a2(wb + 2 + 4 * ib);
+            const uint4 a0 = *reinterpret_cast<const uint4*>(aq + 32 * ib);
+            const uint4 a1 = *reinterpret_cast<const uint4*>(aq + 32 * ib + 16);
+            const uint2 g0 = grid[(qs & 0xff) | ((qh << 8) & 0x700)];
+            const uint2 g1 = grid[((qs >> 8) & 0xff) | ((qh << 5) & 0x700)];
+            const uint2 g2 = grid[((qs >> 16) & 0xff) | ((qh << 2) & 0x700)];
+            const uint2 g3 = grid[(qs >> 24) | ((qh >> 1) & 0x700)];
+            int s = dp4a_s8s8(g0.x, a0.x, 0);
+            s = dp4a_s8s8(g0.y, a0.y, s);
+            s = dp4a_s8s8(g1.x, a0.z, s);
+            s = dp4a_s8s8(g1.y, a0.w, s);
+            s = dp4a_s8s8(g2.x, a1.x, s);
+            s = dp4a_s8s8(g2.y, a1.y, s);
+            s = dp4a_s8s8(g3.x, a1.z, s);
+            s = dp4a_s8s8(g3.y, a1.w, s);
+            const int b = bs32[ib];
+            const int ls = 2 * (int)((qh >> 12) & 7) + 1;
+            isum += ls * (8 * s + ((qh & 0x8000u) ? -b : b));
+        }
+        return (d * dxb) * (float)isum;
+    }
+    __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int /*nrb*/, const uint8_t* aq, const int16_t* bs, float dxb) {
+        return block_dot(sl + f * SZ_IQ1_S, aq, bs, dxb);
+    }
+};
+
+struct BulkIQ2XXS {
+    static constexpr int kType = KTB200_TYPE_IQ2_XXS;
+    static constexpr int kBlockBytes = SZ_IQ2_XXS;
+    static constexpr int kBs = 8;
+    static constexpr int kTableBytes = 256 * 8 + 128 * 8;
+    __device__ static __forceinline__ void stage_tables() {
+        uint2* g = iq2xxs_grid_smem();
+        uint2* m = iq2xxs_signs_smem();
+        for (int i = threadIdx.x; i < 256; i += blockDim.x) g[i] = *reinterpret_cast<const uint2*>(ktb_iq2xxs_grid[i]);
+        for (int i = threadIdx.x; i < 128; i += blockDim.x) {
+            const uint32_t s = ktb_ksigns_iq2xs[i];
+            uint32_t lo = 0, hi = 0;
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                lo |= ((s >> j) & 1u) ? 0xffu << (8 * j) : 0u;
+                hi |= ((s >> (j + 4)) & 1u) ? 0xffu << (8 * j) : 0u;
+            }
+            m[i] = make_uint2(lo, hi);
+        }
+    }
+    __device__ static __forceinline__ float block_dot(const uint8_t* wb, const uint8_t* aq, const int16_t* /*bs32*/, float dxb) {
+        const uint2* grid = iq2xxs_grid_smem();
+        const uint2* sgn = iq2xxs_signs_smem();
+        const float d = fp16_bits_to_f32(*reinterpret_cast<const uint16_t*>(wb)) * 0.125f;
+        int isum = 0;
+#pragma unroll
+        for (int ib = 0; ib < 8; ib++) {
+            const uint32_t aux0 = lds_u32_a2(wb + 2 + 8 * ib), aux1 = lds_u32_a2(wb + 6 + 8 * ib);
+            const uint4 a0 = *reinterpret_cast<const uint4*>(aq + 32 * ib);
+            const uint4 a1 = *reinterpret_cast<const uint4*>(aq + 32 * ib + 16);
+            const uint32_t ax[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+            int s = 0;
+#pragma unroll
+            for (int l = 0; l < 4; l++) {
+                const uint2 g = grid[(aux0 >> (8 * l)) & 0xff];
+                const uint2 m = sgn[(aux1 >> (7 * l)) & 127];
+                s = dp4a_s8s8(__vsub4(g.x ^ m.x, m.x), ax[2 * l], s);
+                s = dp4a_s8s8(__vsub4(g.y ^ m.y, m.y), ax[2 * l + 1], s);
+            }
+            isum += (2 * (int)(aux1 >> 28) + 1) * s;
+        }
+        return (d * dxb) * (float)isum;
+    }
+    __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int /*nrb*/, const uint8_t* aq, const int16_t* bs, float dxb) {
+        return block_dot(sl + f * SZ_IQ2_XXS, aq, bs, dxb);
+    }
+};
+
+// ---------------------------------------------------------------------------------------------------------------
+// Gate/up pairs of IQ1_S or IQ2_XXS experts (gate and up of the same type).  Structure of rows_bulk_q4k_kernel (token
+// chunks, one (token, slot) work list per chunk, Q8_K activations staged side by side), with a 2-row unit per ring slot.
+constexpr int kIqMaxWarps = 16;
+template <class Fmt, int SLOTS>
+__global__ void __launch_bounds__(kIqMaxWarps * 32, 1) rows_bulk_iq_kernel(const RowsParams p, int act_tok, int tc) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    __shared__ int s_np;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, W = blockDim.x >> 5;
+    Fmt::stage_tables();     // read only after the first __syncthreads below
+    int Teff = p.ntokens;
+    if (p.bsz) Teff = min(Teff, *p.bsz);
+    const int nblk = p.ncols / QK_K;
+    const int row_bytes = nblk * Fmt::kBlockBytes;
+    const int unit_bytes = 2 * row_bytes;             // rows 2r, 2r+1 of one matrix
+    const int slot_bytes = 2 * unit_bytes;            // gate unit | up unit
+    const int nru = p.rows / 2;                       // row pairs per matrix
+    const int total_out = p.slots * p.rows;
+    // [tc activation rows: q8 [nblk][272] | bs32 [nblk][8] int16 | dx [nblk]] [pair list] [mbarriers] [rings]
+    int* pairs = reinterpret_cast<int*>(smem + (size_t)tc * act_tok);
+    const size_t off = ((size_t)tc * act_tok + (size_t)tc * p.slots * 4 + 15) & ~(size_t)15;
+    const int bar_bytes = (W * SLOTS * 8 + 15) & ~15;
+    const uint32_t bar_u32 = (uint32_t)__cvta_generic_to_shared(smem + off) + warp * SLOTS * 8;
+    uint8_t* ring = smem + off + bar_bytes + (size_t)warp * SLOTS * slot_bytes;
+    const uint32_t ring_u32 = (uint32_t)__cvta_generic_to_shared(ring);
+    if (lane == 0) {
+#pragma unroll
+        for (int s = 0; s < SLOTS; s++) mbar_init(bar_u32 + 8 * s, 1);
+        mbar_fence_init();
+        fence_proxy_async_smem();
+    }
+    int slot_i = 0, slot_u = 0;
+    uint32_t phase = 0;
+
+  for (int t0 = 0; t0 < Teff; t0 += tc) {
+    const int nt = min(tc, Teff - t0);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int np = 0;
+        for (int tl = 0; tl < nt; tl++)
+            for (int s = 0; s < p.slots; s++) {
+                const long e = (long)p.ids[(long)(t0 + tl) * p.slots + s] - p.id_offset;
+                if (e >= 0 && e < p.n_experts) pairs[np++] = (tl << 8) | s;
+            }
+        s_np = np;
+    }
+    __syncthreads();
+    const int total = s_np * nru;
+    const int u0 = (int)((long)total * blockIdx.x / gridDim.x), u1 = (int)((long)total * (blockIdx.x + 1) / gridDim.x);
+    int nu = u1 - u0 - warp;
+    nu = nu > 0 ? (nu + W - 1) / W : 0;
+    int ipi = 0, iru = 0, iss = 0;
+    if (nu > 0) { ipi = (u0 + warp) / nru; iru = (u0 + warp) - ipi * nru; }
+    int cpi = ipi, cru = iru;
+
+    auto issue_one = [&]() {
+        if (iss < nu) {
+            if (lane == 0) {
+                const int pr = pairs[ipi];
+                const long e = (long)p.ids[(long)(t0 + (pr >> 8)) * p.slots + (pr & 0xff)] - p.id_offset;
+                const long first = (e * p.rows + 2L * iru) * row_bytes;
+                const uint32_t bar = bar_u32 + 8 * slot_i, dst = ring_u32 + slot_i * slot_bytes;
+                mbar_expect_tx(bar, (uint32_t)slot_bytes);
+                bulk_g2s(dst, reinterpret_cast<const uint8_t*>(p.w0) + first, (uint32_t)unit_bytes, bar);
+                bulk_g2s(dst + unit_bytes, reinterpret_cast<const uint8_t*>(p.w1) + first, (uint32_t)unit_bytes, bar);
+            }
+            iss++;
+            iru += W;
+            while (iru >= nru) { iru -= nru; ipi++; }
+            slot_i = (slot_i + 1 == SLOTS) ? 0 : slot_i + 1;
+        }
+    };
+#pragma unroll
+    for (int s = 0; s < SLOTS; s++) issue_one();
+
+    {   // quantise the chunk's activation rows into the padded layout (as rows_bulk_q4k_kernel)
+        float cur[8], nxt[8];
+        const int totalb = nt * nblk;
+        int g = warp;
+        if (g < totalb) load_block8(p.x, (long)(t0 + g / nblk) * p.ncols + (long)(g % nblk) * QK_K + lane * 8, p.hidden_type, cur);
+#pragma unroll 1
+        while (g < totalb) {
+            const int gn = g + W;
+            if (gn < totalb) load_block8(p.x, (long)(t0 + gn / nblk) * p.ncols + (long)(gn % nblk) * QK_K + lane * 8, p.hidden_type, nxt);
+            const int tl = g / nblk, b = g - tl * nblk;
+            uint8_t* at = smem + (size_t)tl * act_tok;
+            warp_quantize_q8k_block(cur, lane, reinterpret_cast<uint32_t*>(at + (size_t)b * kActBlkStride),
+                                    reinterpret_cast<float*>(at + (size_t)nblk * (kActBlkStride + 16)) + b, nullptr,
+                                    reinterpret_cast<int16_t*>(at + (size_t)nblk * kActBlkStride) + b * 8);
+#pragma unroll
+            for (int i = 0; i < 8; i++) cur[i] = nxt[i];
+            g = gn;
+        }
+    }
+    __syncthreads();
+
+    for (int n = 0; n < nu; n++) {
+        mbar_wait(bar_u32 + 8 * slot_u, (phase >> slot_u) & 1u);
+        phase ^= 1u << slot_u;
+        const uint8_t* sl = ring + slot_u * slot_bytes;
+        const int pr = pairs[cpi];
+        const uint8_t* at = smem + (size_t)(pr >> 8) * act_tok;
+        const int16_t* bs32 = reinterpret_cast<const int16_t*>(at + (size_t)nblk * kActBlkStride);
+        const float* dx = reinterpret_cast<const float*>(at + (size_t)nblk * (kActBlkStride + 16));
+        float g0 = 0.f, g1 = 0.f, v0 = 0.f, v1 = 0.f;
+        for (int f = lane; f < 2 * nblk; f += 32) {   // (row, block) of the unit: f = rw * nblk + blk
+            const int rw = f >= nblk, blk = f - rw * nblk;
+            const uint8_t* aq = at + (size_t)blk * kActBlkStride;
+            const float g = Fmt::block_dot(sl + f * Fmt::kBlockBytes, aq, bs32 + blk * 8, dx[blk]);
+            const float u = Fmt::block_dot(sl + unit_bytes + f * Fmt::kBlockBytes, aq, bs32 + blk * 8, dx[blk]);
+            if (rw) { g1 += g; v1 += u; } else { g0 += g; v0 += u; }
+        }
+        const float r = warp_reduce4(g0, g1, v0, v1, lane);   // lane 0: g0, 8: g1, 16: u0, 24: u1
+        __syncwarp();
+        slot_u = (slot_u + 1 == SLOTS) ? 0 : slot_u + 1;
+        issue_one();
+        const float gs = __shfl_sync(0xffffffffu, r, 8 * (lane & 1)), us = __shfl_sync(0xffffffffu, r, 16 + 8 * (lane & 1));
+        if (lane < 2) {
+            const long o = (long)(t0 + (pr >> 8)) * total_out + (long)(pr & 0xff) * p.rows + 2L * cru + lane;
+            p.out_f32[o] = (p.use_silu ? act_silu(gs) : act_relu(gs)) * us;
+        }
+        cru += W;
+        while (cru >= nru) { cru -= nru; cpi++; }
+    }
+  }  // token chunks
+}
+
+}  // namespace ktb

@@ -5,9 +5,11 @@
 #include <cstring>
 #include <new>
 
+#define KTB_IQ_CODEBOOKS
 #include "gemv_bulk.cuh"
 #include "dense_bulk.cuh"
 #include "rawint4.cuh"
+#include "iq.cuh"
 #include "handles.cuh"
 
 namespace ktb {
@@ -302,6 +304,38 @@ static int launch_rows_i4(const RowsParams& p, int T, int device, cudaStream_t s
     return KTB200_OK;
 }
 
+// IQ1_S / IQ2_XXS gate/up pairs through the bulk-copy ring (rows_bulk_iq_kernel, iq.cuh): 2-row units, 2 slots per warp,
+// tokens per chunk as many (<= 8) as leave room for >= 8 warps.  Returns 1 when the launch does not suit it (gate and up
+// of different types, rows not 16-byte aligned in pairs, a shared-expert slot): the generic kernels take it then.
+template <class Fmt>
+static int launch_rows_bulk_iq(const RowsParams& p, int T, int device, cudaStream_t stream) {
+    constexpr int S = 2;
+    if (!cfg_bulk()) return 1;
+    const int nblk = p.ncols / QK_K;
+    if (p.type0 != Fmt::kType || p.type1 != Fmt::kType || p.x0 || !p.ids || nblk % 4 || p.rows % 2 || p.slots > 200) return 1;
+    const long total = (long)p.slots * (p.rows / 2);
+    if (total >= (1L << 26)) return 1;
+    const size_t slot = (size_t)4 * nblk * Fmt::kBlockBytes;
+    const int act_tok = (nblk * kActBlkStride + nblk * 16 + nblk * 4 + 15) & ~15;
+    const size_t cap = kSmemCap - Fmt::kTableBytes;
+    auto head = [&](int tc) { return ((size_t)tc * act_tok + (size_t)tc * p.slots * 4 + 15) & ~(size_t)15; };
+    int tc = T < 8 ? T : 8;
+    while (tc > 1 && head(tc) + 64 + (size_t)8 * S * (slot + 8) > cap) tc--;
+    if (head(tc) + 64 >= cap) return 1;
+    int W = (int)((cap - head(tc) - 16) / (S * (slot + 8)));
+    if (W > kIqMaxWarps) W = kIqMaxWarps;
+    if (W > cfg_bulk_warps()) W = cfg_bulk_warps();
+    if (W < 4) return 1;
+    const size_t smem = head(tc) + (((size_t)W * S * 8 + 15) & ~(size_t)15) + (size_t)W * S * slot;
+    int gx = num_sms(device);
+    if (gx > total) gx = (int)total;
+    if (gx < 1) gx = 1;
+    KTB_CUDA_CHECK(cudaFuncSetAttribute(rows_bulk_iq_kernel<Fmt, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    rows_bulk_iq_kernel<Fmt, S><<<gx, W * 32, smem, stream>>>(p, act_tok, tc);
+    KTB_LAUNCH_CHECK();
+    return KTB200_OK;
+}
+
 template <bool PAIR>
 static int launch_rows(FmtId f, const RowsParams& p_in, int T, int device, cudaStream_t stream) {
     RowsParams p = p_in;
@@ -309,6 +343,11 @@ static int launch_rows(FmtId f, const RowsParams& p_in, int T, int device, cudaS
     if (f == FMT_RAWINT4) {
         if (!PAIR) { set_error("RAWINT4: routed experts only"); return KTB200_EINVAL; }
         return launch_rows_i4(p, T, device, stream);
+    }
+    if (PAIR && f == FMT_GENK && is_iquant(p.type0)) {
+        const int rci = p.type0 == KTB200_TYPE_IQ1_S ? launch_rows_bulk_iq<BulkIQ1S>(p, T, device, stream)
+                                                     : launch_rows_bulk_iq<BulkIQ2XXS>(p, T, device, stream);
+        if (rci != 1) return rci;
     }
     if (!PAIR && f == FMT_Q4K) {
         const int rcd = launch_dense_q4k(p, T, device, stream);
@@ -411,8 +450,9 @@ static int reduce_bulk_plan(int rows, int ncols, int pcap, int S, int device, in
     const int nrows_max = ((quads + gx - 1) / gx) * 4;
     size_t base = (size_t)pcap * nb * (kActBlkStride + 2 * Fmt::kBs + 4) + (size_t)nrows_max * pcap * 4 + (size_t)pcap * 4;
     base = (base + 15) & ~(size_t)15;
-    if (base + 16 >= kSmemCap) return 0;
-    int W = (int)((kSmemCap - base - 16) / ((size_t)S * (item + 8)));
+    const size_t cap = kSmemCap - Fmt::kTableBytes;
+    if (base + 16 >= cap) return 0;
+    int W = (int)((cap - base - 16) / ((size_t)S * (item + 8)));
     if (W > cfg_bulk_warps()) W = cfg_bulk_warps();
     if (W > kBulkMaxWarpsDown) W = kBulkMaxWarpsDown;
     if (W < 2) return 0;
@@ -519,6 +559,11 @@ static int launch_reduce(FmtId f, const ReduceParams& p_in, int T, int device, c
         const int rc = launch_reduce_bulk<BulkQ4K>(p, T, device, stream);
         if (rc != 1) return rc;
     }
+    if (f == FMT_GENK && is_iquant(p.type) && !p.xw) {   // IQ down items (iq.cuh); otherwise the generic kernel
+        const int rc = p.type == KTB200_TYPE_IQ1_S ? launch_reduce_bulk<BulkIQ1S>(p, T, device, stream)
+                                                   : launch_reduce_bulk<BulkIQ2XXS>(p, T, device, stream);
+        if (rc != 1) return rc;
+    }
     if (p.xw && (p.shared_token >= 0 || p.xw_out)) { set_error("per-token shared slot: only the bulk-copy kernels implement it"); return KTB200_EINVAL; }
     if (f == FMT_Q6K8) {
         const int rc = launch_reduce_pipe_q6k8(p, T, device, stream);
@@ -534,6 +579,8 @@ static int launch_reduce(FmtId f, const ReduceParams& p_in, int T, int device, c
 }
 
 static bool weight_type_ok(int t) { return is_kquant(t); }
+// routed experts also take the codebook i-quants (generic per-pair kernels; IQ down-projection items)
+static bool expert_type_ok(int t) { return is_kquant(t) || is_iquant(t); }
 
 // quantize API kernel: one warp per 256-block, packed block_q8_K output (292 B)
 __global__ void __launch_bounds__(256) quantize_q8k_kernel(const void* x, int hidden_type, long n_blocks, uint8_t* out) {
@@ -572,7 +619,7 @@ int ktb200_moe_create(const ktb200_moe_config* c, int device, ktb200_moe** out) 
         set_error("MOEConfig: RAWINT4_G32 must be the type of all three tensors (gate %d up %d down %d)", c->gate_type, c->up_type, c->down_type);
         return KTB200_EINVAL;
     }
-    if (!n_i4 && (!weight_type_ok(c->gate_type) || !weight_type_ok(c->up_type) || !weight_type_ok(c->down_type))) {
+    if (!n_i4 && (!expert_type_ok(c->gate_type) || !expert_type_ok(c->up_type) || !expert_type_ok(c->down_type))) {
         set_error("MOEConfig: unsupported ggml weight type (gate %d up %d down %d)", c->gate_type, c->up_type, c->down_type);
         return KTB200_EINVAL;
     }
@@ -729,6 +776,8 @@ int ktb200_moe_forward_ep(ktb200_moe* m, ktb200_mlp* shared, int qlen, int k, co
     if (!shared || !shared_out || own_token < 0 || own_token >= qlen) { set_error("moe_forward_ep: shared handle, shared_out and 0 <= own_token < qlen are required"); return KTB200_EINVAL; }
     if (!shared->loaded) { set_error("shared expert: Not Loaded"); return KTB200_ESTATE; }
     if (m && is_rawint4(m->cfg.gate_type)) { set_error("moe_forward_ep: RAWINT4_G32 experts are not supported (their kernels have no shared-expert slot)"); return KTB200_EINVAL; }
+    if (m) for (int t : {m->cfg.gate_type, m->cfg.up_type, m->cfg.down_type})
+        if (is_iquant(t)) { set_error("moe_forward_ep: %s experts are not supported (expert parallelism does not take the i-quants)", iquant_name(t)); return KTB200_EINVAL; }
     // shared_out rows are indexed like the tokens: point the kernels at a virtual base so that row `own_token` is shared_out
     uint8_t* base = reinterpret_cast<uint8_t*>(shared_out) - (size_t)own_token * shared->H * type_size(shared->hidden_type);
     return moe_forward_impl(m, qlen, k, ids, weights, input, partial_out, bsz, (cudaStream_t)stream, nullptr, shared, own_token, base);
@@ -812,6 +861,7 @@ struct ktb200_linear {
 int ktb200_linear_create(int in_size, int out_size, const void* proj, int proj_type, int hidden_type, int group_max_len,
                          int device, ktb200_linear** out) {
     if (!out || !proj) { set_error("null argument"); return KTB200_EINVAL; }
+    if (is_iquant(proj_type)) { set_error("LinearConfig: %s is a routed-expert type; linears take Q2_K..Q6_K and IQ4_XS", iquant_name(proj_type)); return KTB200_EINVAL; }
     if (!weight_type_ok(proj_type)) { set_error("LinearConfig: unsupported ggml type %d", proj_type); return KTB200_EINVAL; }
     if (!is_hidden_type(hidden_type)) { set_error("LinearConfig: bad hidden_type %d", hidden_type); return KTB200_EINVAL; }
     if (in_size <= 0 || out_size <= 0 || in_size % QK_K) { set_error("LinearConfig: input_size %d must be a positive multiple of 256", in_size); return KTB200_EINVAL; }
@@ -857,6 +907,8 @@ int ktb200_linear_forward(ktb200_linear* l, int qlen, const void* input, void* o
 int ktb200_mlp_create(int H, int I, const void* gate, const void* up, const void* down, int gate_type, int up_type,
                       int down_type, int hidden_type, int group_max_len, int device, ktb200_mlp** out) {
     if (!out || !gate || !up || !down) { set_error("null argument"); return KTB200_EINVAL; }
+    for (int t : {gate_type, up_type, down_type})
+        if (is_iquant(t)) { set_error("MLPConfig: %s is a routed-expert type; MLPs take Q2_K..Q6_K and IQ4_XS", iquant_name(t)); return KTB200_EINVAL; }
     if (!weight_type_ok(gate_type) || !weight_type_ok(up_type) || !weight_type_ok(down_type)) { set_error("MLPConfig: unsupported ggml type"); return KTB200_EINVAL; }
     if (!is_hidden_type(hidden_type)) { set_error("MLPConfig: bad hidden_type"); return KTB200_EINVAL; }
     if (H <= 0 || I <= 0 || H % QK_K || I % QK_K || group_max_len <= 0) { set_error("MLPConfig: sizes must be positive multiples of 256"); return KTB200_EINVAL; }

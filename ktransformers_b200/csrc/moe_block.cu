@@ -1261,6 +1261,8 @@ extern "C" int ktb200_moe_ep_block_forward(const ktb200_gate_config* gc, ktb200_
     if (k <= 0 || k > c.routed_expert_num || k > 16 || world * k > kEpPairsMax) { set_error("ep_block: top_k=%d (<= 16, world * top_k <= %d)", k, kEpPairsMax); return KTB200_EINVAL; }
     if (c.group_max_len < world) { set_error("ep_block: group_max_len=%d must be >= world=%d (scratch rows)", c.group_max_len, world); return KTB200_EINVAL; }
     if (is_rawint4(c.gate_type)) { set_error("ep_block: RAWINT4_G32 experts are not supported by the expert-parallel kernel"); return KTB200_EINVAL; }
+    for (int t : {c.gate_type, c.up_type, c.down_type})
+        if (is_iquant(t)) { set_error("ep_block: %s experts are not supported by the expert-parallel kernel", iquant_name(t)); return KTB200_EINVAL; }
     const FmtId fd = pick_fmt(c.down_type, m->down_layout);
     const bool sh_ok = !sh || (sh->H == c.hidden_size && sh->I == c.intermediate_size && sh->hidden_type == c.hidden_type &&
                                sh->gate_type == c.gate_type && sh->up_type == c.up_type && sh->down_type == c.down_type &&

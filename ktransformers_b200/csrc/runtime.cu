@@ -40,8 +40,8 @@ int num_sms(int device) {
 extern "C" {
 const char* ktb200_last_error(void) { return ktb::g_err; }
 const char* ktb200_version(void) { return "ktb200 0.1 (sm_90a)"; }
-long ktb200_type_size(int t) { return ktb::type_size(t); }
-long ktb200_blck_size(int t) { return ktb::blck_size(t); }
+long ktb200_type_size(int t) { return ktb::weight_block_bytes(t); }
+long ktb200_blck_size(int t) { return ktb::weight_block_elems(t); }
 unsigned long long ktb200_launch_count(void) { return ktb::g_launches.load(); }
 }
 

@@ -63,13 +63,18 @@ class PeerExchange:
 def attach_expert_parallel(model: torch.nn.Module, hidden_size: int, hidden_type: int, device, group=None) -> PeerExchange:
     """Give every injected MoE block of `model` whose experts are sharded the same PeerExchange."""
     from ..native import RAWINT4_G32
+    from ..util.custom_gguf import GGML_NAMES, B200_EP_GATE_UP_TYPES, B200_EP_DOWN_TYPES
     for m in model.modules():
         gen = getattr(getattr(m, "experts", None), "generate_experts", None)
-        if hasattr(m, "_block_handles") and getattr(gen, "gate_type", None) == RAWINT4_G32:
-            # the single-launch NVLink kernel does not take INT4 experts, and without it a sharded block would return its
-            # shard's partial sums as the layer output
-            raise ValueError(f"attach_expert_parallel: {getattr(m, 'key', type(m).__name__)} has RAWINT4_G32 experts, "
-                             "which the expert-parallel kernel does not support")
+        if not hasattr(m, "_block_handles") or getattr(gen, "gate_type", None) is None:
+            continue
+        types = (gen.gate_type, gen.up_type, gen.down_type)
+        names = ["RAWINT4_G32" if t == RAWINT4_G32 else GGML_NAMES.get(int(t), str(t)) for t in types]
+        if names[0] not in B200_EP_GATE_UP_TYPES or names[1] not in B200_EP_GATE_UP_TYPES or names[2] not in B200_EP_DOWN_TYPES:
+            # the single-launch NVLink kernel takes Q4_K gate/up and Q4_K/Q6_K down only, and without it a sharded block would
+            # return its shard's partial sums as the layer output
+            raise ValueError(f"attach_expert_parallel: {getattr(m, 'key', type(m).__name__)} has {'/'.join(names)} experts "
+                             "(gate/up/down), which the expert-parallel kernel does not support")
     ex = PeerExchange(hidden_size, hidden_type, device, group)
     for m in model.modules():
         if hasattr(m, "_block_handles"):

@@ -22,7 +22,7 @@ import torch
 from torch import nn
 
 from .. import native
-from ..util.custom_gguf import GGML_NAMES, TORCH_TO_GGML_HIDDEN, B200_WEIGHT_TYPES
+from ..util.custom_gguf import GGML_NAMES, TORCH_TO_GGML_HIDDEN, B200_WEIGHT_TYPES, B200_EXPERT_TYPES
 from ..util.utils import InferenceState
 from .base_operator import BaseInjectedModule
 
@@ -112,7 +112,7 @@ class KExpertsB200(KExpertsBase):
         if n_i4 not in (0, 3):
             raise ValueError("KExpertsB200: RAWINT4_G32 must be the type of all three expert tensors")
         for t in (self.gate_type, self.up_type, self.down_type) if not n_i4 else ():
-            if GGML_NAMES.get(t) not in B200_WEIGHT_TYPES:
+            if GGML_NAMES.get(t) not in B200_EXPERT_TYPES:
                 raise ValueError(f"KExpertsB200: ggml type {GGML_NAMES.get(t, t)} is not supported by the sm_90a kernels")
         E = self.n_routed_experts
         per, lo = E // self.ep_size, (E // self.ep_size) * self.ep_rank

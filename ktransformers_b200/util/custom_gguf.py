@@ -65,7 +65,12 @@ GGML_BLOCK_SIZES = {t.name: GGML_QUANT_SIZES[t][1] for t in GGML_QUANT_SIZES}
 
 # types the sm_90a kernels consume / dequantise directly
 B200_WEIGHT_TYPES = {"Q2_K", "Q3_K", "Q4_K", "Q5_K", "Q6_K", "IQ4_XS"}
-B200_DEQUANT_TYPES = B200_WEIGHT_TYPES | {"Q8_0", "F32", "F16", "BF16"}
+# routed experts also take ggml's codebook i-quants (DeepSeek-R1's 1.5-2-bit GGUF files); linears and MLPs do not
+B200_EXPERT_TYPES = B200_WEIGHT_TYPES | {"IQ1_S", "IQ2_XXS"}
+B200_DEQUANT_TYPES = B200_EXPERT_TYPES | {"Q8_0", "F32", "F16", "BF16"}
+# what the single-launch expert-parallel kernel takes: Q4_K gate/up, Q4_K or Q6_K down
+B200_EP_GATE_UP_TYPES = {"Q4_K"}
+B200_EP_DOWN_TYPES = {"Q4_K", "Q6_K"}
 
 TORCH_TO_GGML_HIDDEN = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 30}
 
