@@ -341,6 +341,32 @@ size_t ktb200_mla_workspace_bytes(int batch, int num_heads, int max_splits);
 int ktb200_mla_decode(const ktb200_mla_params* p, void* stream);
 /* Diagnostics: while non-NULL, one CTA of ktb200_mla_decode dumps the raw scores of its first tile (>= 2048 floats). */
 void ktb200_debug_mla(float* debug_dev);
+/* ------------------------------------------------------------------------------------------
+ * Causal MLA prefill attention over the decompressed heads (the non-absorbed prefill of
+ * archive/ktransformers/operators/attention.py:349-478: kv_b_proj, then flash_attn_func(..., causal=True)).
+ * With P = kv_len - q_len tokens already cached, query i of the chunk sits at position P + i and attends to keys j <= P + i:
+ *   s = (q_nope . k_nope_j + q_pe . k_pe_j) * sm_scale  (fp32), online softmax in fp32, P rounded to bf16 before P.V,
+ *   out [batch][q_len][num_heads][128] bf16 (contiguous) = (sum_j P_j v_j) / sum_j P_j.
+ * Operands (bf16) are read in place; strides are in elements, token / head / batch:
+ *   q_nope [.][q_len][num_heads][128], q_pe [.][q_len][num_heads][64]   (e.g. the q_b output view and the roped q_pe)
+ *   k_nope, v [.][kv_len][num_heads][128]                               (e.g. the two halves of each head of kv_b_proj's output)
+ *   k_pe [.][kv_len][64], shared by all heads                           (e.g. columns 512..575 of the latent cache rows)
+ * Head dims must be 128 / 64 / 128.  Every pointer must be 16-byte aligned and every stride a multiple of 8 elements.
+ * KTB200_EINVAL (before any device work) for q_len < 1, q_len > kv_len, batch or num_heads < 1, sm_scale <= 0, null
+ * pointers, other head dims or misalignment.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct ktb200_mla_prefill_params {
+    int batch, q_len, kv_len, num_heads;
+    int qk_nope_head_dim, qk_rope_head_dim, v_head_dim;
+    float sm_scale;
+    const void* q_nope; long q_nope_token_stride, q_nope_head_stride, q_nope_batch_stride;
+    const void* q_pe; long q_pe_token_stride, q_pe_head_stride, q_pe_batch_stride;
+    const void* k_nope; long k_nope_token_stride, k_nope_head_stride, k_nope_batch_stride;
+    const void* v; long v_token_stride, v_head_stride, v_batch_stride;
+    const void* k_pe; long k_pe_token_stride, k_pe_batch_stride;
+    void* out;
+} ktb200_mla_prefill_params;
+int ktb200_mla_prefill(const ktb200_mla_prefill_params* p, void* stream);
 /* Debug aid of the grouped (prefill) expert GEMM: when non-null, CTA 0 of the gate and down GEMMs writes clock64 stamps of its
  * first 96 stages, [kernel 2][role 3 = producer, MMA warpgroup, unused][stage 96][4] int64 (tools/grouped_probe.py prints them). */
 void ktb200_debug_grouped(long long* trace_dev);

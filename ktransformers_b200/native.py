@@ -48,6 +48,18 @@ class MlaParams(C.Structure):
                 ("lse_out", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("kv_cache_rows", C.c_long)]
 
 
+class MlaPrefillParams(C.Structure):
+    """struct ktb200_mla_prefill_params (include/ktb200.h); strides in elements, token / head / batch."""
+    _fields_ = [("batch", C.c_int), ("q_len", C.c_int), ("kv_len", C.c_int), ("num_heads", C.c_int),
+                ("qk_nope_head_dim", C.c_int), ("qk_rope_head_dim", C.c_int), ("v_head_dim", C.c_int), ("sm_scale", C.c_float),
+                ("q_nope", C.c_void_p), ("q_nope_token_stride", C.c_long), ("q_nope_head_stride", C.c_long), ("q_nope_batch_stride", C.c_long),
+                ("q_pe", C.c_void_p), ("q_pe_token_stride", C.c_long), ("q_pe_head_stride", C.c_long), ("q_pe_batch_stride", C.c_long),
+                ("k_nope", C.c_void_p), ("k_nope_token_stride", C.c_long), ("k_nope_head_stride", C.c_long), ("k_nope_batch_stride", C.c_long),
+                ("v", C.c_void_p), ("v_token_stride", C.c_long), ("v_head_stride", C.c_long), ("v_batch_stride", C.c_long),
+                ("k_pe", C.c_void_p), ("k_pe_token_stride", C.c_long), ("k_pe_batch_stride", C.c_long),
+                ("out", C.c_void_p)]
+
+
 _lib = None
 _lock = threading.Lock()
 
@@ -97,6 +109,7 @@ SYMBOLS = {
     "ktb200_mla_workspace_bytes": (C.c_size_t, [_I, _I, _I]),
     "ktb200_mla_decode": (_I, [C.POINTER(MlaParams), _VP]),
     "ktb200_debug_mla": (None, [_VP]),
+    "ktb200_mla_prefill": (_I, [C.POINTER(MlaPrefillParams), _VP]),
     "ktb200_debug_grouped": (None, [_VP]),
     "ktb200_mla_absorb_q": (_I, [_VP, _L, _L, _VP, _I, _I, _I, _VP, _I, _VP]),
     "ktb200_mla_absorb_o": (_I, [_VP, _VP, _I, _I, _I, _VP, _I, _VP]),

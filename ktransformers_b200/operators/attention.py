@@ -5,9 +5,17 @@ decode branch): q projections -> RoPE -> paged latent-cache update -> q_nope . W
 over the 576-wide latents -> . W_UV^T -> o_proj.  The attention itself is `MLAWrapper.run` = ktb200_mla_decode (wgmma +
 TMA, csrc/mla.cu); the cache write is ktb200_mla_kv_write; the projections are whatever modules the rules injected
 (KLinearB200 on raw GGUF blocks, or nn.Linear); the two absorb products are ktb200_mla_absorb_q / _o (HBM-bound batched
-GEMVs over the bf16 halves of kv_b_proj; torch.matmul for other dtypes).  Prefill (q_len > 1 without absorb) is outside this path and raises."""
+GEMVs over the bf16 halves of kv_b_proj; torch.matmul for other dtypes).
+
+Prefill (q_len > 1 without absorb_for_prefill) follows the reference's non-absorbed branch of the same function: the same
+projections, RoPE and cache update, then the first S = P + q_len cached latents of each sequence go through kv_b_proj
+(dense, as the reference calls it) and ktb200_mla_prefill (csrc/mla_prefill.cu, wgmma + TMA) runs causal attention over
+the decompressed heads in place: q_nope from the q_b output, k_nope / v from the kv_b_proj output, k_pe from the cache
+rows.  P is the cache's host-side token count, so the path makes no device-to-host synchronisation; positions are
+[P, P + q_len), as StaticCache.update assumes.  bf16 only."""
 from __future__ import annotations
 
+import ctypes as C
 from typing import Optional, Tuple
 
 import torch
@@ -39,9 +47,10 @@ class KDeepseekV2Attention(BaseInjectedModule, DeepseekV3Attention):
                 position_ids: Optional[torch.Tensor] = None, past_key_value=None, output_attentions: bool = False,
                 use_cache: bool = False, cache_position: Optional[torch.Tensor] = None, **kwargs):
         bsz, q_len, _ = hidden_states.size()
-        if q_len != 1 and not self.absorb_for_prefill:
-            raise NotImplementedError("KDeepseekV2Attention: the H100 path covers absorbed decode (q_len == 1)")
+        prefill = q_len != 1 and not self.absorb_for_prefill
         assert past_key_value is not None, "decode needs the paged latent cache (models/custom_cache.StaticCache)"
+        if prefill:   # the reference's kv_seq_len: the cache's host counter before the update, plus the new tokens
+            kv_seq_len = past_key_value.get_seq_length(self.layer_idx) + q_len
         q = self.q_proj(hidden_states) if self.q_lora_rank is None else self.q_b_proj(self.q_a_layernorm(self.q_a_proj(hidden_states)))
         q = q.view(bsz, q_len, self.num_heads, self.q_head_dim)
         q_nope, q_pe = torch.split(q, [self.qk_nope_head_dim, self.qk_rope_head_dim], dim=-1)
@@ -54,6 +63,8 @@ class KDeepseekV2Attention(BaseInjectedModule, DeepseekV3Attention):
 
         cache_kwargs = {"sin": sin, "cos": cos, "cache_position": cache_position}
         kv_with_k_pe, page_table = past_key_value.update(compressed_kv, k_pe, self.layer_idx, cache_kwargs)
+        if prefill:
+            return self.forward_prefill(q, q_pe, kv_with_k_pe, past_key_value.max_pages, kv_seq_len), None, past_key_value
         ckv_pages = kv_with_k_pe[:, :, :, : self.kv_lora_rank].view(-1, past_key_value.page_size, self.kv_lora_rank)
         kpe_pages = kv_with_k_pe[:, :, :, self.kv_lora_rank:].view(-1, past_key_value.page_size, self.qk_rope_head_dim)
 
@@ -92,3 +103,27 @@ class KDeepseekV2Attention(BaseInjectedModule, DeepseekV3Attention):
             attn = torch.matmul(attn.transpose(1, 2), out_absorb.mT).transpose(1, 2).contiguous()     # [b, 1, h, 128]
         attn = self.o_proj(attn.reshape(bsz, q_len, self.num_heads * self.v_head_dim))
         return attn, None, past_key_value
+
+    def forward_prefill(self, q: torch.Tensor, q_pe: torch.Tensor, cache: torch.Tensor, max_pages: int, kv_seq_len: int) -> torch.Tensor:
+        """Causal attention of a prompt chunk over the first kv_seq_len cached tokens of each sequence (attention.py:349-478,
+        q_len > 1), then o_proj.  q [b, q_len, heads, 192] is the q_b output, q_pe [b, q_len, heads, 64] the roped part,
+        cache the layer's latent buffer [max_batch * max_pages, page_size, 1, 576] after the update; with the identity page
+        table the rows of sequence b are the contiguous rows [b * max_pages * page_size, ...)."""
+        bsz, q_len = q.shape[0], q.shape[1]
+        if q.dtype != torch.bfloat16 or q_pe.dtype != torch.bfloat16 or self.kv_b_proj.weight.dtype != torch.bfloat16:
+            raise NotImplementedError(f"KDeepseekV2Attention prefill is bf16 only (q {q.dtype}, kv_b_proj {self.kv_b_proj.weight.dtype})")
+        rows = cache.view(-1, max_pages * cache.shape[1], cache.shape[-1])[:bsz, :kv_seq_len]      # [b, S, 576]
+        kv = self.kv_b_proj(rows[..., : self.kv_lora_rank])                                          # [b, S, heads * 256]
+        kv = kv.view(bsz, kv_seq_len, self.num_heads, self.qk_nope_head_dim + self.v_head_dim)
+        k_nope, v = kv[..., : self.qk_nope_head_dim], kv[..., self.qk_nope_head_dim:]
+        q_nope, k_pe = q[..., : self.qk_nope_head_dim], rows[..., self.kv_lora_rank:]
+        out = torch.empty((bsz, q_len, self.num_heads, self.v_head_dim), dtype=q.dtype, device=q.device)
+        p = native.MlaPrefillParams(bsz, q_len, kv_seq_len, self.num_heads, self.qk_nope_head_dim, self.qk_rope_head_dim, self.v_head_dim,
+                                    self.softmax_scale,
+                                    q_nope.data_ptr(), q_nope.stride(1), q_nope.stride(2), q_nope.stride(0),
+                                    q_pe.data_ptr(), q_pe.stride(1), q_pe.stride(2), q_pe.stride(0),
+                                    k_nope.data_ptr(), k_nope.stride(1), k_nope.stride(2), k_nope.stride(0),
+                                    v.data_ptr(), v.stride(1), v.stride(2), v.stride(0),
+                                    k_pe.data_ptr(), k_pe.stride(1), k_pe.stride(0), out.data_ptr())
+        native.check(native.lib().ktb200_mla_prefill(C.byref(p), torch.cuda.current_stream(q.device).cuda_stream))
+        return self.o_proj(out.view(bsz, q_len, self.num_heads * self.v_head_dim))
