@@ -321,6 +321,37 @@ int ktb200_moe_ep_block_forward(const ktb200_gate_config* gate, ktb200_moe* moe,
                                 const void* x_own_dev, void* y_out_dev, int64_t* idx_dev, float* w_dev, int phase_mask, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Expert-parallel MoE layer for ANY number of tokens per GPU (prompt chunks, mixed batches): KDeepseekV3MoE.forward with the
+ * EP branch of DeepseekV3MoE.moe_infer (archive/ktransformers/models/modeling_deepseek_v3.py:550-605), no host round trips.
+ * Rank r holds counts[r] tokens (0 allowed) and owns experts [r*E/world, (r+1)*E/world).  Every token's output is what the
+ * single-GPU layer computes, up to the order of the fp32 cross-rank sum:
+ *   y[t] = round(sum over ranks r in rank order of partial_r[t]) + round(shared(x[t]))
+ * partial_r[t] = the fp32 weighted sum of t's experts that rank r owns, in expert_ids order (the shard's ordinary expert
+ * kernels, so every expert format ktb200_moe_forward runs is taken, RAWINT4 and the i-quants included).
+ * Each rank's region (symmetric: the same layout on every rank, mapped by every peer) holds the message rows {x, ids, weights}
+ * per source rank, the fp32 partial rows [world][max_tokens_per_rank][hidden] of its own tokens, a local fp32 scratch and
+ * flag words of its own; it starts zeroed and serves every layer (epochs live in it).  ktb200_ep_tokens_layout returns its
+ * size in bytes and, when `offsets` is non-NULL, the byte offsets of {x, ids, weights, partial, scratch, flags}; -1 on bad
+ * sizes.  flags: send[world] | deliver[world] | 2 epochs | status (1: a peer wait gave up after 4 s) | 2 arrival counters.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct ktb200_ep_tokens_comm {
+    int rank, world, max_tokens_per_rank, hidden_size, hidden_type, top_k;
+    void* const* bufs;   /* HOST array of `world` DEVICE pointers valid on this rank: every rank's region */
+} ktb200_ep_tokens_comm;
+long ktb200_ep_tokens_layout(int world, int max_tokens_per_rank, int hidden_size, int hidden_type, int top_k, long* offsets);
+/* counts: HOST int[world], identical on every rank.  x_own / y_out [counts[rank]][hidden] hidden_type; idx_out int64 and
+ * w_out fp32 [counts[rank]][top_k] receive the own tokens' routing and must stay untouched until the combine phase.
+ * `moe` owns ids [rank * expert_num, (rank + 1) * expert_num) of the gate's n_experts; `shared` may be NULL.
+ * phase_mask: 7 = the whole layer; 1 = route + send, 2 = experts + deliver, 4 = shared expert + combine, as separate calls
+ * (one GPU can emulate N ranks with them).  Every rank must issue the same sequence of calls.  Eager only (the gate and the
+ * grouped expert GEMMs allocate on first use), not capturable.  KTB200_EINVAL before any device work for counts outside
+ * [0, max_tokens_per_rank], rank / world out of range, null or not 16-byte aligned peer regions, an x_own that is not 16-byte
+ * aligned, and handles whose sizes, types or shard do not fit. */
+int ktb200_moe_ep_forward_tokens(const ktb200_gate_config* gate, ktb200_moe* moe, ktb200_mlp* shared, const ktb200_ep_tokens_comm* comm,
+                                 const int* counts, const void* x_own_dev, void* y_out_dev, int64_t* idx_dev, float* w_dev, int phase_mask,
+                                 void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Absorbed-MLA paged decode attention.  Replaces MLAWrapper.run / BatchMLAPagedAttentionWrapper
  * (archive/ktransformers/operators/flashinfer_wrapper.py:117-161; attention.py:419-447) and the
  * Triton split-KV decode (triton_attention.py:358-385).

@@ -508,7 +508,8 @@ bool grouped_ok(const ktb200_moe* m, int k) {
            c.intermediate_size % 256 == 0 && c.hidden_size % kGM == 0 && c.intermediate_size % kGM == 0 && c.expert_num <= 1023 && k <= 32;
 }
 
-int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, const float* weights, const void* input, void* output, const int* bsz, cudaStream_t s) {
+int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, const float* weights, const void* input, void* output, const int* bsz, cudaStream_t s,
+                        int out_type) {
     const ktb200_moe_config& c = m->cfg;
     const int E = c.expert_num, H = c.hidden_size, I = c.intermediate_size, dev = m->device;
     static const int chunk_cap = [] { const char* e = getenv("KTB200_GROUPED_CHUNK"); return e ? atoi(e) : 1024; }();
@@ -523,14 +524,14 @@ int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, cons
         attr[dev & 63] = true;
     }
     const FmtId fd = pick_fmt(c.down_type, m->down_layout);
-    const size_t hb = type_size(c.hidden_type);
+    const size_t hb = type_size(c.hidden_type), ob = type_size(out_type);
     const int grid = num_sms(dev);
     for (int t0 = 0; t0 < qlen; t0 += Tc) {
         const int T = qlen - t0 < Tc ? qlen - t0 : Tc, P = T * k;
         const int64_t* ids_c = ids + (size_t)t0 * k;
         const float* w_c = weights + (size_t)t0 * k;
         const uint8_t* x_c = reinterpret_cast<const uint8_t*>(input) + (size_t)t0 * H * hb;
-        uint8_t* o_c = reinterpret_cast<uint8_t*>(output) + (size_t)t0 * H * hb;
+        uint8_t* o_c = reinterpret_cast<uint8_t*>(output) + (size_t)t0 * H * ob;
         KTB_CUDA_CHECK(cudaMemsetAsync(g.counts, 0, (size_t)E * sizeof(int), s));
         grp_count_kernel<<<(P + 255) / 256, 256, 0, s>>>(ids_c, P, k, c.expert_id_offset, E, bsz, t0, g.counts);
         grp_scan_kernel<<<1, 32, 0, s>>>(g.counts, E, g.offsets, g.nt_prefix, g.cursor);
@@ -553,7 +554,7 @@ int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, cons
         gd.w = reinterpret_cast<const uint8_t*>(c.down_proj); gd.out = g.dd; gd.trace = g_grp_trace ? g_grp_trace + 3 * 96 * 4 : nullptr;
         if (fd == FMT_Q6K4T) grouped_gemm_kernel<1><<<grid, kGThreads, kGSmem, s>>>(gd);
         else grouped_gemm_kernel<0><<<grid, kGThreads, kGSmem, s>>>(gd);
-        grp_combine_kernel<<<dim3((H + 255) / 256, T), 256, 0, s>>>(g.dd, g.pos, w_c, T, k, H, bsz, t0, o_c, c.hidden_type);
+        grp_combine_kernel<<<dim3((H + 255) / 256, T), 256, 0, s>>>(g.dd, g.pos, w_c, T, k, H, bsz, t0, o_c, out_type);
         KTB_LAUNCH_CHECK();
         count_launch(9);   // + the one KTB_LAUNCH_CHECK counts = 10 launches per chunk
     }

@@ -705,7 +705,8 @@ float* ktb200_moe_intermediate(ktb200_moe* m) { return m ? m->inter : nullptr; }
 extern "C++" {
 namespace ktb {
 bool grouped_ok(const ktb200_moe* m, int k);
-int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, const float* weights, const void* input, void* output, const int* bsz, cudaStream_t s);
+int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, const float* weights, const void* input, void* output, const int* bsz, cudaStream_t s,
+                        int out_type);
 void grouped_set_trace(long long* t);
 }
 }
@@ -717,9 +718,11 @@ static int grouped_min_qlen() {
     return v;
 }
 
+// out_type: the type of `output` (-1: the handle's hidden_type).  The input rows are always of the hidden type; only the down
+// kernels and the grouped combine write `output`, so an F32 out_type yields the unrounded fp32 routed sums.
 static int moe_forward_impl(ktb200_moe* m, int qlen, int k, const int64_t* ids, const float* weights, const void* input,
                             void* output, const int* bsz, cudaStream_t s, cudaEvent_t mid, const ktb200_mlp* sh = nullptr,
-                            int shared_token = -1, void* shared_out = nullptr) {
+                            int shared_token = -1, void* shared_out = nullptr, int out_type = -1) {
     if (!m) { set_error("null handle"); return KTB200_EINVAL; }
     if (!m->loaded) { set_error("Not Loaded"); return KTB200_ESTATE; }
     if (qlen <= 0) return KTB200_OK;
@@ -727,10 +730,12 @@ static int moe_forward_impl(ktb200_moe* m, int qlen, int k, const int64_t* ids, 
     if (k <= 0 || k > c.routed_expert_num) { set_error("forward: k=%d outside (0, routed_expert_num=%d]", k, c.routed_expert_num); return KTB200_EINVAL; }
     if (qlen > c.group_max_len) { set_error("forward: qlen=%d exceeds group_max_len=%d", qlen, c.group_max_len); return KTB200_EINVAL; }
     if (!ids || !weights || !input || !output) { set_error("forward: null pointer"); return KTB200_EINVAL; }
+    if (out_type < 0) out_type = c.hidden_type;
+    if (out_type != c.hidden_type && sh) { set_error("forward: a shared expert needs the hidden output type"); return KTB200_EINVAL; }
     DeviceGuard g(m->device);
 
     if (!mid && !shared_out && grouped_min_qlen() > 0 && qlen >= grouped_min_qlen() && grouped_ok(m, k)) {
-        int rc = moe_forward_grouped(m, qlen, k, ids, weights, input, output, bsz, s);
+        int rc = moe_forward_grouped(m, qlen, k, ids, weights, input, output, bsz, s, out_type);
         if (rc || !sh) return rc;
         return ktb200_mlp_forward(const_cast<ktb200_mlp*>(sh), qlen, input, output, 1, bsz, (void*)s);
     }
@@ -758,7 +763,7 @@ static int moe_forward_impl(ktb200_moe* m, int qlen, int k, const int64_t* ids, 
     dp.shared_token = -1;
     dp.w = c.down_proj; dp.type = c.down_type; dp.n_experts = c.expert_num; dp.rows = c.hidden_size;
     dp.ncols = c.intermediate_size; dp.slots = k; dp.ids = ids; dp.id_offset = c.expert_id_offset;
-    dp.weights = weights; dp.a = m->inter; dp.out = output; dp.hidden_type = c.hidden_type; dp.accumulate = 0; dp.bsz = bsz;
+    dp.weights = weights; dp.a = m->inter; dp.out = output; dp.hidden_type = out_type; dp.accumulate = 0; dp.bsz = bsz;
     if (fuse) { dp.xw = sh->down; dp.shared_token = shared_token; dp.xw_out = shared_out; dp.xw_out_type = sh->hidden_type; }
     rc = launch_reduce(fd, dp, qlen, m->device, s);
     if (rc || !sh || fuse) return rc;
@@ -786,6 +791,16 @@ int ktb200_moe_forward_ep(ktb200_moe* m, ktb200_mlp* shared, int qlen, int k, co
 int ktb200_moe_forward(ktb200_moe* m, int qlen, int k, const int64_t* ids, const float* weights, const void* input,
                        void* output, const int* bsz, void* stream) {
     return moe_forward_impl(m, qlen, k, ids, weights, input, output, bsz, (cudaStream_t)stream, nullptr);
+}
+
+// the shard step of ktb200_moe_ep_forward_tokens (ep_tokens.cu): the routed sums of this handle's experts, unrounded fp32
+extern "C++" {
+namespace ktb {
+int moe_forward_f32_out(ktb200_moe* m, int qlen, int k, const int64_t* ids, const float* weights, const void* input, float* output,
+                        cudaStream_t s) {
+    return moe_forward_impl(m, qlen, k, ids, weights, input, output, nullptr, s, nullptr, nullptr, -1, nullptr, KTB200_TYPE_F32);
+}
+}  // namespace ktb
 }
 
 int ktb200_moe_forward_timed(ktb200_moe* m, int qlen, int k, const int64_t* ids, const float* weights, const void* input,

@@ -103,6 +103,8 @@ SYMBOLS = {
     "ktb200_moe_block_prefetch_hint": (_I, [_VP, _VP, _VP, _I]),
     "ktb200_ep_msg_bytes": (_L, [_I, _I]),
     "ktb200_moe_ep_block_forward": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _VP]),
+    "ktb200_ep_tokens_layout": (_L, [_I, _I, _I, _I, _I, _VP]),
+    "ktb200_moe_ep_forward_tokens": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _VP]),
     "ktb200_debug_block_trace": (None, [_VP]),
     "ktb200_debug_block_sync_words": (_L, [_VP, _VP, _L]),
     "ktb200_debug_stream_read": (_I, [_VP, _L, _I, _I, _I, _I, _VP, C.POINTER(C.c_float)]),
@@ -131,6 +133,31 @@ class EpComm(C.Structure):
         c._keep = (arr(tok_ptrs), arr(part_ptrs), arr(flag_ptrs))      # the host arrays must outlive the struct
         c.token_bufs, c.partial_bufs, c.flag_bufs = (C.cast(a, C.POINTER(C.c_void_p)) for a in c._keep)
         return c
+
+
+class EpTokensComm(C.Structure):
+    """ktb200_ep_tokens_comm (include/ktb200.h): every rank's region of the multi-token expert-parallel layer."""
+    _fields_ = [("rank", C.c_int), ("world", C.c_int), ("max_tokens_per_rank", C.c_int), ("hidden_size", C.c_int),
+                ("hidden_type", C.c_int), ("top_k", C.c_int), ("bufs", C.POINTER(C.c_void_p))]
+
+    @classmethod
+    def make(cls, rank, world, max_tokens_per_rank, hidden_size, hidden_type, top_k, buf_ptrs):
+        c = cls(rank, world, max_tokens_per_rank, hidden_size, hidden_type, top_k)
+        c._keep = (C.c_void_p * world)(*[int(x) for x in buf_ptrs])      # the host array must outlive the struct
+        c.bufs = C.cast(c._keep, C.POINTER(C.c_void_p))
+        return c
+
+
+EP_TOKENS_REGIONS = ("x", "ids", "weights", "partial", "scratch", "flags")
+
+
+def ep_tokens_layout(world: int, max_tokens_per_rank: int, hidden_size: int, hidden_type: int, top_k: int) -> tuple[int, dict]:
+    """(bytes, {region: byte offset}) of one rank's region of ktb200_moe_ep_forward_tokens."""
+    off = (C.c_long * 6)()
+    n = lib().ktb200_ep_tokens_layout(world, max_tokens_per_rank, hidden_size, hidden_type, top_k, off)
+    if n < 0:
+        check(EINVAL)
+    return int(n), dict(zip(EP_TOKENS_REGIONS, (int(o) for o in off)))
 
 
 def build(verbose: bool = False) -> str:

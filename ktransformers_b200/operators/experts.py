@@ -362,6 +362,11 @@ class _KDeepseekMoEMixin:
     KExpertsB200 take ONE call, `ktb200_moe_block_forward`: router, routed experts and shared expert in a single
     persistent launch, bit-identical to the three-step path below (include/ktb200.h).  The shared expert for that call
     is a `ktb200_mlp` handle built once from the raw GGUF tensors `<key>.shared_experts.{gate,up,down}_proj.weight`.
+
+    Sharded experts (expert_parallel_size > 1) need `ep_exchange` (attach_expert_parallel) and raise without it.  A step
+    with one token on every rank takes the one-launch decode kernel (`ktb200_moe_ep_block_forward`); any other step
+    (prompt chunks, ranks with different token counts, 0 included) takes `ktb200_moe_ep_forward_tokens` with the counts
+    announced by `ep_exchange.begin_step`.
     """
 
     BLOCK_MAX_TOKENS = 8
@@ -374,8 +379,9 @@ class _KDeepseekMoEMixin:
         if isinstance(gen, KExpertsB200) and gen.handle is not None and self.config.n_shared_experts is not None:
             self._shared_mlp_handle(gen)
 
-    def _block_handles(self, x):
-        """(gate_cfg, moe_handle, mlp_handle_or_None) when the single-launch path applies, else None."""
+    def _block_handles(self, x, need_mlp=True):
+        """(gate_cfg, moe_handle, mlp_handle_or_None) when the single-launch path applies, else None.  need_mlp=False: also
+        when the block's shared expert has no ktb200_mlp handle (mlp None then; the caller runs the shared module)."""
         gate, gen = getattr(self, "gate", None), getattr(getattr(self, "experts", None), "generate_experts", None)
         if not (isinstance(gen, KExpertsB200) and gen.handle is not None and x.is_cuda):
             return None
@@ -394,7 +400,7 @@ class _KDeepseekMoEMixin:
         mlp = None
         if self.config.n_shared_experts is not None:
             mlp = getattr(self, "_ktb_mlp", None)
-            if mlp is None:
+            if mlp is None and need_mlp:
                 return None
         return cfg, gen.handle, mlp
 
@@ -421,12 +427,57 @@ class _KDeepseekMoEMixin:
         self._ktb_mlp, self._ktb_mlp_raw = h, raw
         return h
 
+    def _ep_check(self, gen):
+        if getattr(gen, "ep_size", 1) > 1 and getattr(self, "ep_exchange", None) is None:
+            # without the exchange the shard's experts would return only their partial sum as the layer output
+            raise RuntimeError(f"{getattr(self, 'key', type(self).__name__)}: the experts are sharded (expert_parallel_size "
+                               f"{gen.ep_size}) but no expert-parallel exchange is attached (attach_expert_parallel)")
+
+    def ep_tokens_forward(self, hidden_states, phase_mask=7, counts=None):
+        """The sharded layer for any number of tokens on this rank (`ktb200_moe_ep_forward_tokens`); `counts` defaults to
+        this layer's take of the step's counts (`ep_exchange.take_step_counts`).  phase_mask 7 returns the output; 1, 2 and
+        4 run one phase each (1 takes the counts and keeps them with the routing and output buffers for 2 and 4; 4 returns
+        the output), so that one GPU can drive N ranks' blocks in loopback."""
+        orig_shape = hidden_states.shape
+        n_tok = hidden_states.numel() // orig_shape[-1]
+        hs = self._block_handles(hidden_states, need_mlp=False)
+        if hs is None:
+            raise RuntimeError(f"{getattr(self, 'key', type(self).__name__)}: the expert-parallel layer needs KMoEGateB200 routing and "
+                               "loaded KExpertsB200 experts of the hidden dtype in generate mode")
+        cfg, moe, mlp = hs
+        if phase_mask & 1 or getattr(self, "_ep_pending", None) is None:
+            counts = counts if counts is not None else self.ep_exchange.take_step_counts(n_tok)
+            if counts is None:
+                raise RuntimeError("expert-parallel step: no token counts were announced for this step; call "
+                                   "ep_exchange.begin_step(n_tokens) on every rank at the start of each forward step")
+            x = hidden_states.reshape(n_tok, orig_shape[-1]).contiguous()
+            self._ep_pending = (x, torch.empty_like(x), torch.empty((n_tok, cfg.top_k), dtype=torch.int64, device=x.device),
+                                torch.empty((n_tok, cfg.top_k), dtype=torch.float32, device=x.device), counts)
+        x, y, idx, wt, counts = self._ep_pending
+        native.check(native.lib().ktb200_moe_ep_forward_tokens(C.byref(cfg), moe, mlp, C.byref(self.ep_exchange.tok_comm), counts,
+                                                               x.data_ptr(), y.data_ptr(), idx.data_ptr(), wt.data_ptr(), phase_mask,
+                                                               _stream(x.device)))
+        if not phase_mask & 4:
+            return None
+        self._ep_pending = None
+        self.last_topk = (idx, wt)
+        y = y.view(*orig_shape)
+        if mlp is None and self.config.n_shared_experts is not None:
+            y = y + self.shared_experts(hidden_states).view(*orig_shape)       # two rounded terms, like the unsharded block
+        return y
+
     def forward(self, hidden_states):
         identity = hidden_states
         orig_shape = hidden_states.shape
         sequence_length = orig_shape[1]
         n_tok = hidden_states.numel() // orig_shape[-1]
         gen0 = getattr(getattr(self, "experts", None), "generate_experts", None)
+        self._ep_check(gen0)
+        if getattr(gen0, "ep_size", 1) > 1:
+            # one take per layer: None when no step was announced (then only the one-token decode case can run)
+            counts = self.ep_exchange.take_step_counts(n_tok)
+            if n_tok != 1 or (counts is not None and any(c != 1 for c in counts)):
+                return self.ep_tokens_forward(hidden_states, counts=counts)
         if getattr(gen0, "ep_size", 1) > 1 and n_tok == 1:
             # expert-parallel decode, one token per GPU: router, NVLink exchange, owned experts and combine in ONE launch
             hs = self._block_handles(hidden_states)
@@ -441,6 +492,7 @@ class _KDeepseekMoEMixin:
                                                                       y.data_ptr(), idx.data_ptr(), wt.data_ptr(), 7, _stream(x.device)))
                 self.last_topk = (idx, wt)
                 return y.view(*orig_shape)
+            return self.ep_tokens_forward(hidden_states, counts=counts)
         if n_tok <= self.BLOCK_MAX_TOKENS and getattr(gen0, "ep_size", 1) == 1:
             hs = self._block_handles(hidden_states)
             if hs is not None:
@@ -518,10 +570,14 @@ class KDeepseekV2MoE(_KDeepseekMoEMixin, BaseInjectedModule, _V2):
 
 class KDeepseekV3MoEV2(_KDeepseekMoEMixin, BaseInjectedModule, _V3):
     """experts.py:1172-1271: `forward(hidden_states, bsz_tensor, cuda_graph_idx)`; rows at or beyond `bsz_tensor[0]` are padding
-    and are left untouched by every kernel (kt-kernel/operators/common.hpp:255-258 semantics, on the device)."""
+    and are left untouched by every kernel (kt-kernel/operators/common.hpp:255-258 semantics, on the device).
+
+    Except under expert parallelism (sharded experts): the exchange works on host-known token counts, so `bsz_tensor` is
+    not read, and every row of the chunk, padding included, is computed and written like a real token."""
 
     def forward(self, hidden_states, bsz_tensor=None, cuda_graph_idx=0):
-        if bsz_tensor is None:
+        gen0 = getattr(getattr(self, "experts", None), "generate_experts", None)
+        if bsz_tensor is None or getattr(gen0, "ep_size", 1) > 1:
             return super().forward(hidden_states)
         identity, orig_shape = hidden_states, hidden_states.shape
         n_tok = hidden_states.numel() // orig_shape[-1]
