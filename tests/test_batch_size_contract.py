@@ -387,6 +387,10 @@ CASES = {
     "linear-q4k-7168x2112": lambda: linear_case(6, Q4_K, 7168, 2112, False),
     "linear-q4k-7168x2112-bias": lambda: linear_case(8, Q4_K, 7168, 2112, True),
     "linear-q4k-256x777-bias": lambda: linear_case(5, Q4_K, 256, 777, True),
+    # prompt-sized batches: rows_bulk_q4k_kernel in token chunks of 8, rows_kernel (rows under 16 blocks), the Q5_K pipe kernel
+    "linear-q4k-bulk-T40-bias": lambda: linear_case(40, Q4_K, 7168, 1536, True),
+    "linear-q4k-rows-T20-bias": lambda: linear_case(20, Q4_K, 1536, 2048, True),
+    "linear-q5k-pipe-T12-bias": lambda: linear_case(12, Q5_K, 7168, 1536, True),
     # ktb200_mlp_forward
     "mlp": lambda: mlp_case(6, 0),
     "mlp-accumulate": lambda: mlp_case(6, 1),
@@ -410,8 +414,9 @@ def test_bsz_contract_eager(name):
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_bsz_contract_graph_replay(name):
+    """batches of more than 16 tokens also replay with a live count inside a later token chunk"""
     case = CASES[name]()
-    contract_graph(case, REPLAY_BS + (case.qlen,))
+    contract_graph(case, REPLAY_BS + ((case.qlen // 2 + 1,) if case.qlen > 16 else ()) + (case.qlen,))
 
 
 def test_fp8_case_shapes_pick_the_k_splits():

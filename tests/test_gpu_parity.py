@@ -266,7 +266,9 @@ def test_linear_and_mlp_vs_golden(golden_dir):
 @pytest.mark.parametrize("t,in_f,out_f", [(Q4_K, 7168, 1536), (Q6_K, 2048, 7168), (Q5_K, 1536, 512), (Q6_K, 512, 100), (Q3_K, 256, 64),
                                            # the dense segment-ring kernel (dense_bulk.cuh): 5 rows per segment with a ragged tail,
                                            # two and three segments per row, one block per row
-                                           (Q4_K, 1536, 2048 + 3), (Q4_K, 16384, 512), (Q4_K, 18432, 256), (Q4_K, 256, 777), (Q4_K, 7168, 2112)])
+                                           (Q4_K, 1536, 2048 + 3), (Q4_K, 16384, 512), (Q4_K, 18432, 256), (Q4_K, 256, 777), (Q4_K, 7168, 2112),
+                                           # Q2_K and IQ4_XS linears (generic kernel)
+                                           (Q2_K, 1024, 512), (IQ4_XS, 2048, 256)])
 def test_linear_vs_oracle(oracle, t, in_f, out_f):
     w = _synth(t, out_f * in_f, 31)
     w_np = w.cpu().numpy()
