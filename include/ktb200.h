@@ -42,7 +42,9 @@ enum ktb200_ggml_type {
      *   IQ1_S    50 B: fp16 d, qs[32], qh uint16[8]; sub-block ib has ls = 2*((qh>>12)&7)+1, delta = qh bit 15 ? -1/8 : +1/8,
      *            group l = iq1s_grid[qs[4ib+l] | ((qh >> 3l) & 7) << 8]; value = d*ls*(grid + delta)
      * vec_dot_type Q8_K.  Routed experts only (ktb200_moe_create, any mix with the K-quants); linears, MLP handles and the
-     * expert-parallel entry points reject them.  The codebooks are ktransformers_b200/csrc/iq_tables.h. */
+     * one-token expert-parallel entry points reject them.  ktb200_moe_forward runs them per (token, expert) pair below 80
+     * tokens and on the grouped tensor-core GEMM from 80 (gate, up and down each in its own format).  The codebooks are
+     * ktransformers_b200/csrc/iq_tables.h. */
     KTB200_TYPE_IQ2_XXS = 16, KTB200_TYPE_IQ1_S = 19,
     /* Not a ggml type: ggml's ids stay below 64, so 256 cannot collide with one.
      * Symmetric INT4 in groups of 32 with bf16 scales (compressed-tensors "pack-quantized", kt-kernel's RAWINT4; Kimi-K2's

@@ -152,6 +152,21 @@ __device__ __forceinline__ float warp_sum(float v) {
 // ------------------------------------------------------------------ hidden-type conversions
 __device__ __forceinline__ float fp16_bits_to_f32(uint16_t h) { return __half2float(__ushort_as_half(h)); }
 
+// ------------------------------------------------------------------ IQ1_S / IQ2_XXS arithmetic shared by iq.cuh and grouped.cu
+// a super-block's fp32 term (DESIGN.md §2): ((d / 8) * dx) * S with the exact integer S of the super-block
+__device__ __forceinline__ float iq_d8(uint16_t d_bits) { return fp16_bits_to_f32(d_bits) * 0.125f; }
+__device__ __forceinline__ float iq_term(float d8, float dx, int isum) { return (d8 * dx) * (float)isum; }
+// an IQ2_XXS sign pattern (ksigns_iq2xs byte) as byte masks: value = (grid ^ m) - m per byte
+__device__ __forceinline__ uint2 iq2_sign_masks(uint32_t s) {
+    uint32_t lo = 0, hi = 0;
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+        lo |= ((s >> j) & 1u) ? 0xffu << (8 * j) : 0u;
+        hi |= ((s >> (j + 4)) & 1u) ? 0xffu << (8 * j) : 0u;
+    }
+    return make_uint2(lo, hi);
+}
+
 // ggml_compute_fp32_to_bf16 (third_party/llama.cpp/ggml-impl.h:87-104): RNE, NaN quieted,
 // fp32 subnormals flushed to signed zero.
 __device__ __forceinline__ uint16_t f32_to_bf16_ggml(float f) {

@@ -20,12 +20,24 @@
 //     warps 8-15   two MMA warpgroups, 64 weight rows each: the integer MMAs of a stage (+ the mins MMA on the second half),
 //                  int32 scale-and-add in registers, fp32 finish per super-block, stores at the end of the tile; 3 shared-memory
 //                  stages between the two roles
+//
+// IQ1_S (FMT 2) and IQ2_XXS (FMT 3), DeepSeek-R1's codebook experts: 32-value sub-blocks with one odd integer scale ls each and
+// no mins, so the Q4_K shape minus its mins MMA.  The producers expand the codebooks (staged in shared memory from iq_tables.h)
+// into the s8 A tile — IQ1_S 8 * grid + delta (-9..9), IQ2_XXS +-grid — the operands the decode kernels (iq.cuh) feed to dp4a;
+// one s8.s8 K = 32 MMA per sub-block, isum += ls * that, and per super-block the decode kernels' iq_term((d/8), dx, isum).
+// The raw blocks (50 / 66 B) are only 2-byte aligned: a producer fetches the aligned 4-byte words that cover its bytes with
+// cp.async and funnel-shifts them by 16 bits when the block starts on an odd half-word (the block parity, tracked per row).
+// That keeps the Q4_K producers' asynchronous 6-stage prefetch; 16-bit loads staged in registers would hold those stages in
+// the producers' 96 registers and take two to four times the load instructions.  Their own shared-memory plan: no mins tiles,
+// 32-row B, 48-byte raw slots and the 16 KB codebook in place of the Q4_K / Q6_K plan's 80-byte slots.
 #include <cuda_fp16.h>
 
 #include "act_quant.cuh"
 #include "common.cuh"
 #include "handles.cuh"
 #include "wgmma.cuh"
+#define KTB_IQ_TABLE static __device__ const
+#include "iq_tables.h"
 
 namespace ktb {
 
@@ -48,6 +60,13 @@ struct GrpMisc {
 };
 constexpr int kGSmem = kOffMiscG + (int)sizeof(GrpMisc) + 1024;
 static_assert(kGSmem <= 227 * 1024, "shared memory budget");
+// IQ1_S / IQ2_XXS plan: A stages as above, B of 32 token rows, raw slots of three 16-byte units per thread (0-1 the covering
+// weight words and the word of d, 24 the token scale, 2 the activation piece), the codebook (IQ1_S 2048 x 8 B; IQ2_XXS 256 x 8 B
+// grid + 128 x 8 B sign masks), the same misc block
+constexpr int kGBI = kGN * 128, kRawPitchI = 48, kRawSlotI = 2 * kGM * kRawPitchI, kTabI = 2048 * 8;
+constexpr int kOffBI = kGStages * kGA, kOffRawI = kOffBI + kGStages * kGBI, kOffTabI = kOffRawI + kGRaw * kRawSlotI, kOffMiscI = kOffTabI + kTabI;
+constexpr int kGSmemI = kOffMiscI + (int)sizeof(GrpMisc) + 1024;
+static_assert(kGSmemI <= 227 * 1024 && kOffBI % 1024 == 0 && kGBI % 1024 == 0, "IQ shared-memory plan");
 
 struct GrpGemmParams {
     const uint8_t* w;          // expert weights
@@ -103,15 +122,28 @@ __global__ void grp_tiles_kernel(const int* nt_prefix, const int* offsets, int E
 //   Q4_K: 0-1 the 32 bytes of qs of chunk 2 hh + part, 2 block header, 3 activation piece, 4 activation 16-sums (threads 0-63) or
 //         token scale (threads 64-95)
 //   Q6_K: 0-1 ql (16 bytes at l and at 32 + l), 2 qh, 3 activation piece, 4 = 8 scales | d (2 of 4 bytes) | token scale (threads 64-95)
+//   IQ (three units, sub-blocks 4 hh + 2 part + {0, 1}): IQ1_S bytes 0-11 the words covering qs[8 (2 hh + part) .. + 8],
+//         12-19 those covering qh[2 (2 hh + part) .. + 2]; IQ2_XXS 0-19 those covering the 16 bytes of the two sub-blocks;
+//         20 the word holding d, 24 token scale (threads 64-95), 2 activation piece
 template <int FMT>
 __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGemmParams p) {
+    constexpr bool IQ = FMT >= 2;
+    constexpr int offB = IQ ? kOffBI : kOffB, strideB = IQ ? kGBI : kGB, offRaw = IQ ? kOffRawI : kOffRaw, rawPitch = IQ ? kRawPitchI : kRawPitch,
+                  rawSlot = IQ ? kRawSlotI : kRawSlot, BS = FMT == 2 ? SZ_IQ1_S : SZ_IQ2_XXS;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base - raw);
-    GrpMisc& misc = *reinterpret_cast<GrpMisc*>(smem + kOffMiscG);
+    GrpMisc& misc = *reinterpret_cast<GrpMisc*>(smem + (IQ ? kOffMiscI : kOffMiscG));
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nblk = p.Kc / QK_K, nst = 2 * nblk, MT = p.R / kGM;
+    uint2* tab = reinterpret_cast<uint2*>(smem + kOffTabI);   // IQ codebooks (read after the __syncthreads below)
+    if (FMT == 2) {
+        for (int i = tid; i < 2048; i += kGThreads) tab[i] = *reinterpret_cast<const uint2*>(ktb_iq1s_grid[i]);
+    } else if (FMT == 3) {
+        for (int i = tid; i < 256; i += kGThreads) tab[i] = *reinterpret_cast<const uint2*>(ktb_iq2xxs_grid[i]);
+        if (tid < 128) tab[256 + tid] = iq2_sign_masks(ktb_ksigns_iq2xs[tid]);
+    }
     if (tid == 0) {
         for (int s = 0; s < kGStages; s++) { bar_init(smem_u32(&misc.ab_full[s]), kGProdWarps); bar_init(smem_u32(&misc.smem_free[s]), kGMmaWarps); }
         for (int s = 0; s < kGHdr; s++) bar_init(smem_u32(&misc.hdr_free[s]), kGMmaWarps);
@@ -127,8 +159,8 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
         // `part` is warp-uniform (warps 0-3: first half of the row's share, warps 4-7: second) so that no branch below diverges
         regs_dec<96>();
         const int pt = tid, r = pt & (kGM - 1), part = pt >> 7, sw = r & 7, bn = pt >> 3, pc = pt & 7;
-        const uint32_t raw_dst = base + kOffRaw + pt * kRawPitch;
-        const uint8_t* raw_src = smem + kOffRaw + pt * kRawPitch;
+        const uint32_t raw_dst = base + offRaw + pt * rawPitch;
+        const uint8_t* raw_src = smem + offRaw + pt * rawPitch;
         const int c16 = 4 * nblk * 16;   // Q6_K tiles: bytes between two 16-byte chunk planes of an item
         // fetch cursor: runs kGRaw stages ahead of the conversion, across tile boundaries; plain running pointers
         int ftile = blockIdx.x, fst = 0, ffi = 0;
@@ -145,6 +177,7 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
             if (pt >= 64 && pt < 96 && pt - 64 < ti.w) fdx = p.xd + (long)(p.rowmap ? __ldg(p.rowmap + ti.z + pt - 64) : ti.z + pt - 64) * nblk;
             const int row = ti.y + r;
             if (FMT == 0) fw = p.w + (long)ti.x * p.expert_bytes + (long)row * nblk * SZ_Q4_K + 16 + part * 32;   // this thread's qs of block 0, first half
+            else if (IQ) fw = p.w + (long)ti.x * p.expert_bytes + (long)row * nblk * BS;                         // block 0 of the row
             else {
                 fitem = p.w + (long)ti.x * p.expert_bytes + (long)(row >> 2) * 4 * nblk * SZ_Q6_K;
                 ffi = (row & 3) * nblk;
@@ -159,6 +192,25 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                     cp_async16(dst, q);
                     cp_async16(dst + 16, q + 16);
                     if (part == 0 || hh == 1) cp_async16(dst + 32, fw - 16 - part * 32);
+                } else if (IQ) {
+                    // every word fetched holds at least one byte this thread needs (so it lies inside the tensor's pages);
+                    // the last word of a field is only needed when the block starts on a word (the fields then start mid-word)
+                    const int q = 2 * hh + part;
+                    const bool mid = (reinterpret_cast<uintptr_t>(fw) & 2) == 0;
+                    const uint8_t* qs = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(fw + 2 + (FMT == 2 ? 8 : 16) * q) & ~(uintptr_t)3);
+                    cp_async4(dst, qs);
+                    cp_async4(dst + 4, qs + 4);
+                    if (FMT == 2) {
+                        if (mid) cp_async4(dst + 8, qs + 8);
+                        const uint8_t* qh = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(fw + 34 + 4 * q) & ~(uintptr_t)3);
+                        cp_async4(dst + 12, qh);
+                        if (mid) cp_async4(dst + 16, qh + 4);
+                    } else {
+                        cp_async4(dst + 8, qs + 8);
+                        cp_async4(dst + 12, qs + 12);
+                        if (mid) cp_async4(dst + 16, qs + 16);
+                    }
+                    cp_async4(dst + 20, reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(fw) & ~(uintptr_t)3));
                 } else {
                     const uint8_t* q = fw + (long)(4 * hh) * c16;
                     cp_async16(dst, q);
@@ -169,11 +221,11 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                         cp_async4(dst + 72, fitem + (long)13 * c16 + (ffi >> 1) * 4);
                     }
                 }
-                if (fxq) { cp_async16(dst + 48, fxq); fxq += 128; }
+                if (fxq) { cp_async16(dst + (IQ ? 32 : 48), fxq); fxq += 128; }
                 if (hh == 1) {
                     if (FMT == 0 && fbs) { cp_async16(dst + 64, fbs); fbs += 16; }
-                    if (fdx) { cp_async4(dst + (FMT == 0 ? 64 : 76), fdx); fdx += 1; }
-                    fw += FMT == 0 ? SZ_Q4_K : 16;
+                    if (fdx) { cp_async4(dst + (FMT == 0 ? 64 : IQ ? 24 : 76), fdx); fdx += 1; }
+                    fw += FMT == 0 ? SZ_Q4_K : IQ ? BS : 16;
                     ffi++;
                 }
                 if (++fst == nst) { fst = 0; ftile += gridDim.x; enter_tile(); }
@@ -181,21 +233,24 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
             cp_async_commit();
         };
         enter_tile();
-        for (int i = 0; i < kGRaw; i++) issue(raw_dst + i * kRawSlot);
+        for (int i = 0; i < kGRaw; i++) issue(raw_dst + i * rawSlot);
         int slot = 0;
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int4 ti = __ldg(p.tinfo + tile);
             const int n_valid = ti.w;
             int dsel = ((ti.y + r) & 3) * nblk;   // Q6_K: which half of the fetched word holds this block's d
+            // IQ: 16 when the current block starts on a word (its fields then start mid-word), else 0; 50 and 66 are 2 mod 4,
+            // so it alternates block by block
+            uint32_t ish = IQ ? ((reinterpret_cast<uintptr_t>(p.w + (long)ti.x * p.expert_bytes + (long)(ti.y + r) * nblk * BS) & 2) ? 0u : 16u) : 0u;
             for (int st = 0; st < nst; st++) {
                 const int hh = st & 1;
                 const bool tr = p.trace && blockIdx.x == 0 && tid == 0 && tile == 0 && st < 96;
                 if (tr) p.trace[(0 * 96 + st) * 4 + 0] = clock64();
                 cp_async_wait<kGRaw - 1>();
                 if (tr) p.trace[(0 * 96 + st) * 4 + 1] = clock64();
-                const uint4* rs = reinterpret_cast<const uint4*>(raw_src + slot * kRawSlot);
-                const uint4 f0 = rs[0], f1 = rs[1], f2 = rs[2], f3 = rs[3], f4 = rs[4];
-                issue(raw_dst + slot * kRawSlot);   // refill the slot just read (thread-private bytes: no barrier involved)
+                const uint4* rs = reinterpret_cast<const uint4*>(raw_src + slot * rawSlot);
+                const uint4 f0 = rs[0], f1 = rs[1], f2 = rs[2], f3 = rs[IQ ? 2 : 3], f4 = rs[IQ ? 1 : 4];
+                issue(raw_dst + slot * rawSlot);   // refill the slot just read (thread-private bytes: no barrier involved)
                 slot = slot == kGRaw - 1 ? 0 : slot + 1;
                 bar_wait(smem_u32(&misc.smem_free[stage]), sphase ^ 1);
                 bar_wait(smem_u32(&misc.hdr_free[hs]), hphase ^ 1);
@@ -225,6 +280,43 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                         uint8_t* a2 = smem + kOffA2 + stage * kGA2 + (r >> 3) * 256 + (r & 7) * 16 + part * 128;
                         *reinterpret_cast<uint4*>(a2) = make_uint4(h2(mn[0], mn[0]), h2(mn[1], mn[1]), h2(mn[2], mn[2]), h2(mn[3], mn[3]));
                     }
+                } else if (IQ) {
+                    // sub-block 4 hh + 2 part + j -> A chunks 4 part + 2 j and 4 part + 2 j + 1; header word `part` = its two ls
+                    // (16 bits each), word 2 = d / 8 as f32
+                    const uint32_t w[5] = {f0.x, f0.y, f0.z, f0.w, f1.x};
+                    const uint32_t dbits = ish ? (f1.y & 0xffffu) : (f1.y >> 16);
+                    uint32_t ls[2];
+#pragma unroll
+                    for (int j = 0; j < 2; j++) {
+                        uint32_t v[8];
+                        if (FMT == 2) {   // 8 * grid + delta, delta = qh bit 15 ? -1 : +1 per byte
+                            const uint32_t qs = __funnelshift_r(w[j], w[j + 1], ish), qh = __funnelshift_r(w[3], w[4], ish) >> (16 * j);
+                            const uint32_t dl = (qh & 0x8000u) ? 0xffffffffu : 0x01010101u;
+#pragma unroll
+                            for (int l = 0; l < 4; l++) {
+                                const uint2 g = tab[((qs >> (8 * l)) & 0xffu) | (((qh >> (3 * l)) & 7u) << 8)];
+                                v[2 * l] = __vadd4((g.x << 3) & 0xf8f8f8f8u, dl);
+                                v[2 * l + 1] = __vadd4((g.y << 3) & 0xf8f8f8f8u, dl);
+                            }
+                            ls[j] = 2 * ((qh >> 12) & 7u) + 1;
+                        } else {          // +-grid through the sign masks
+                            const uint32_t aux0 = __funnelshift_r(w[2 * j], w[2 * j + 1], ish), aux1 = __funnelshift_r(w[2 * j + 1], w[2 * j + 2], ish);
+#pragma unroll
+                            for (int l = 0; l < 4; l++) {
+                                const uint2 g = tab[(aux0 >> (8 * l)) & 0xffu], m = tab[256 + ((aux1 >> (7 * l)) & 127u)];
+                                v[2 * l] = __vsub4(g.x ^ m.x, m.x);
+                                v[2 * l + 1] = __vsub4(g.y ^ m.y, m.y);
+                            }
+                            ls[j] = 2 * (aux1 >> 28) + 1;
+                        }
+                        const int c0 = 4 * part + 2 * j;
+                        *reinterpret_cast<uint4*>(arow + (((c0 + 0) ^ sw) << 4)) = make_uint4(v[0], v[1], v[2], v[3]);
+                        *reinterpret_cast<uint4*>(arow + (((c0 + 1) ^ sw) << 4)) = make_uint4(v[4], v[5], v[6], v[7]);
+                    }
+                    uint32_t* hrow = reinterpret_cast<uint32_t*>(&misc.hdr[hs][r]);
+                    hrow[part] = ls[0] | (ls[1] << 16);
+                    if (part == 0) hrow[2] = __float_as_uint(iq_d8((uint16_t)dbits));
+                    if (hh == 1) ish ^= 16u;
                 } else {
                     // element 32 g + l of the half (l = 16 part + 0..15): g = 0 ql[l] & 15 | (qh & 3) << 4, g = 1 ql[32 + l] & 15 | (qh >> 2 & 3) << 4,
                     // g = 2 ql[l] >> 4 | (qh >> 4 & 3) << 4, g = 3 ql[32 + l] >> 4 | (qh >> 6 & 3) << 4; stored as q - 32 in int8
@@ -253,16 +345,16 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                     dsel += hh;
                 }
                 // activations: piece (bn, pc)
-                uint8_t* Bs = smem + kOffB + stage * kGB;
+                uint8_t* Bs = smem + offB + stage * strideB;
                 const uint4 bv = bn < n_valid ? f3 : z;
-                if (FMT == 0) {
+                if (FMT != 1) {
                     *reinterpret_cast<uint4*>(Bs + bn * 128 + ((pc ^ (bn & 7)) << 4)) = bv;
                 } else {   // a 16-byte piece is one Q6_K sub-block: rows 0-31 keep the even pieces, rows 32-63 the odd ones
                     *reinterpret_cast<uint4*>(Bs + bn * 128 + ((pc ^ (bn & 7)) << 4)) = (pc & 1) ? z : bv;
                     *reinterpret_cast<uint4*>(Bs + (kGN + bn) * 128 + ((pc ^ (bn & 7)) << 4)) = (pc & 1) ? bv : z;
                 }
                 if (hh == 1 && pt < 96) {   // token scales, and (Q4_K) the sixteen 16-value sums of the super-block as fp16
-                    if (pt >= 64) misc.dxs[hs][pt - 64] = pt - 64 < n_valid ? __uint_as_float(FMT == 0 ? f4.x : f4.w) : 0.f;
+                    if (pt >= 64) misc.dxs[hs][pt - 64] = pt - 64 < n_valid ? __uint_as_float(FMT == 0 ? f4.x : IQ ? f4.z : f4.w) : 0.f;
                     else if (FMT == 0) {
                         const int n2 = pt >> 1, kg = pt & 1;
                         uint4 vv = z;
@@ -303,7 +395,7 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                 if (tr) p.trace[(1 * 96 + st) * 4 + 0] = clock64();
                 bar_wait(smem_u32(&misc.ab_full[stage]), sphase);
                 if (tr) p.trace[(1 * 96 + st) * 4 + 1] = clock64();
-                const uint32_t a = base + stage * kGA + g * (kGA / 2), b = base + kOffB + stage * kGB;
+                const uint32_t a = base + stage * kGA + g * (kGA / 2), b = base + offB + stage * strideB;
                 uint32_t hw[2][4];
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
@@ -349,6 +441,31 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                             const float dw = __low2float(dm), dmin = __high2float(dm);
                             const float dx = misc.dxs[hs][8 * (i >> 2) + cq + (i & 1)];
                             acc[i] += (dw * dx) * (float)isum[i] - (dmin * dx) * ms[i];
+                            isum[i] = 0;
+                        }
+                    }
+                } else if (IQ) {
+                    // sub-block c of the stage: one MMA into its own accumulator, times its ls (header word c / 2, half c % 2)
+#pragma unroll
+                    for (int c = 0; c < 4; c += 2) {
+                        uint32_t v0[16], v1[16];
+                        fence();
+                        mma_s8s8_m64n32(v0, smem_desc(a + c * 32, 16, 1024, kLayoutSw128), smem_desc(b + c * 32, 16, 1024, kLayoutSw128), 0);
+                        mma_s8s8_m64n32(v1, smem_desc(a + c * 32 + 32, 16, 1024, kLayoutSw128), smem_desc(b + c * 32 + 32, 16, 1024, kLayoutSw128), 0);
+                        commit();
+                        wait<0>();
+                        fence_regs(v0);
+                        fence_regs(v1);
+#pragma unroll
+                        for (int i = 0; i < 16; i++) {
+                            const uint32_t lw = hw[(i >> 1) & 1][c >> 1];
+                            isum[i] += (int)(lw & 0xffffu) * (int)v0[i] + (int)(lw >> 16) * (int)v1[i];
+                        }
+                    }
+                    if (hh == 1) {
+#pragma unroll
+                        for (int i = 0; i < 16; i++) {
+                            acc[i] += iq_term(__uint_as_float(hw[(i >> 1) & 1][2]), misc.dxs[hs][8 * (i >> 2) + cq + (i & 1)], isum[i]);
                             isum[i] = 0;
                         }
                     }
@@ -500,11 +617,30 @@ static int grp_ensure(int dev, int tokens, int k, int E, int H, int I) {
     return KTB200_OK;
 }
 
-// true when ktb200_moe_forward may take the grouped tensor-core path for this handle
+// the grouped_gemm_kernel format of one weight tensor (gate, up and down are separate launches), -1: none.  Q6_K only in the
+// 4-row tile layout, which ktb200_moe_load_weights gives down tensors of eligible shapes.
+static int grouped_fmt(int type, int layout) {
+    if (type == KTB200_TYPE_Q4_K) return 0;
+    if (type == KTB200_TYPE_Q6_K && layout == LAYOUT_T4) return 1;
+    if (type == KTB200_TYPE_IQ1_S) return 2;
+    if (type == KTB200_TYPE_IQ2_XXS) return 3;
+    return -1;
+}
+static void grouped_gemm(int fmt, const GrpGemmParams& p, int grid, cudaStream_t s) {
+    switch (fmt) {
+        case 0: grouped_gemm_kernel<0><<<grid, kGThreads, kGSmem, s>>>(p); break;
+        case 1: grouped_gemm_kernel<1><<<grid, kGThreads, kGSmem, s>>>(p); break;
+        case 2: grouped_gemm_kernel<2><<<grid, kGThreads, kGSmemI, s>>>(p); break;
+        default: grouped_gemm_kernel<3><<<grid, kGThreads, kGSmemI, s>>>(p); break;
+    }
+}
+
+// true when ktb200_moe_forward may take the grouped tensor-core path for this handle: gate and up Q4_K, IQ1_S or IQ2_XXS (each
+// on its own), down any of those or Q6_K in the tile layout
 bool grouped_ok(const ktb200_moe* m, int k) {
     const ktb200_moe_config& c = m->cfg;
-    const FmtId fd = pick_fmt(c.down_type, m->down_layout);
-    return c.gate_type == KTB200_TYPE_Q4_K && c.up_type == KTB200_TYPE_Q4_K && (fd == FMT_Q6K4T || fd == FMT_Q4K) && c.hidden_size % 256 == 0 &&
+    const int fg = grouped_fmt(c.gate_type, LAYOUT_RAW), fu = grouped_fmt(c.up_type, LAYOUT_RAW), fd = grouped_fmt(c.down_type, m->down_layout);
+    return fg >= 0 && fg != 1 && fu >= 0 && fu != 1 && fd >= 0 && c.hidden_size % 256 == 0 &&
            c.intermediate_size % 256 == 0 && c.hidden_size % kGM == 0 && c.intermediate_size % kGM == 0 && c.expert_num <= 1023 && k <= 32;
 }
 
@@ -521,9 +657,11 @@ int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, cons
     if (!attr[dev & 63]) {
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem));
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmemI));
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmemI));
         attr[dev & 63] = true;
     }
-    const FmtId fd = pick_fmt(c.down_type, m->down_layout);
+    const int fg = grouped_fmt(c.gate_type, LAYOUT_RAW), fu = grouped_fmt(c.up_type, LAYOUT_RAW), fd = grouped_fmt(c.down_type, m->down_layout);
     const size_t hb = type_size(c.hidden_type), ob = type_size(out_type);
     const int grid = num_sms(dev);
     for (int t0 = 0; t0 < qlen; t0 += Tc) {
@@ -542,18 +680,18 @@ int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, cons
         grp_quant_x_kernel<<<(T * (H / 256) + 7) / 8, 256, 0, s>>>(x_c, c.hidden_type, T, H, g.xq, g.xd, g.xbs);
         GrpGemmParams gp{};
         gp.R = I; gp.Kc = H; gp.xq = g.xq; gp.xd = g.xd; gp.xbs = g.xbs; gp.rowmap = g.tokmap; gp.tinfo = g.tinfo_gu; gp.nt_prefix = g.nt_prefix; gp.E = E;
-        gp.expert_bytes = (long)I * (H / 256) * SZ_Q4_K;
+        gp.expert_bytes = (long)I * (H / 256) * weight_block_bytes(c.gate_type);
         gp.w = reinterpret_cast<const uint8_t*>(c.gate_proj); gp.out = g.g; gp.trace = g_grp_trace;
-        grouped_gemm_kernel<0><<<grid, kGThreads, kGSmem, s>>>(gp);
+        grouped_gemm(fg, gp, grid, s);
+        gp.expert_bytes = (long)I * (H / 256) * weight_block_bytes(c.up_type);
         gp.w = reinterpret_cast<const uint8_t*>(c.up_proj); gp.out = g.u; gp.trace = nullptr;
-        grouped_gemm_kernel<0><<<grid, kGThreads, kGSmem, s>>>(gp);
+        grouped_gemm(fu, gp, grid, s);
         grp_act_quant_kernel<<<(P * (I / 256) + 7) / 8, 256, 0, s>>>(g.g, g.u, g.offsets, E, I, c.use_silu, g.aq, g.ad, g.abs16);
         GrpGemmParams gd{};
         gd.R = H; gd.Kc = I; gd.xq = g.aq; gd.xd = g.ad; gd.xbs = g.abs16; gd.rowmap = nullptr; gd.tinfo = g.tinfo_d; gd.nt_prefix = g.nt_prefix;
-        gd.E = E; gd.expert_bytes = (long)H * (I / 256) * (fd == FMT_Q6K4T ? SZ_Q6_K : SZ_Q4_K);
+        gd.E = E; gd.expert_bytes = (long)H * (I / 256) * weight_block_bytes(c.down_type);
         gd.w = reinterpret_cast<const uint8_t*>(c.down_proj); gd.out = g.dd; gd.trace = g_grp_trace ? g_grp_trace + 3 * 96 * 4 : nullptr;
-        if (fd == FMT_Q6K4T) grouped_gemm_kernel<1><<<grid, kGThreads, kGSmem, s>>>(gd);
-        else grouped_gemm_kernel<0><<<grid, kGThreads, kGSmem, s>>>(gd);
+        grouped_gemm(fd, gd, grid, s);
         grp_combine_kernel<<<dim3((H + 255) / 256, T), 256, 0, s>>>(g.dd, g.pos, w_c, T, k, H, bsz, t0, o_c, out_type);
         KTB_LAUNCH_CHECK();
         count_launch(9);   // + the one KTB_LAUNCH_CHECK counts = 10 launches per chunk

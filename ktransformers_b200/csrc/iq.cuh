@@ -41,7 +41,7 @@ struct BulkIQ1S {
     // one super-block at `wb` (shared memory, 2-byte aligned) against one padded int8 activation block
     __device__ static __forceinline__ float block_dot(const uint8_t* wb, const uint8_t* aq, const int16_t* bs32, float dxb) {
         const uint2* grid = iq1s_grid_smem();
-        const float d = fp16_bits_to_f32(*reinterpret_cast<const uint16_t*>(wb)) * 0.125f;
+        const float d = iq_d8(*reinterpret_cast<const uint16_t*>(wb));
         int isum = 0;
 #pragma unroll
         for (int ib = 0; ib < 8; ib++) {
@@ -65,7 +65,7 @@ struct BulkIQ1S {
             const int ls = 2 * (int)((qh >> 12) & 7) + 1;
             isum += ls * (8 * s + ((qh & 0x8000u) ? -b : b));
         }
-        return (d * dxb) * (float)isum;
+        return iq_term(d, dxb, isum);
     }
     __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int /*nrb*/, const uint8_t* aq, const int16_t* bs, float dxb) {
         return block_dot(sl + f * SZ_IQ1_S, aq, bs, dxb);
@@ -81,21 +81,12 @@ struct BulkIQ2XXS {
         uint2* g = iq2xxs_grid_smem();
         uint2* m = iq2xxs_signs_smem();
         for (int i = threadIdx.x; i < 256; i += blockDim.x) g[i] = *reinterpret_cast<const uint2*>(ktb_iq2xxs_grid[i]);
-        for (int i = threadIdx.x; i < 128; i += blockDim.x) {
-            const uint32_t s = ktb_ksigns_iq2xs[i];
-            uint32_t lo = 0, hi = 0;
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-                lo |= ((s >> j) & 1u) ? 0xffu << (8 * j) : 0u;
-                hi |= ((s >> (j + 4)) & 1u) ? 0xffu << (8 * j) : 0u;
-            }
-            m[i] = make_uint2(lo, hi);
-        }
+        for (int i = threadIdx.x; i < 128; i += blockDim.x) m[i] = iq2_sign_masks(ktb_ksigns_iq2xs[i]);
     }
     __device__ static __forceinline__ float block_dot(const uint8_t* wb, const uint8_t* aq, const int16_t* /*bs32*/, float dxb) {
         const uint2* grid = iq2xxs_grid_smem();
         const uint2* sgn = iq2xxs_signs_smem();
-        const float d = fp16_bits_to_f32(*reinterpret_cast<const uint16_t*>(wb)) * 0.125f;
+        const float d = iq_d8(*reinterpret_cast<const uint16_t*>(wb));
         int isum = 0;
 #pragma unroll
         for (int ib = 0; ib < 8; ib++) {
@@ -113,7 +104,7 @@ struct BulkIQ2XXS {
             }
             isum += (2 * (int)(aux1 >> 28) + 1) * s;
         }
-        return (d * dxb) * (float)isum;
+        return iq_term(d, dxb, isum);
     }
     __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int /*nrb*/, const uint8_t* aq, const int16_t* bs, float dxb) {
         return block_dot(sl + f * SZ_IQ2_XXS, aq, bs, dxb);

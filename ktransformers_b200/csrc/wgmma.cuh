@@ -135,6 +135,14 @@ __device__ __forceinline__ void mma_u8s8_m64n32(uint32_t (&d)[16], uint64_t desc
         : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
         : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
+// s32 += s8 . s8, K-major, 64 x 32 x 32
+__device__ __forceinline__ void mma_s8s8_m64n32(uint32_t (&d)[16], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
 // s32 += s8 . s8, K-major, 64 x 64 x 32
 __device__ __forceinline__ void mma_s8s8_m64n64(uint32_t (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
     asm volatile(

@@ -337,7 +337,7 @@ class KTransformersExperts(BaseInjectedModule, KExpertsBase):
 class KTransformersExpertsV2(KTransformersExperts):
     """experts.py:1273-1350: the balance-serve variant whose forward carries `bsz_tensor` (device-side live batch size) and a
     CUDA-graph slot.  With `prefill_op: None` the generate experts serve both phases (one GPU-resident KExpertsB200: per-pair
-    GEMV kernels for decode batches, the grouped tensor-core path from KTB200_GROUPED_MIN tokens up)."""
+    GEMV kernels for decode batches, the grouped tensor-core path from 48 tokens up, 80 for IQ1_S / IQ2_XXS experts)."""
 
     def forward(self, input_tensor, expert_ids, weights, bsz_tensor=None, cuda_graph_idx=0):
         if self.mode == InferenceState.GENERATE or (self.mode == InferenceState.PREFILL and self.prefill_experts is None):

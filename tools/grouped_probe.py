@@ -1,42 +1,163 @@
-"""Times the grouped (prefill) MoE path at DeepSeek-V3 shapes: tokens/s at qlen in {64, 256, 1024, 4096}, against the per-pair kernels."""
-import ctypes as C, os, sys, time
-import numpy as np, torch
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from ktransformers_b200 import native
-from ktransformers_b200.util.synth import synth_blocks
-Q4_K, Q6_K, BF16 = 12, 14, 30
-lib = native.lib()
-E, k, H, I = int(os.environ.get("E", 256)), 8, 7168, 2048
-gate, up, down = synth_blocks(Q4_K, E * I * H, "cuda", 1), synth_blocks(Q4_K, E * I * H, "cuda", 2), synth_blocks(Q6_K, E * H * I, "cuda", 3)
-cfg = native.MoeConfig(E, k, H, I, 64, 10, 4096, 1, gate.data_ptr(), up.data_ptr(), down.data_ptr(), Q4_K, Q4_K, Q6_K, BF16, 0)
-h = C.c_void_p(); native.check(lib.ktb200_moe_create(C.byref(cfg), 0, C.byref(h)))
-s = torch.cuda.current_stream().cuda_stream
-native.check(lib.ktb200_moe_load_weights(h, s))
-g = torch.Generator(device="cuda").manual_seed(0)
-for qlen in [int(v) for v in os.environ.get("QLENS", "64,256,1024,4096").split(",")]:
-    x = (torch.randn(qlen, H, device="cuda", generator=g) / 100).bfloat16()
-    ids = torch.stack([torch.randperm(E, device="cuda", generator=g)[:k] for _ in range(qlen)]).long()
-    w = torch.rand(qlen, k, device="cuda", generator=g)
-    out = torch.zeros_like(x)
-    def run(): native.check(lib.ktb200_moe_forward(h, qlen, k, ids.data_ptr(), w.data_ptr(), x.data_ptr(), out.data_ptr(), None, s))
-    for _ in range(2): run()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(True), torch.cuda.Event(True)
-    n = 5
-    e0.record()
-    for _ in range(n): run()
-    e1.record(); torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / n
-    flops = 2.0 * qlen * k * 3 * H * I
-    print(f"qlen {qlen}: {ms:.3f} ms  {qlen / ms * 1e3:.0f} tok/s  {flops / ms / 1e9:.1f} TFLOP/s-equivalent  (KTB200_GROUPED_MIN={os.environ.get('KTB200_GROUPED_MIN', '48')})", flush=True)
+"""Times the grouped (prefill) MoE path at DeepSeek-V3 shapes (E 256, H 7168, I 2048, k 8, BF16) against the per-pair kernels,
+for three expert type sets: Q4_K/Q4_K/Q6_K and DeepSeek-R1's IQ1_S x3 and IQ1_S/IQ1_S/IQ2_XXS.
 
-if os.environ.get("TRACE"):
-    tr = torch.zeros(2 * 3 * 96 * 4, dtype=torch.int64, device="cuda")
-    lib.ktb200_debug_grouped(tr.data_ptr()); run(); torch.cuda.synchronize(); lib.ktb200_debug_grouped(None)
-    t = tr.cpu().numpy().reshape(2, 3, 96, 4)
-    for kname, kk in (("gate (Q4_K)", 0), ("down (Q6_K)", 1)):
-        t0 = t[kk, 0, 0, 0]
-        print(f"--- {kname}: cycles since the producer's first stage; P = wait_group done / smem_free seen / arrived, M = before ab_full / ab_full seen / MMAs + scale-and-add done / arrived")
-        for st in range(0, 40):
-            P, M = t[kk, 0, st] - t0, t[kk, 1, st] - t0
-            print(f"st {st:2d}  P {P[0]:6d} {P[1]:6d} {P[2]:6d} {P[3]:6d} | M {M[0]:6d} {M[1]:6d} {M[2]:6d} {M[3]:6d}")
+Every (type set, arm) runs in an interpreter of its own on the same seeded weights and inputs: arm "grouped" as shipped,
+arm "per-pair" with KTB200_GROUPED_MIN above every qlen (the threshold is read once per process), and, when BASELINE_LIB names
+another build of libktb200.so, arm "baseline" = the grouped path of that build.  Arms alternate, REPS times; the table gives
+the fastest repetition, ms per layer, tok/s over 58 MoE layers, and the share of the HBM bound for the bytes the grouped GEMMs
+read (every expert's three matrices once per 32-token tile of its tokens, at 3.35 TB/s).  Outputs are compared at every timed
+size: per-pair against grouped within assert_bf16_close's bound, baseline against grouped bit for bit where both builds run
+the same kernels (else within that bound).
+
+    python tools/grouped_probe.py                       TYPES=q4k,iq1x3,iq1_iq1_iq2  QLENS=48,64,256,1024,4096  REPS=2
+    TRACE=1 python tools/grouped_probe.py               clock64 stamps of the gate and down GEMMs' CTA 0 (grouped arm)
+"""
+import json, os, subprocess, sys, tempfile
+import numpy as np, torch
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+Q4_K, Q6_K, IQ2_XXS, IQ1_S, BF16 = 12, 14, 16, 19, 30
+TYPE_SETS = {"q4k": (Q4_K, Q4_K, Q6_K), "iq1x3": (IQ1_S,) * 3, "iq1_iq1_iq2": (IQ1_S, IQ1_S, IQ2_XXS)}
+NAMES = {Q4_K: "Q4_K", Q6_K: "Q6_K", IQ1_S: "IQ1_S", IQ2_XXS: "IQ2_XXS"}
+BLOCK = {Q4_K: 144, Q6_K: 210, IQ1_S: 50, IQ2_XXS: 66}
+E, k, H, I, LAYERS, HBM = int(os.environ.get("E", 256)), 8, 7168, 2048, 58, 3.35e12
+
+
+def weights(t, n, seed):
+    """seeded raw blocks on the device: synth_blocks for the K-quants; random bytes with d in [0.75, 1.25) / 64 (IQ1_S) or / 512
+    (IQ2_XXS) for the i-quants (every bit pattern is a valid i-quant block)"""
+    if t in (Q4_K, Q6_K):
+        from ktransformers_b200.util.synth import synth_blocks
+        return synth_blocks(t, n, "cuda", seed)
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    b = torch.randint(0, 256, (n // 256, BLOCK[t]), dtype=torch.uint8, device="cuda", generator=g)
+    d = ((torch.rand(n // 256, device="cuda", generator=g) * 0.5 + 0.75) / (64 if t == IQ1_S else 512)).half()
+    b[:, 0:2] = d.view(torch.uint8).view(-1, 2)
+    return b.reshape(-1)
+
+
+def worker(tset, qlens, outdir):
+    import ctypes as C
+    from ktransformers_b200 import native
+    if os.environ.get("PROBE_LIB"):
+        native.LIB_PATH = os.environ["PROBE_LIB"]
+    lib = native.lib()
+    gt, ut, dt = TYPE_SETS[tset]
+    w3 = [weights(t, E * I * H, s) for t, s in ((gt, 1), (ut, 2), (dt, 3))]
+    cfg = native.MoeConfig(E, k, H, I, 64, 10, max(qlens), 1, *(t.data_ptr() for t in w3), gt, ut, dt, BF16, 0)
+    h = C.c_void_p()
+    native.check(lib.ktb200_moe_create(C.byref(cfg), 0, C.byref(h)))
+    s = torch.cuda.current_stream().cuda_stream
+    native.check(lib.ktb200_moe_load_weights(h, s))
+    g = torch.Generator(device="cuda").manual_seed(0)
+    res = {}
+    for qlen in qlens:
+        x = (torch.randn(qlen, H, device="cuda", generator=g) / 100).bfloat16()
+        ids = torch.stack([torch.randperm(E, device="cuda", generator=g)[:k] for _ in range(qlen)]).long()
+        w = torch.rand(qlen, k, device="cuda", generator=g)
+        out = torch.zeros_like(x)
+
+        def run():
+            native.check(lib.ktb200_moe_forward(h, qlen, k, ids.data_ptr(), w.data_ptr(), x.data_ptr(), out.data_ptr(), None, s))
+        for _ in range(2):
+            run()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(True), torch.cuda.Event(True)
+        n = 5
+        e0.record()
+        for _ in range(n):
+            run()
+        e1.record()
+        torch.cuda.synchronize()
+        counts = torch.bincount(ids.reshape(-1), minlength=E)
+        res[qlen] = {"ms": e0.elapsed_time(e1) / n, "tiles": ((counts + 31) // 32).tolist()}
+        np.save(os.path.join(outdir, f"{qlen}.npy"), out.view(torch.int16).cpu().numpy())
+    if os.environ.get("TRACE"):
+        tr = torch.zeros(2 * 3 * 96 * 4, dtype=torch.int64, device="cuda")
+        lib.ktb200_debug_grouped(tr.data_ptr()); run(); torch.cuda.synchronize(); lib.ktb200_debug_grouped(None)
+        t = tr.cpu().numpy().reshape(2, 3, 96, 4)
+        for kname, kk in ((f"gate ({NAMES[gt]}, grouped_gemm_kernel<{(0, 0, 2, 3)[[Q4_K, Q6_K, IQ1_S, IQ2_XXS].index(gt)]}>)", 0),
+                          (f"down ({NAMES[dt]}, grouped_gemm_kernel<{(0, 1, 2, 3)[[Q4_K, Q6_K, IQ1_S, IQ2_XXS].index(dt)]}>)", 1)):
+            t0 = t[kk, 0, 0, 0]
+            print(f"--- {kname}, qlen {qlen}: cycles since the producer's first stage; P = wait_group done / smem_free seen / arrived, "
+                  f"M = before ab_full / ab_full seen / MMAs + scale-and-add done / arrived")
+            for st in range(0, 40):
+                P, M = t[kk, 0, st] - t0, t[kk, 1, st] - t0
+                print(f"st {st:2d}  P {P[0]:6d} {P[1]:6d} {P[2]:6d} {P[3]:6d} | M {M[0]:6d} {M[1]:6d} {M[2]:6d} {M[3]:6d}")
+    lib.ktb200_moe_destroy(h)
+    print("RESULT " + json.dumps(res), flush=True)
+
+
+def bf16_close(got, want):
+    """tests/test_gpu_parity.py assert_bf16_close: within 2^-7 of the larger magnitude + 1e-3 of max |want|, > 97 % bit-identical"""
+    a = (got.astype(np.uint32) << 16).view(np.float32)
+    b = (want.astype(np.uint32) << 16).view(np.float32)
+    ok = np.abs(a - b) <= 2.0 ** -7 * np.maximum(np.abs(a), np.abs(b)) + 1e-3 * np.abs(b).max()
+    return bool(ok.all()) and float((got == want).mean()) > 0.97, float((got == want).mean())
+
+
+def main():
+    tsets = os.environ.get("TYPES", "q4k,iq1x3,iq1_iq1_iq2").split(",")
+    qlens = [int(v) for v in os.environ.get("QLENS", "48,64,256,1024,4096").split(",")]
+    reps = int(os.environ.get("REPS", 2))
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    print(f"card: {torch.cuda.get_device_name(0)}; nvidia-smi name, power limit, max SM clock: {smi.stdout.strip()}", flush=True)
+    arms = {"grouped": {}, "per-pair": {"KTB200_GROUPED_MIN": str(max(qlens) + 1)}}
+    if os.environ.get("BASELINE_LIB"):
+        arms["baseline"] = {"PROBE_LIB": os.environ["BASELINE_LIB"]}
+    tmp = tempfile.mkdtemp(prefix="grouped_probe_")
+    ok = True
+    for tset in tsets:
+        best = {}
+        for rep in range(reps):
+            for arm, env in arms.items():
+                d = os.path.join(tmp, tset, arm)
+                os.makedirs(d, exist_ok=True)
+                env = dict(os.environ, **env)
+                if arm != "grouped" or rep:
+                    env.pop("TRACE", None)
+                r = subprocess.run([sys.executable, os.path.abspath(__file__), "--worker", tset, ",".join(map(str, qlens)), d],
+                                   env=env, capture_output=True, text=True)
+                lines = r.stdout.splitlines()
+                if r.returncode:
+                    print(r.stdout[-2000:], r.stderr[-3000:])
+                    raise SystemExit(f"{tset} {arm}: worker failed")
+                print("\n".join(l for l in lines if not l.startswith("RESULT ")), end="" if len(lines) < 2 else "\n")
+                res = json.loads(next(l for l in lines if l.startswith("RESULT "))[7:])
+                for q, v in res.items():
+                    b = best.setdefault((arm, int(q)), v)
+                    b["ms"] = min(b["ms"], v["ms"])
+                    b.setdefault("all", []).append(v["ms"])
+        gt, ut, dt = TYPE_SETS[tset]
+        eb = [I * H // 256 * BLOCK[t] for t in (gt, ut, dt)]
+        print(f"\n{NAMES[gt]}/{NAMES[ut]}/{NAMES[dt]}  (E {E}, H {H}, I {I}, k {k}, BF16; ms per layer = fastest of {reps}, all reps in brackets)")
+        print(f"{'qlen':>6} | {'grouped ms':>22} {'tok/s/58L':>9} {'HBM share':>9} | {'per-pair ms':>22} {'tok/s/58L':>9} | {'speed-up':>8} | outputs")
+        for q in qlens:
+            gr, pp = best[("grouped", q)], best[("per-pair", q)]
+            tile_bytes = sum(gr["tiles"]) * sum(eb)
+            a, b = (np.load(os.path.join(tmp, tset, arm, f"{q}.npy")).view(np.uint16) for arm in ("grouped", "per-pair"))
+            close, exact = bf16_close(b, a)
+            cmp = f"per-pair {'within' if close else 'OUTSIDE'} bf16 bound ({exact:.2%} bit-identical)"
+            ok &= close
+            if "baseline" in arms:
+                # bit-identical where both builds take the same kernels; otherwise (a route the baseline build lacks) the
+                # per-pair bound
+                bl = best[("baseline", q)]
+                c = np.load(os.path.join(tmp, tset, "baseline", f"{q}.npy")).view(np.uint16)
+                same = np.array_equal(c, a)
+                close = same or bf16_close(c, a)[0]
+                ok &= close
+                verdict = "bit-identical" if same else "within bf16 bound" if close else "OUTSIDE bf16 bound"
+                cmp += f"; baseline {verdict}, {bl['ms']:.3f} ms [{' '.join(f'{v:.3f}' for v in bl['all'])}]"
+            fmt = lambda v: f"{v['ms']:8.3f} [{' '.join(f'{x:.2f}' for x in v['all'])}]"
+            print(f"{q:6d} | {fmt(gr):>22} {q / (LAYERS * gr['ms']) * 1e3:9.0f} {tile_bytes / HBM * 1e3 / gr['ms']:9.1%} | {fmt(pp):>22} "
+                  f"{q / (LAYERS * pp['ms']) * 1e3:9.0f} | {pp['ms'] / gr['ms']:7.2f}x | {cmp}", flush=True)
+    print("all outputs agree" if ok else "OUTPUT MISMATCH")
+    sys.exit(0 if ok else 1)
+
+
+if __name__ == "__main__":
+    if len(sys.argv) > 1 and sys.argv[1] == "--worker":
+        worker(sys.argv[2], [int(v) for v in sys.argv[3].split(",")], sys.argv[4])
+    else:
+        main()
