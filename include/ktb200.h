@@ -362,7 +362,7 @@ int ktb200_moe_ep_forward_tokens(const ktb200_gate_config* gate, ktb200_moe* moe
  *   out [B][Hq][512] bf16 ; lse_out optional fp32 [B][Hq] (natural log)
  * ------------------------------------------------------------------------------------------ */
 typedef struct ktb200_mla_params {
-    int batch, num_heads, page_size, max_pages_per_seq, num_kv_splits; /* splits <=0: auto */
+    int batch, num_heads, page_size, max_pages_per_seq, num_kv_splits; /* splits <=0: auto; > 128: KTB200_EINVAL */
     float sm_scale;
     const void* q_nope; const void* q_pe; const void* kv_cache;
     const int* page_table; const int* kv_len;

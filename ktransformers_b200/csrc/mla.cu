@@ -35,6 +35,7 @@ constexpr int kDV = 512;
 constexpr int kHG = 64;              // heads per CTA (wgmma M)
 constexpr int kLT = 32;              // kv tokens per tile (N of S, K of P.V)
 constexpr int kStages = 4;
+constexpr int kMaxSplits = 128;      // mla_merge_kernel: one thread (and one ws[] slot) per split
 constexpr int kChunks = kDK / 64;    // 9 column chunks of 64 bf16 = 128 B (one swizzle row)
 constexpr int kMlaConsumerWarps = 8, kMlaThreads = kMlaConsumerWarps * 32 + 128;
 constexpr int kStageBytes = kLT * kDK * 2;         // 36,864 = 9 regions of 32 rows x 128 B
@@ -256,15 +257,17 @@ __global__ void __launch_bounds__(kMlaThreads, 1) mla_decode_tc_kernel(const __g
 }
 
 // out[b][h][:] = sum_s w_s * o_part[b][s][h][:],  w_s = 2^(lse_s - max) / sum ; lse (natural log) optional
+// 128 threads (4 warps), one per split: ktb200_mla_decode refuses num_kv_splits > kMaxSplits
+static_assert(kMaxSplits == 128, "mla_merge_kernel reduces over exactly 4 warps");
 __global__ void __launch_bounds__(128) mla_merge_kernel(const float* o_part, const float* lse_part, int num_splits, int num_heads,
                                                         __nv_bfloat16* out, float* lse_out) {
-    __shared__ float ws[128];
+    __shared__ float ws[kMaxSplits];
     __shared__ float red[8];
     griddep_launch_dependents();
     griddep_wait();
     const int bh = blockIdx.x, b = bh / num_heads, h = bh % num_heads;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const float my = tid < num_splits ? lse_part[((long)b * num_splits + tid) * num_heads + h] : -INFINITY;   // num_splits <= 128
+    const float my = tid < num_splits ? lse_part[((long)b * num_splits + tid) * num_heads + h] : -INFINITY;   // num_splits <= kMaxSplits
     float mx = my;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
@@ -320,7 +323,7 @@ static int pick_splits(int batch, int num_heads, int max_kv_tiles, int device) {
     int s = (num_sms(device) + groups - 1) / groups;          // one CTA per SM (227 KB of shared memory each)
     const int cap = (max_kv_tiles + 3) / 4;                   // at least 4 tiles (128 tokens) per split
     if (s > cap) s = cap;
-    if (s > 128) s = 128;
+    if (s > kMaxSplits) s = kMaxSplits;
     if (s < 1) s = 1;
     return s;
 }
@@ -346,7 +349,7 @@ static float* g_mla_debug = nullptr;
 extern "C" {
 
 size_t ktb200_mla_workspace_bytes(int batch, int num_heads, int max_splits) {
-    if (max_splits <= 0) max_splits = 128;
+    if (max_splits <= 0) max_splits = ktb::kMaxSplits;
     return (size_t)batch * max_splits * num_heads * (ktb::kDV + 1) * sizeof(float);
 }
 
@@ -359,6 +362,10 @@ int ktb200_mla_decode(const ktb200_mla_params* q, void* stream) {
         return KTB200_EINVAL;
     }
     if (((uintptr_t)q->kv_cache & 15) || ((uintptr_t)q->q_nope & 15) || ((uintptr_t)q->q_pe & 15)) { set_error("mla_decode: q / kv_cache must be 16-byte aligned"); return KTB200_EINVAL; }
+    if (q->num_kv_splits > kMaxSplits) {   // the merge kernel weighs at most kMaxSplits partials
+        set_error("mla_decode: num_kv_splits %d exceeds the maximum of %d", q->num_kv_splits, kMaxSplits);
+        return KTB200_EINVAL;
+    }
     int dev = 0;
     KTB_CUDA_CHECK(cudaGetDevice(&dev));
     const int max_tiles = q->max_pages_per_seq * (q->page_size / kLT);

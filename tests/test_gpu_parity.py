@@ -564,6 +564,7 @@ def _mla_case(rng, B, Hq, page_size, lens, shuffle_pages=True):
 @pytest.mark.parametrize("B,Hq,page_size,lens,splits", [
     (1, 128, 64, [1], 0), (1, 128, 64, [33], 0), (1, 128, 64, [1000], 0), (1, 128, 64, [4096], 0),
     (3, 128, 64, [17, 640, 2049], 0), (2, 16, 32, [95, 128], 0), (1, 128, 256, [777], 3), (2, 40, 64, [64, 65], 1),
+    (2, 128, 64, [3001, 4500], 5),      # 29 tiles per CTA: the 4-stage ring wraps 7 times (longer lengths: test_mla_lengths.py)
 ])
 def test_mla_decode_vs_oracle(B, Hq, page_size, lens, splits):
     from oracle import mla_oracle

@@ -280,6 +280,20 @@ def test_ep_comm_argument_checks_need_no_gpu():
         native.check(lib.ktb200_ep_all_gather_tokens(C.byref(ok), None, None, None))       # null token
 
 
+@pytest.mark.parametrize("splits", [129, 200, 2 ** 31 - 1])
+def test_mla_decode_refuses_more_than_128_kv_splits(splits):
+    """the split-KV merge weighs at most 128 partials: ktb200_mla_decode refuses more before any device work (the pointers
+    are aligned stand-ins that are never dereferenced; 128 itself runs on the GPU in tests/test_mla_lengths.py)"""
+    import ctypes as C
+    from ktransformers_b200 import native
+    lib = native.lib()
+    base = 1 << 24
+    p = native.MlaParams(1, 128, 64, 128, splits, 0.07, base, base + (1 << 20), base + (2 << 20), base + (3 << 20), base + (4 << 20),
+                         base + (5 << 20), None, base + (6 << 20), 1 << 30, 128 * 64)
+    assert lib.ktb200_mla_decode(C.byref(p), None) == native.EINVAL
+    assert f"num_kv_splits {splits} exceeds the maximum of 128" in lib.ktb200_last_error().decode()
+
+
 def test_pybind_module_exposes_the_reference_extension_surface():
     """kt_kernel_ext_b200 (csrc/ext_bindings.cpp) — the compiled pybind boundary: names and call shapes of
     kt-kernel/ext_bindings.cpp (MOEConfig :746-831, bind_moe_module :447-471, CPUInfer :554-565)."""

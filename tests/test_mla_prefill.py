@@ -177,7 +177,7 @@ class _Case:
         return out
 
 
-GRID = [(0, 2), (0, 64), (0, 129), (0, 1024), (63, 1), (300, 200), (1000, 37)]
+GRID = [(0, 2), (0, 64), (0, 129), (0, 1024), (63, 1), (300, 200), (1000, 37), (2100, 300)]   # longer: test_mla_lengths.py
 
 
 @pytest.mark.gpu
