@@ -52,7 +52,9 @@ enum ktb200_ggml_type {
      *   bytes 0..15          eight bf16 group scales
      *   bytes 16+16j..31+16j group j = four 32-bit words, word w holds columns 8w..8w+7 of the group, column 8w+i in
      *                        bits 4i..4i+3 as u = q + 8 (the compressed-tensors words unchanged)
-     * value = (u - 8) * scale.  Routed experts only (ktb200_moe_*): linears and MLP handles reject it. */
+     * value = (u - 8) * scale.  Routed experts only (ktb200_moe_*): linears and MLP handles reject it.  ktb200_moe_forward
+     * runs them per (token, expert) pair below 96 tokens and on the grouped tensor-core GEMM from 96 (bf16 planes of the
+     * activations against u - 8, DESIGN.md §4.5). */
     KTB200_TYPE_RAWINT4_G32 = 256
 };
 
@@ -116,7 +118,10 @@ int ktb200_moe_warm_up(ktb200_moe* moe, void* stream);
  * Arithmetic: identical to the reference CPU path — activations quantised to the weight type's
  * vec_dot_type (Q8_K / Q8_0) with the reference's rounding, integer dot products, fp32 scales,
  * fp32 accumulation over experts in expert_ids order, output rounded like ggml from_float.
- * RAWINT4_G32 experts are W4A16 instead: fp32 activations against (u - 8) * scale, fp32 sums (DESIGN.md §2). */
+ * RAWINT4_G32 experts are W4A16 instead: fp32 activations against (u - 8) * scale, fp32 sums (DESIGN.md §2).
+ * Routes: per-pair GEMV kernels for short batches; from 48 tokens (80 for a handle with an i-quant tensor, 96 for RAWINT4;
+ * KTB200_GROUPED_MIN overrides) the grouped tensor-core GEMMs, which read each expert once per 32-token tile and grow a
+ * per-device scratch arena on first use. */
 int ktb200_moe_forward(ktb200_moe* moe, int qlen, int k, const int64_t* expert_ids_dev,
                        const float* weights_dev, const void* input_dev, void* output_dev,
                        const int* bsz_tensor_dev, void* stream);

@@ -20,7 +20,7 @@
 //                    needed (16-byte peer stores, one CTA per token); the last CTA to finish bumps epoch_send and releases
 //                    send[rank] on every rank.
 //   2 experts + deliver   ep_tok_wait_kernel waits for the world send flags; the shard's ordinary expert kernels run on
-//                    the gathered rows in place with fp32 output (per-pair kernels below 48 rows / 80 for IQ, grouped GEMM above, in
+//                    the gathered rows in place with fp32 output (per-pair kernels below 48 rows / 80 for IQ / 96 for RAWINT4, grouped GEMM above, in
 //                    chunks of min(group_max_len, scratch rows)); ep_tok_deliver_kernel stores each needed row into its
 //                    owner's part slot; after the last chunk its last CTA bumps epoch_deliver and releases deliver[rank]
 //                    on every rank (also when nothing was delivered to that rank).

@@ -507,6 +507,214 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// RAWINT4_G32 (Kimi-K2's compressed-tensors experts) on the bf16 tensor path: W4A16, nothing quantised (DESIGN.md §2).
+// A = u - 8 (-8..7, exact in bf16); B = the activations split into NP exact bf16 planes x = hi + mid + lo (grp_split_*):
+// every product (u - 8) * plane is exact in fp32 (4 x 8 significant bits), and all 2 NP MMAs of a 32-value group sum into one
+// group accumulator, so the tensor core sums exact products in fp32 — the per-pair kernels' group sum in another order.  Then
+// one FFMA per group, acc = fma(gsum, s, acc) with the row's bf16 scale, as i4_block_dot.  NP = 1 for BF16 gate/up (hi = x),
+// NP = 3 for F16 / F32 gate/up and for the down projection (a = act(g) * u in fp32).  The planes are a function of the fp32
+// value only, so a narrow input and the same value widened to F32 give bit-identical sums: the extra planes add exact zeros.
+// grouped_i4_kernel: the tile table, persistent tile loop, roles, rings and stores of grouped_gemm_kernel; stage = 64 of K =
+// two groups.  Producer thread (row, part) converts group `part` of its row: (w >> 4j) & 0x000F000F | 0x43004300 is the bf16
+// pair (128 + u of column 8i + j, 128 + u of column 8i + j + 4) of word i, minus 136 that is u - 8; so within every 8 columns
+// K position 2j holds column j and 2j + 1 column j + 4, and the split kernels write B in that order (i4_split8).
+// Shared-memory plan (I4Plan): A stages as kGA, NP B planes of 32 token rows per stage, raw slots of 2 + NP 16-byte units per
+// thread (0 the group's four words, 1 the stage's scale word, 2.. the activation pieces), the misc block with hdr[.][row].x =
+// the scale word (low half group 2q, high half group 2q + 1 of the block's quarter q).
+template <int NP>
+struct I4Plan {
+    static constexpr int kB = NP * kGN * 128, kPitch = 16 * (2 + NP), kSlot = 2 * kGM * kPitch;
+    static constexpr int kOffB = kGStages * kGA, kOffRaw = kOffB + kGStages * kB, kOffMisc = kOffRaw + kGRaw * kSlot;
+    static constexpr int kSmem = kOffMisc + (int)sizeof(GrpMisc) + 1024;
+};
+static_assert(I4Plan<1>::kSmem <= 227 * 1024 && I4Plan<3>::kSmem <= 227 * 1024 && I4Plan<1>::kOffB % 1024 == 0 && kGN * 128 % 1024 == 0,
+              "RAWINT4 shared-memory plan");
+
+struct GrpI4Params {
+    const uint8_t* w;          // expert weights, RAWINT4_G32 blocks
+    long expert_bytes;
+    int R, Kc;
+    const uint16_t* x;         // bf16 planes [rows][NP][Kc] in the K order of the A tile (i4_split8)
+    const int* rowmap;         // sorted position -> activation row (null: identity)
+    const int4* tinfo;
+    const int* nt_prefix;
+    int E;
+    float* out;                // [P][R] fp32
+    long long* trace;          // as GrpGemmParams::trace
+};
+
+// the bf16 pair (u - 8 of column j, u - 8 of column j + 4) of the 8 columns in word w
+__device__ __forceinline__ uint32_t i4_bf16x2(uint32_t w, int j) {
+    const uint32_t v = ((w >> (4 * j)) & 0x000F000Fu) | 0x43004300u;
+    uint32_t r;
+    asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(r) : "r"(v), "r"(0x43084308u));   // (128 + u) - 136, exact
+    return r;
+}
+// 8 consecutive values -> NP bf16 planes (hi = bf16_rn(x), mid = bf16_rn(x - hi), lo = bf16_rn(x - hi - mid); every difference
+// is exact) in the K order of i4_bf16x2; plane p at dst + p * Kc
+template <int NP>
+__device__ __forceinline__ void i4_split8(const float (&x)[8], uint16_t* dst, int Kc) {
+    uint32_t v[NP][4];
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+        float r0 = x[j], r1 = x[j + 4];
+#pragma unroll
+        for (int p = 0; p < NP; p++) {
+            const __nv_bfloat16 b0 = __float2bfloat16_rn(r0), b1 = __float2bfloat16_rn(r1);
+            v[p][j] = (uint32_t)__bfloat16_as_ushort(b0) | ((uint32_t)__bfloat16_as_ushort(b1) << 16);
+            r0 -= __bfloat162float(b0);
+            r1 -= __bfloat162float(b1);
+        }
+    }
+#pragma unroll
+    for (int p = 0; p < NP; p++) *reinterpret_cast<uint4*>(dst + (long)p * Kc) = make_uint4(v[p][0], v[p][1], v[p][2], v[p][3]);
+}
+
+template <int NP>
+__global__ void __launch_bounds__(kGThreads, 1) grouped_i4_kernel(const GrpI4Params p) {
+    using L = I4Plan<NP>;
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t raw = smem_u32(smem_raw);
+    const uint32_t base = (raw + 1023u) & ~1023u;
+    uint8_t* smem = smem_raw + (base - raw);
+    GrpMisc& misc = *reinterpret_cast<GrpMisc*>(smem + L::kOffMisc);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int nst = p.Kc / 64, MT = p.R / kGM;
+    if (tid == 0) {
+        for (int s = 0; s < kGStages; s++) { bar_init(smem_u32(&misc.ab_full[s]), kGProdWarps); bar_init(smem_u32(&misc.smem_free[s]), kGMmaWarps); }
+        for (int s = 0; s < kGHdr; s++) bar_init(smem_u32(&misc.hdr_free[s]), kGMmaWarps);
+        bar_fence_init();
+    }
+    __syncthreads();
+    const int total_tiles = p.nt_prefix[p.E] * MT;
+    int stage = 0, sphase = 0, hs = 0, hphase = 0;
+
+    if (warp < kGProdWarps) {
+        // ========================================================================== producers: thread = (weight row r, group `part`)
+        regs_dec<96>();
+        const int pt = tid, r = pt & (kGM - 1), part = pt >> 7, sw = r & 7, bn = pt >> 3, pc = pt & 7;
+        const uint32_t raw_dst = base + L::kOffRaw + pt * L::kPitch;
+        const uint8_t* raw_src = smem + L::kOffRaw + pt * L::kPitch;
+        int ftile = blockIdx.x, fst = 0;
+        const uint8_t* fw = nullptr;    // block 0 of this thread's weight row
+        const uint16_t* fx = nullptr;   // this thread's activation piece of stage 0, plane 0 (null: no token row)
+        auto enter_tile = [&]() {
+            if (ftile >= total_tiles) return;
+            const int4 ti = __ldg(p.tinfo + ftile);
+            fx = bn < ti.w ? p.x + (long)(p.rowmap ? __ldg(p.rowmap + ti.z + bn) : ti.z + bn) * NP * p.Kc + pc * 8 : nullptr;
+            fw = p.w + (long)ti.x * p.expert_bytes + (long)(ti.y + r) * (p.Kc / QK_K) * SZ_RAWINT4;
+        };
+        auto issue = [&](uint32_t dst) {
+            if (ftile < total_tiles) {
+                const uint8_t* blk = fw + (fst >> 2) * SZ_RAWINT4;
+                const int q = fst & 3;
+                cp_async16(dst, blk + 16 + 16 * (2 * q + part));
+                if (part == 0) cp_async4(dst + 16, blk + 4 * q);
+                if (fx) {
+#pragma unroll
+                    for (int pl = 0; pl < NP; pl++) cp_async16(dst + 32 + 16 * pl, fx + (long)pl * p.Kc + fst * 64);
+                }
+                if (++fst == nst) { fst = 0; ftile += gridDim.x; enter_tile(); }
+            }
+            cp_async_commit();
+        };
+        enter_tile();
+        for (int i = 0; i < kGRaw; i++) issue(raw_dst + i * L::kSlot);
+        int slot = 0;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            const int n_valid = __ldg(p.tinfo + tile).w;
+            for (int st = 0; st < nst; st++) {
+                const bool tr = p.trace && blockIdx.x == 0 && tid == 0 && tile == 0 && st < 96;
+                if (tr) p.trace[(0 * 96 + st) * 4 + 0] = clock64();
+                cp_async_wait<kGRaw - 1>();
+                if (tr) p.trace[(0 * 96 + st) * 4 + 1] = clock64();
+                const uint4* rs = reinterpret_cast<const uint4*>(raw_src + slot * L::kSlot);
+                const uint4 f0 = rs[0];
+                const uint32_t scw = rs[1].x;
+                uint4 fb[NP];
+#pragma unroll
+                for (int pl = 0; pl < NP; pl++) fb[pl] = rs[2 + pl];
+                issue(raw_dst + slot * L::kSlot);   // refill the slot just read (thread-private bytes)
+                slot = slot == kGRaw - 1 ? 0 : slot + 1;
+                bar_wait(smem_u32(&misc.smem_free[stage]), sphase ^ 1);
+                bar_wait(smem_u32(&misc.hdr_free[hs]), hphase ^ 1);
+                if (tr) p.trace[(0 * 96 + st) * 4 + 2] = clock64();
+                uint8_t* arow = smem + stage * kGA + r * 128;
+                const uint32_t wd[4] = {f0.x, f0.y, f0.z, f0.w};
+#pragma unroll
+                for (int i = 0; i < 4; i++)   // word i of group `part` -> 16-byte chunk 4 part + i of the row
+                    *reinterpret_cast<uint4*>(arow + (((4 * part + i) ^ sw) << 4)) =
+                        make_uint4(i4_bf16x2(wd[i], 0), i4_bf16x2(wd[i], 1), i4_bf16x2(wd[i], 2), i4_bf16x2(wd[i], 3));
+                if (part == 0) misc.hdr[hs][r].x = scw;
+                uint8_t* Bs = smem + L::kOffB + stage * L::kB + bn * 128 + ((pc ^ (bn & 7)) << 4);
+                const uint4 z = make_uint4(0, 0, 0, 0);
+#pragma unroll
+                for (int pl = 0; pl < NP; pl++) *reinterpret_cast<uint4*>(Bs + pl * (kGN * 128)) = bn < n_valid ? fb[pl] : z;
+                fence_async_smem();
+                __syncwarp();
+                if (lane == 0) bar_arrive(smem_u32(&misc.ab_full[stage]));
+                if (tr) p.trace[(0 * 96 + st) * 4 + 3] = clock64();
+                if (++stage == kGStages) { stage = 0; sphase ^= 1; }
+                if (++hs == kGHdr) { hs = 0; hphase ^= 1; }
+            }
+        }
+        cp_async_wait<0>();
+    } else {
+        // ========================================================================== MMA warpgroups: g owns weight rows 64 g .. 64 g + 63
+        // register i of an accumulator: row ra + 8 ((i >> 1) & 1), token column 8 (i >> 2) + cq + (i & 1)
+        regs_inc<160>();
+        const int mw = warp - kGProdWarps, g = mw >> 2, ra = 64 * g + 16 * (mw & 3) + (lane >> 2), cq = 2 * (lane & 3);
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            const int4 ti = __ldg(p.tinfo + tile);
+            float acc[16];
+#pragma unroll
+            for (int i = 0; i < 16; i++) acc[i] = 0.f;
+            for (int st = 0; st < nst; st++) {
+                const bool tr = p.trace && blockIdx.x == 0 && mw == 0 && lane == 0 && tile == 0 && st < 96;
+                if (tr) p.trace[(1 * 96 + st) * 4 + 0] = clock64();
+                bar_wait(smem_u32(&misc.ab_full[stage]), sphase);
+                if (tr) p.trace[(1 * 96 + st) * 4 + 1] = clock64();
+                const uint32_t a = base + stage * kGA + g * (kGA / 2), b = base + L::kOffB + stage * L::kB;
+                // group accumulators of the stage's two groups: every plane's two K = 16 MMAs into the same one
+                float g0[16], g1[16];
+#pragma unroll
+                for (int i = 0; i < 16; i++) { g0[i] = 0.f; g1[i] = 0.f; }
+                fence();
+#pragma unroll
+                for (int pl = 0; pl < NP; pl++)
+#pragma unroll
+                    for (int ks = 0; ks < 2; ks++) {
+                        mma_bf16_m64n32(g0, smem_desc(a + 32 * ks, 16, 1024, kLayoutSw128), smem_desc(b + pl * (kGN * 128) + 32 * ks, 16, 1024, kLayoutSw128), 1);
+                        mma_bf16_m64n32(g1, smem_desc(a + 64 + 32 * ks, 16, 1024, kLayoutSw128), smem_desc(b + pl * (kGN * 128) + 64 + 32 * ks, 16, 1024, kLayoutSw128), 1);
+                    }
+                commit();
+                wait<0>();
+                fence_regs(g0);
+                fence_regs(g1);
+                const uint32_t s0 = misc.hdr[hs][ra].x, s1 = misc.hdr[hs][ra + 8].x;
+#pragma unroll
+                for (int i = 0; i < 16; i++) {
+                    const uint32_t sc = (i & 2) ? s1 : s0;
+                    acc[i] = __fmaf_rn(g0[i], __uint_as_float(sc << 16), acc[i]);
+                    acc[i] = __fmaf_rn(g1[i], __uint_as_float(sc & 0xffff0000u), acc[i]);
+                }
+                if (tr) p.trace[(1 * 96 + st) * 4 + 2] = clock64();
+                __syncwarp();
+                if (lane == 0) { bar_arrive(smem_u32(&misc.smem_free[stage])); bar_arrive(smem_u32(&misc.hdr_free[hs])); }
+                if (tr) p.trace[(1 * 96 + st) * 4 + 3] = clock64();
+                if (++stage == kGStages) { stage = 0; sphase ^= 1; }
+                if (++hs == kGHdr) { hs = 0; hphase ^= 1; }
+            }
+#pragma unroll
+            for (int i = 0; i < 16; i++) {
+                const int n = 8 * (i >> 2) + cq + (i & 1);
+                if (n < ti.w) p.out[(long)(ti.z + n) * p.R + ti.y + ra + 8 * ((i >> 1) & 1)] = acc[i];
+            }
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // bookkeeping kernels (moe.cpp:250-290: m_local_num_, m_local_pos_, prefix offsets)
 __global__ void grp_count_kernel(const int64_t* ids, int npairs, int k, int id_offset, int n_local, const int* bsz, int t0, int* counts) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -558,6 +766,29 @@ __global__ void __launch_bounds__(256) grp_act_quant_kernel(const float* g, cons
     for (int i = 0; i < 8; i++) x[i] = (use_silu ? act_silu(gv[i]) : act_relu(gv[i])) * uv[i];
     warp_quantize_q8k_block(x, lane, reinterpret_cast<uint32_t*>(q + (long)r * ncols + (long)b * QK_K), d + (long)r * nblk + b, bs + (long)r * (ncols / 16) + b * 16);
 }
+// RAWINT4 counterparts of the two kernels above: rows of `src` (hidden type) -> NP bf16 planes [nrows][NP][ncols], and
+// a = act(g) * u (fp32, sorted pair rows, the per-pair kernels' formula) -> 3 planes; one thread per 8 values
+template <int NP>
+__global__ void __launch_bounds__(256) grp_split_x_kernel(const void* src, int hidden_type, int nrows, int ncols, uint16_t* out) {
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x, n8 = ncols / 8;
+    if (i >= (long)nrows * n8) return;
+    const long r = i / n8, c = (i - r * n8) * 8;
+    float x[8];
+    load_block8(src, r * ncols + c, hidden_type, x);
+    i4_split8<NP>(x, out + r * NP * ncols + c, ncols);
+}
+__global__ void __launch_bounds__(256) grp_split_act_kernel(const float* g, const float* u, const int* offsets, int E, int ncols, int use_silu, uint16_t* out) {
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x, n8 = ncols / 8;
+    if (i >= (long)offsets[E] * n8) return;
+    const long r = i / n8, c = (i - r * n8) * 8, o = r * ncols + c;
+    const float4 g0 = *reinterpret_cast<const float4*>(g + o), g1 = *reinterpret_cast<const float4*>(g + o + 4);
+    const float4 u0 = *reinterpret_cast<const float4*>(u + o), u1 = *reinterpret_cast<const float4*>(u + o + 4);
+    const float gv[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w}, uv[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
+    float x[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) x[j] = (use_silu ? act_silu(gv[j]) : act_relu(gv[j])) * uv[j];
+    i4_split8<3>(x, out + r * 3 * ncols + c, ncols);
+}
 // out[t] = sum_j w[t][j] * down[pos[t][j]] in expert_ids order, one FMA per expert (moe.cpp:340-358), rounded like from_float
 __global__ void __launch_bounds__(256) grp_combine_kernel(const float* dd, const int* pos, const float* weights, int T, int k, int H, const int* bsz, int t0, void* out,
                                                           int hidden_type) {
@@ -581,22 +812,32 @@ struct GrpScratch {
     int8_t *xq = nullptr, *aq = nullptr;
     float *xd = nullptr, *ad = nullptr, *g = nullptr, *u = nullptr, *dd = nullptr;
     int16_t *xbs = nullptr, *abs16 = nullptr;
+    size_t cap_xp = 0, cap_ap = 0;           // RAWINT4 bf16 planes (elements): tokens * 3 H, pairs * 3 I
+    uint16_t *xp = nullptr, *ap = nullptr;
 };
 static long long* g_grp_trace = nullptr;
 void grouped_set_trace(long long* t) { g_grp_trace = t; }
 static GrpScratch g_grp[64];   // one arena per device, shared by every handle (calls on one device are stream-ordered by the caller)
 
-static int grp_ensure(int dev, int tokens, int k, int E, int H, int I) {
+// planes: the handle is RAWINT4 and needs the bf16 plane buffers (other handles leave them as they are)
+static int grp_ensure(int dev, int tokens, int k, int E, int H, int I, bool planes) {
     GrpScratch& s = g_grp[dev & 63];
     size_t P = (size_t)tokens * k, nx = (size_t)tokens * H, na = P * I, nd = P * H;
     size_t tg = (P / kGN + E) * (size_t)(I / kGM), td = (P / kGN + E) * (size_t)(H / kGM);   // upper bounds of the tile counts
-    if (s.cap_pairs >= P && s.cap_x >= nx && s.cap_a >= na && s.cap_d >= nd && s.cap_tiles_gu >= tg && s.cap_tiles_d >= td) return KTB200_OK;
+    size_t nxp = planes ? 3 * nx : 0, nap = planes ? 3 * na : 0;
+    if (s.cap_pairs >= P && s.cap_x >= nx && s.cap_a >= na && s.cap_d >= nd && s.cap_tiles_gu >= tg && s.cap_tiles_d >= td && s.cap_xp >= nxp &&
+        s.cap_ap >= nap)
+        return KTB200_OK;
     tg = tg > s.cap_tiles_gu ? tg : s.cap_tiles_gu; td = td > s.cap_tiles_d ? td : s.cap_tiles_d;
     P = P > s.cap_pairs ? P : s.cap_pairs; nx = nx > s.cap_x ? nx : s.cap_x; na = na > s.cap_a ? na : s.cap_a; nd = nd > s.cap_d ? nd : s.cap_d;   // grow only
+    nxp = nxp > s.cap_xp ? nxp : s.cap_xp; nap = nap > s.cap_ap ? nap : s.cap_ap;
     KTB_CUDA_CHECK(cudaDeviceSynchronize());   // earlier calls may still be using the arena
     cudaFree(s.counts); cudaFree(s.tokmap); cudaFree(s.pos); cudaFree(s.xq); cudaFree(s.xd); cudaFree(s.xbs); cudaFree(s.aq); cudaFree(s.ad); cudaFree(s.abs16);
-    cudaFree(s.g); cudaFree(s.u); cudaFree(s.dd); cudaFree(s.tinfo_gu); cudaFree(s.tinfo_d);
+    cudaFree(s.g); cudaFree(s.u); cudaFree(s.dd); cudaFree(s.tinfo_gu); cudaFree(s.tinfo_d); cudaFree(s.xp); cudaFree(s.ap);
     s = GrpScratch();
+    if (nxp) KTB_CUDA_CHECK(cudaMalloc(&s.xp, nxp * sizeof(uint16_t)));
+    if (nap) KTB_CUDA_CHECK(cudaMalloc(&s.ap, nap * sizeof(uint16_t)));
+    s.cap_xp = nxp; s.cap_ap = nap;
     const size_t cp = P;
     KTB_CUDA_CHECK(cudaMalloc(&s.counts, (size_t)(4 * 1024 + 8) * sizeof(int)));
     s.offsets = s.counts + 1024; s.nt_prefix = s.counts + 2048 + 1; s.cursor = s.counts + 3072 + 2;
@@ -624,7 +865,12 @@ static int grouped_fmt(int type, int layout) {
     if (type == KTB200_TYPE_Q6_K && layout == LAYOUT_T4) return 1;
     if (type == KTB200_TYPE_IQ1_S) return 2;
     if (type == KTB200_TYPE_IQ2_XXS) return 3;
+    if (type == KTB200_TYPE_RAWINT4_G32) return 4;   // grouped_i4_kernel (NP picked per launch), never mixed with the others
     return -1;
+}
+static void grouped_i4(int np, const GrpI4Params& p, int grid, cudaStream_t s) {
+    if (np == 1) grouped_i4_kernel<1><<<grid, kGThreads, I4Plan<1>::kSmem, s>>>(p);
+    else grouped_i4_kernel<3><<<grid, kGThreads, I4Plan<3>::kSmem, s>>>(p);
 }
 static void grouped_gemm(int fmt, const GrpGemmParams& p, int grid, cudaStream_t s) {
     switch (fmt) {
@@ -636,11 +882,11 @@ static void grouped_gemm(int fmt, const GrpGemmParams& p, int grid, cudaStream_t
 }
 
 // true when ktb200_moe_forward may take the grouped tensor-core path for this handle: gate and up Q4_K, IQ1_S or IQ2_XXS (each
-// on its own), down any of those or Q6_K in the tile layout
+// on its own), down any of those or Q6_K in the tile layout; or all three RAWINT4_G32
 bool grouped_ok(const ktb200_moe* m, int k) {
     const ktb200_moe_config& c = m->cfg;
     const int fg = grouped_fmt(c.gate_type, LAYOUT_RAW), fu = grouped_fmt(c.up_type, LAYOUT_RAW), fd = grouped_fmt(c.down_type, m->down_layout);
-    return fg >= 0 && fg != 1 && fu >= 0 && fu != 1 && fd >= 0 && c.hidden_size % 256 == 0 &&
+    return fg >= 0 && fg != 1 && fu >= 0 && fu != 1 && fd >= 0 && (fg == 4) == (fu == 4) && (fu == 4) == (fd == 4) && c.hidden_size % 256 == 0 &&
            c.intermediate_size % 256 == 0 && c.hidden_size % kGM == 0 && c.intermediate_size % kGM == 0 && c.expert_num <= 1023 && k <= 32;
 }
 
@@ -650,7 +896,10 @@ int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, cons
     const int E = c.expert_num, H = c.hidden_size, I = c.intermediate_size, dev = m->device;
     static const int chunk_cap = [] { const char* e = getenv("KTB200_GROUPED_CHUNK"); return e ? atoi(e) : 1024; }();
     const int Tc = qlen < chunk_cap ? qlen : chunk_cap;
-    int rc = grp_ensure(dev, Tc, k, E, H, I);   // grow-only scratch: not capturable on first use (like ktb200_moe_gate_forward)
+    const int fg = grouped_fmt(c.gate_type, LAYOUT_RAW), fu = grouped_fmt(c.up_type, LAYOUT_RAW), fd = grouped_fmt(c.down_type, m->down_layout);
+    const bool i4 = fg == 4;
+    const int np = c.hidden_type == KTB200_TYPE_BF16 ? 1 : 3;   // RAWINT4 gate/up planes: one holds bf16, three any fp32
+    int rc = grp_ensure(dev, Tc, k, E, H, I, i4);   // grow-only scratch: not capturable on first use (like ktb200_moe_gate_forward)
     if (rc) return rc;
     GrpScratch& g = g_grp[dev & 63];
     static bool attr[64] = {};
@@ -659,9 +908,10 @@ int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, cons
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmemI));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmemI));
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_i4_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, I4Plan<1>::kSmem));
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_i4_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, I4Plan<3>::kSmem));
         attr[dev & 63] = true;
     }
-    const int fg = grouped_fmt(c.gate_type, LAYOUT_RAW), fu = grouped_fmt(c.up_type, LAYOUT_RAW), fd = grouped_fmt(c.down_type, m->down_layout);
     const size_t hb = type_size(c.hidden_type), ob = type_size(out_type);
     const int grid = num_sms(dev);
     for (int t0 = 0; t0 < qlen; t0 += Tc) {
@@ -677,21 +927,39 @@ int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, cons
         const int ub_gu = (P / kGN + E) * (I / kGM), ub_d = (P / kGN + E) * (H / kGM);
         grp_tiles_kernel<<<(ub_gu + 255) / 256, 256, 0, s>>>(g.nt_prefix, g.offsets, E, I / kGM, g.tinfo_gu);
         grp_tiles_kernel<<<(ub_d + 255) / 256, 256, 0, s>>>(g.nt_prefix, g.offsets, E, H / kGM, g.tinfo_d);
-        grp_quant_x_kernel<<<(T * (H / 256) + 7) / 8, 256, 0, s>>>(x_c, c.hidden_type, T, H, g.xq, g.xd, g.xbs);
-        GrpGemmParams gp{};
-        gp.R = I; gp.Kc = H; gp.xq = g.xq; gp.xd = g.xd; gp.xbs = g.xbs; gp.rowmap = g.tokmap; gp.tinfo = g.tinfo_gu; gp.nt_prefix = g.nt_prefix; gp.E = E;
-        gp.expert_bytes = (long)I * (H / 256) * weight_block_bytes(c.gate_type);
-        gp.w = reinterpret_cast<const uint8_t*>(c.gate_proj); gp.out = g.g; gp.trace = g_grp_trace;
-        grouped_gemm(fg, gp, grid, s);
-        gp.expert_bytes = (long)I * (H / 256) * weight_block_bytes(c.up_type);
-        gp.w = reinterpret_cast<const uint8_t*>(c.up_proj); gp.out = g.u; gp.trace = nullptr;
-        grouped_gemm(fu, gp, grid, s);
-        grp_act_quant_kernel<<<(P * (I / 256) + 7) / 8, 256, 0, s>>>(g.g, g.u, g.offsets, E, I, c.use_silu, g.aq, g.ad, g.abs16);
-        GrpGemmParams gd{};
-        gd.R = H; gd.Kc = I; gd.xq = g.aq; gd.xd = g.ad; gd.xbs = g.abs16; gd.rowmap = nullptr; gd.tinfo = g.tinfo_d; gd.nt_prefix = g.nt_prefix;
-        gd.E = E; gd.expert_bytes = (long)H * (I / 256) * weight_block_bytes(c.down_type);
-        gd.w = reinterpret_cast<const uint8_t*>(c.down_proj); gd.out = g.dd; gd.trace = g_grp_trace ? g_grp_trace + 3 * 96 * 4 : nullptr;
-        grouped_gemm(fd, gd, grid, s);
+        if (i4) {   // the same ten launches with the plane splits in place of the Q8_K quantisers
+            if (np == 1) grp_split_x_kernel<1><<<(T * (H / 8) + 255) / 256, 256, 0, s>>>(x_c, c.hidden_type, T, H, g.xp);
+            else grp_split_x_kernel<3><<<(T * (H / 8) + 255) / 256, 256, 0, s>>>(x_c, c.hidden_type, T, H, g.xp);
+            GrpI4Params ip{};
+            ip.R = I; ip.Kc = H; ip.x = g.xp; ip.rowmap = g.tokmap; ip.tinfo = g.tinfo_gu; ip.nt_prefix = g.nt_prefix; ip.E = E;
+            ip.expert_bytes = (long)I * (H / 256) * SZ_RAWINT4;
+            ip.w = reinterpret_cast<const uint8_t*>(c.gate_proj); ip.out = g.g; ip.trace = g_grp_trace;
+            grouped_i4(np, ip, grid, s);
+            ip.w = reinterpret_cast<const uint8_t*>(c.up_proj); ip.out = g.u; ip.trace = nullptr;
+            grouped_i4(np, ip, grid, s);
+            grp_split_act_kernel<<<(P * (I / 8) + 255) / 256, 256, 0, s>>>(g.g, g.u, g.offsets, E, I, c.use_silu, g.ap);
+            GrpI4Params id{};
+            id.R = H; id.Kc = I; id.x = g.ap; id.rowmap = nullptr; id.tinfo = g.tinfo_d; id.nt_prefix = g.nt_prefix; id.E = E;
+            id.expert_bytes = (long)H * (I / 256) * SZ_RAWINT4;
+            id.w = reinterpret_cast<const uint8_t*>(c.down_proj); id.out = g.dd; id.trace = g_grp_trace ? g_grp_trace + 3 * 96 * 4 : nullptr;
+            grouped_i4(3, id, grid, s);
+        } else {
+            grp_quant_x_kernel<<<(T * (H / 256) + 7) / 8, 256, 0, s>>>(x_c, c.hidden_type, T, H, g.xq, g.xd, g.xbs);
+            GrpGemmParams gp{};
+            gp.R = I; gp.Kc = H; gp.xq = g.xq; gp.xd = g.xd; gp.xbs = g.xbs; gp.rowmap = g.tokmap; gp.tinfo = g.tinfo_gu; gp.nt_prefix = g.nt_prefix; gp.E = E;
+            gp.expert_bytes = (long)I * (H / 256) * weight_block_bytes(c.gate_type);
+            gp.w = reinterpret_cast<const uint8_t*>(c.gate_proj); gp.out = g.g; gp.trace = g_grp_trace;
+            grouped_gemm(fg, gp, grid, s);
+            gp.expert_bytes = (long)I * (H / 256) * weight_block_bytes(c.up_type);
+            gp.w = reinterpret_cast<const uint8_t*>(c.up_proj); gp.out = g.u; gp.trace = nullptr;
+            grouped_gemm(fu, gp, grid, s);
+            grp_act_quant_kernel<<<(P * (I / 256) + 7) / 8, 256, 0, s>>>(g.g, g.u, g.offsets, E, I, c.use_silu, g.aq, g.ad, g.abs16);
+            GrpGemmParams gd{};
+            gd.R = H; gd.Kc = I; gd.xq = g.aq; gd.xd = g.ad; gd.xbs = g.abs16; gd.rowmap = nullptr; gd.tinfo = g.tinfo_d; gd.nt_prefix = g.nt_prefix;
+            gd.E = E; gd.expert_bytes = (long)H * (I / 256) * weight_block_bytes(c.down_type);
+            gd.w = reinterpret_cast<const uint8_t*>(c.down_proj); gd.out = g.dd; gd.trace = g_grp_trace ? g_grp_trace + 3 * 96 * 4 : nullptr;
+            grouped_gemm(fd, gd, grid, s);
+        }
         grp_combine_kernel<<<dim3((H + 255) / 256, T), 256, 0, s>>>(g.dd, g.pos, w_c, T, k, H, bsz, t0, o_c, out_type);
         KTB_LAUNCH_CHECK();
         count_launch(9);   // + the one KTB_LAUNCH_CHECK counts = 10 launches per chunk

@@ -712,13 +712,14 @@ void grouped_set_trace(long long* t);
 }
 // qlen from which the per-expert tensor-core GEMMs (grouped.cu) replace the per-pair GEMV kernels: the reference makes the
 // same split between MOE::forward_one and MOE::forward_many (moe.cpp:367-377, threshold group_min_len).  48 tokens; 80 for a
-// handle with an IQ1_S or IQ2_XXS tensor, whose per-pair kernels stay faster up to about 68 tokens at DeepSeek-R1's shapes
-// (DESIGN.md §5).  KTB200_GROUPED_MIN, when set, is the threshold of every handle (0: never).
+// handle with an IQ1_S or IQ2_XXS tensor, whose per-pair kernels stay faster up to about 68 tokens at DeepSeek-R1's shapes;
+// 96 for RAWINT4_G32, whose per-pair kernels stay faster up to 88 tokens at Kimi-K2's shapes (DESIGN.md §5).  KTB200_GROUPED_MIN, when set, is the threshold of every handle (0: never).
 void ktb200_debug_grouped(long long* trace_dev) { ktb::grouped_set_trace(trace_dev); }
 static int grouped_min_qlen(const ktb200_moe_config& c) {
     static const char* env = getenv("KTB200_GROUPED_MIN");
     static const int v = env ? atoi(env) : 0;
     if (env) return v;
+    if (is_rawint4(c.gate_type)) return 96;
     return is_iquant(c.gate_type) || is_iquant(c.up_type) || is_iquant(c.down_type) ? 80 : 48;
 }
 

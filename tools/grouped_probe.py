@@ -1,31 +1,49 @@
 """Times the grouped (prefill) MoE path at DeepSeek-V3 shapes (E 256, H 7168, I 2048, k 8, BF16) against the per-pair kernels,
-for three expert type sets: Q4_K/Q4_K/Q6_K and DeepSeek-R1's IQ1_S x3 and IQ1_S/IQ1_S/IQ2_XXS.
+for three expert type sets: Q4_K/Q4_K/Q6_K and DeepSeek-R1's IQ1_S x3 and IQ1_S/IQ1_S/IQ2_XXS; and set "i4" at Kimi-K2's shapes
+(RAWINT4_G32 x3, E 384, 60 MoE layers), packed with ktb200_rawint4_pack from seeded words and scales as tools/rawint4_probe.py.
 
 Every (type set, arm) runs in an interpreter of its own on the same seeded weights and inputs: arm "grouped" as shipped,
 arm "per-pair" with KTB200_GROUPED_MIN above every qlen (the threshold is read once per process), and, when BASELINE_LIB names
 another build of libktb200.so, arm "baseline" = the grouped path of that build.  Arms alternate, REPS times; the table gives
-the fastest repetition, ms per layer, tok/s over 58 MoE layers, and the share of the HBM bound for the bytes the grouped GEMMs
+the fastest repetition, ms per layer, tok/s over the model's MoE layers (V3/R1 58, K2 60), and the share of the HBM bound for the bytes the grouped GEMMs
 read (every expert's three matrices once per 32-token tile of its tokens, at 3.35 TB/s).  Outputs are compared at every timed
 size: per-pair against grouped within assert_bf16_close's bound, baseline against grouped bit for bit where both builds run
 the same kernels (else within that bound).
 
     python tools/grouped_probe.py                       TYPES=q4k,iq1x3,iq1_iq1_iq2  QLENS=48,64,256,1024,4096  REPS=2
+    TYPES=i4 QLENS=8,16,24,32,48,64,128,256,1024,4096 python tools/grouped_probe.py
     TRACE=1 python tools/grouped_probe.py               clock64 stamps of the gate and down GEMMs' CTA 0 (grouped arm)
 """
 import json, os, subprocess, sys, tempfile
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-Q4_K, Q6_K, IQ2_XXS, IQ1_S, BF16 = 12, 14, 16, 19, 30
-TYPE_SETS = {"q4k": (Q4_K, Q4_K, Q6_K), "iq1x3": (IQ1_S,) * 3, "iq1_iq1_iq2": (IQ1_S, IQ1_S, IQ2_XXS)}
-NAMES = {Q4_K: "Q4_K", Q6_K: "Q6_K", IQ1_S: "IQ1_S", IQ2_XXS: "IQ2_XXS"}
-BLOCK = {Q4_K: 144, Q6_K: 210, IQ1_S: 50, IQ2_XXS: 66}
-E, k, H, I, LAYERS, HBM = int(os.environ.get("E", 256)), 8, 7168, 2048, 58, 3.35e12
+Q4_K, Q6_K, IQ2_XXS, IQ1_S, BF16, I4 = 12, 14, 16, 19, 30, 256
+TYPE_SETS = {"q4k": (Q4_K, Q4_K, Q6_K), "iq1x3": (IQ1_S,) * 3, "iq1_iq1_iq2": (IQ1_S, IQ1_S, IQ2_XXS), "i4": (I4,) * 3}
+NAMES = {Q4_K: "Q4_K", Q6_K: "Q6_K", IQ1_S: "IQ1_S", IQ2_XXS: "IQ2_XXS", I4: "RAWINT4_G32"}
+BLOCK = {Q4_K: 144, Q6_K: 210, IQ1_S: 50, IQ2_XXS: 66, I4: 144}
+KERNEL = {Q4_K: "grouped_gemm_kernel<0>", Q6_K: "grouped_gemm_kernel<1>", IQ1_S: "grouped_gemm_kernel<2>", IQ2_XXS: "grouped_gemm_kernel<3>",
+          I4: "grouped_i4_kernel<1> (gate, BF16) / <3> (down)"}
+k, H, I, HBM = 8, 7168, 2048, 3.35e12
+# (experts, MoE layers) per type set: DeepSeek-V3/R1 256 and 58, Kimi-K2 384 and 60; E in the environment overrides the experts
+SHAPE = {"i4": (384, 60)}
+set_e = lambda tset: int(os.environ.get("E", SHAPE.get(tset, (256, 58))[0]))
+set_layers = lambda tset: SHAPE.get(tset, (256, 58))[1]
 
 
-def weights(t, n, seed):
+def weights(t, n, seed, cols=H):
     """seeded raw blocks on the device: synth_blocks for the K-quants; random bytes with d in [0.75, 1.25) / 64 (IQ1_S) or / 512
-    (IQ2_XXS) for the i-quants (every bit pattern is a valid i-quant block)"""
+    (IQ2_XXS) for the i-quants (every bit pattern is a valid i-quant block); RAWINT4 packed from random words and bf16 scales
+    in [0.005, 0.025) (tools/rawint4_probe.py)"""
+    if t == I4:
+        from ktransformers_b200 import native
+        g = torch.Generator(device="cuda").manual_seed(seed)
+        packed = torch.randint(0, 256, (n // 2,), dtype=torch.uint8, device="cuda", generator=g).view(torch.int32)
+        scale = (torch.rand(n // 32, device="cuda", generator=g) * 0.02 + 0.005).to(torch.bfloat16)
+        blocks = torch.empty(n // 256 * 144, dtype=torch.uint8, device="cuda")
+        native.check(native.lib().ktb200_rawint4_pack(packed.data_ptr(), scale.data_ptr(), n // cols, cols, blocks.data_ptr(),
+                                                      torch.cuda.current_stream().cuda_stream))
+        return blocks
     if t in (Q4_K, Q6_K):
         from ktransformers_b200.util.synth import synth_blocks
         return synth_blocks(t, n, "cuda", seed)
@@ -43,7 +61,8 @@ def worker(tset, qlens, outdir):
         native.LIB_PATH = os.environ["PROBE_LIB"]
     lib = native.lib()
     gt, ut, dt = TYPE_SETS[tset]
-    w3 = [weights(t, E * I * H, s) for t, s in ((gt, 1), (ut, 2), (dt, 3))]
+    E = set_e(tset)
+    w3 = [weights(t, E * I * H, s, c) for t, s, c in ((gt, 1, H), (ut, 2, H), (dt, 3, I))]
     cfg = native.MoeConfig(E, k, H, I, 64, 10, max(qlens), 1, *(t.data_ptr() for t in w3), gt, ut, dt, BF16, 0)
     h = C.c_void_p()
     native.check(lib.ktb200_moe_create(C.byref(cfg), 0, C.byref(h)))
@@ -76,8 +95,7 @@ def worker(tset, qlens, outdir):
         tr = torch.zeros(2 * 3 * 96 * 4, dtype=torch.int64, device="cuda")
         lib.ktb200_debug_grouped(tr.data_ptr()); run(); torch.cuda.synchronize(); lib.ktb200_debug_grouped(None)
         t = tr.cpu().numpy().reshape(2, 3, 96, 4)
-        for kname, kk in ((f"gate ({NAMES[gt]}, grouped_gemm_kernel<{(0, 0, 2, 3)[[Q4_K, Q6_K, IQ1_S, IQ2_XXS].index(gt)]}>)", 0),
-                          (f"down ({NAMES[dt]}, grouped_gemm_kernel<{(0, 1, 2, 3)[[Q4_K, Q6_K, IQ1_S, IQ2_XXS].index(dt)]}>)", 1)):
+        for kname, kk in ((f"gate ({NAMES[gt]}, {KERNEL[gt]})", 0), (f"down ({NAMES[dt]}, {KERNEL[dt]})", 1)):
             t0 = t[kk, 0, 0, 0]
             print(f"--- {kname}, qlen {qlen}: cycles since the producer's first stage; P = wait_group done / smem_free seen / arrived, "
                   f"M = before ab_full / ab_full seen / MMAs + scale-and-add done / arrived")
@@ -129,9 +147,11 @@ def main():
                     b["ms"] = min(b["ms"], v["ms"])
                     b.setdefault("all", []).append(v["ms"])
         gt, ut, dt = TYPE_SETS[tset]
+        E, LAYERS = set_e(tset), set_layers(tset)
         eb = [I * H // 256 * BLOCK[t] for t in (gt, ut, dt)]
         print(f"\n{NAMES[gt]}/{NAMES[ut]}/{NAMES[dt]}  (E {E}, H {H}, I {I}, k {k}, BF16; ms per layer = fastest of {reps}, all reps in brackets)")
-        print(f"{'qlen':>6} | {'grouped ms':>22} {'tok/s/58L':>9} {'HBM share':>9} | {'per-pair ms':>22} {'tok/s/58L':>9} | {'speed-up':>8} | outputs")
+        tl = f"tok/s/{LAYERS}L"
+        print(f"{'qlen':>6} | {'grouped ms':>22} {tl:>9} {'HBM share':>9} | {'per-pair ms':>22} {tl:>9} | {'speed-up':>8} | outputs")
         for q in qlens:
             gr, pp = best[("grouped", q)], best[("per-pair", q)]
             tile_bytes = sum(gr["tiles"]) * sum(eb)
