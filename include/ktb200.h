@@ -119,8 +119,8 @@ int ktb200_moe_warm_up(ktb200_moe* moe, void* stream);
  * vec_dot_type (Q8_K / Q8_0) with the reference's rounding, integer dot products, fp32 scales,
  * fp32 accumulation over experts in expert_ids order, output rounded like ggml from_float.
  * RAWINT4_G32 experts are W4A16 instead: fp32 activations against (u - 8) * scale, fp32 sums (DESIGN.md §2).
- * Routes: per-pair GEMV kernels for short batches; from 48 tokens (80 for a handle with an i-quant tensor, 96 for RAWINT4;
- * KTB200_GROUPED_MIN overrides) the grouped tensor-core GEMMs, which read each expert once per 32-token tile and grow a
+ * Routes: per-pair GEMV kernels for short batches; from 48 tokens (Q2_K..Q6_K experts; 80 for a handle with an i-quant
+ * tensor, 96 for RAWINT4; KTB200_GROUPED_MIN overrides) the grouped tensor-core GEMMs, which read each expert once per 32-token tile and grow a
  * per-device scratch arena on first use. */
 int ktb200_moe_forward(ktb200_moe* moe, int qlen, int k, const int64_t* expert_ids_dev,
                        const float* weights_dev, const void* input_dev, void* output_dev,

@@ -30,6 +30,17 @@
 // That keeps the Q4_K producers' asynchronous 6-stage prefetch; 16-bit loads staged in registers would hold those stages in
 // the producers' 96 registers and take two to four times the load instructions.  Their own shared-memory plan: no mins tiles,
 // 32-row B, 48-byte raw slots and the 16 KB codebook in place of the Q4_K / Q6_K plan's 80-byte slots.
+//
+// Q5_K (FMT 5), Q3_K (FMT 6) and Q2_K (FMT 7), the other K-quants of llama.cpp's expert mixes, reuse those two shapes:
+//   Q5_K  the Q4_K path with the fifth bit: bit 2c / 2c + 1 of qh[l] ORed in as bit 4 of the u8 operand (0..31); same header,
+//         mins MMA and finish.  Seven 16-byte raw units per thread (qh adds two), so a 112-byte pitch (odd multiple of 16)
+//         and a 4-deep raw ring in the region of the 6-deep 80-byte one.
+//   Q3_K  the Q6_K path: s8 operands q - 4 (hmask bit clear) in -4..3, the 6-bit scales - 32 as the header's 8 signed bytes,
+//         finish (d * dx) * isum.  110-byte blocks are 2-byte aligned: covering 4-byte words + 16-bit funnel shift (as IQ).
+//   Q2_K  the Q6_K sub-block MMAs on operands 0..3, the 4-bit scales in the int32 scale-and-add, the 16 4-bit mins through
+//         the Q4_K mins MMA (K = 16, one min per 16-value sum) and Q4_K's finish.  84-byte blocks: 4-byte cp.async words.
+// Q3_K / Q2_K split a row's stage between its two producer threads by byte position l (as Q6_K), so a thread converts 16 qs
+// (and 16 hmask) bytes and the 80-byte plan holds its share.
 #include <cuda_fp16.h>
 
 #include "act_quant.cuh"
@@ -60,6 +71,9 @@ struct GrpMisc {
 };
 constexpr int kGSmem = kOffMiscG + (int)sizeof(GrpMisc) + 1024;
 static_assert(kGSmem <= 227 * 1024, "shared memory budget");
+// Q5_K: the kGSmem plan with seven-unit raw slots (7 x 16 = 112 bytes, an odd multiple of 16) 4 deep in the raw region
+constexpr int kGRaw5 = 4, kRawPitch5 = 112, kRawSlot5 = 2 * kGM * kRawPitch5;
+static_assert(kGRaw5 * kRawSlot5 <= kGRaw * kRawSlot, "Q5_K raw ring");
 // IQ1_S / IQ2_XXS plan: A stages as above, B of 32 token rows, raw slots of three 16-byte units per thread (0-1 the covering
 // weight words and the word of d, 24 the token scale, 2 the activation piece), the codebook (IQ1_S 2048 x 8 B; IQ2_XXS 256 x 8 B
 // grid + 128 x 8 B sign masks), the same misc block
@@ -125,11 +139,20 @@ __global__ void grp_tiles_kernel(const int* nt_prefix, const int* offsets, int E
 //   IQ (three units, sub-blocks 4 hh + 2 part + {0, 1}): IQ1_S bytes 0-11 the words covering qs[8 (2 hh + part) .. + 8],
 //         12-19 those covering qh[2 (2 hh + part) .. + 2]; IQ2_XXS 0-19 those covering the 16 bytes of the two sub-blocks;
 //         20 the word holding d, 24 token scale (threads 64-95), 2 activation piece
+//   Q5_K: Q4_K's five units, 5-6 the 32 bytes of qh
+//   Q3_K (l = 16 part + 0..15 of the half): bytes 0-15 the words covering scales[12] and d, 16-35 those covering hmask[l],
+//         36-55 those covering qs[32 hh + l], 56 token scale (threads 64-95), 4 activation piece
+//   Q2_K: 0 scales[16], 1 qs[32 hh + l], 2 d | dmin (bytes 32-35), 3 activation piece, 4 as Q4_K
 template <int FMT>
 __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGemmParams p) {
-    constexpr bool IQ = FMT >= 2;
-    constexpr int offB = IQ ? kOffBI : kOffB, strideB = IQ ? kGBI : kGB, offRaw = IQ ? kOffRawI : kOffRaw, rawPitch = IQ ? kRawPitchI : kRawPitch,
-                  rawSlot = IQ ? kRawSlotI : kRawSlot, BS = FMT == 2 ? SZ_IQ1_S : SZ_IQ2_XXS;
+    constexpr bool IQ = FMT == 2 || FMT == 3;
+    constexpr bool K4 = FMT == 0 || FMT == 5;                 // 32-value sub-blocks with mins, u8 operands (Q4_K, Q5_K)
+    constexpr bool MINS = K4 || FMT == 7;                     // the mins MMA and Q4_K's finish (Q4_K, Q5_K, Q2_K)
+    constexpr bool SUB16 = FMT == 1 || FMT == 6 || FMT == 7;  // 16-value sub-blocks on the 64-row B (Q6_K, Q3_K, Q2_K)
+    constexpr int nRaw = FMT == 5 ? kGRaw5 : kGRaw;
+    constexpr int offB = IQ ? kOffBI : kOffB, strideB = IQ ? kGBI : kGB, offRaw = IQ ? kOffRawI : kOffRaw,
+                  rawPitch = IQ ? kRawPitchI : FMT == 5 ? kRawPitch5 : kRawPitch, rawSlot = IQ ? kRawSlotI : FMT == 5 ? kRawSlot5 : kRawSlot,
+                  BS = FMT == 2 ? SZ_IQ1_S : FMT == 3 ? SZ_IQ2_XXS : FMT == 6 ? SZ_Q3_K : SZ_Q2_K;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
@@ -173,11 +196,12 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
             const int4 ti = __ldg(p.tinfo + ftile);
             fxq = nullptr; fbs = nullptr; fdx = nullptr;
             if (bn < ti.w) fxq = p.xq + (long)(p.rowmap ? __ldg(p.rowmap + ti.z + bn) : ti.z + bn) * p.Kc + pc * 16;
-            if (FMT == 0 && pt < 64 && (pt >> 1) < ti.w) fbs = p.xbs + (long)(p.rowmap ? __ldg(p.rowmap + ti.z + (pt >> 1)) : ti.z + (pt >> 1)) * (p.Kc / 16) + (pt & 1) * 8;
+            if (MINS && pt < 64 && (pt >> 1) < ti.w) fbs = p.xbs + (long)(p.rowmap ? __ldg(p.rowmap + ti.z + (pt >> 1)) : ti.z + (pt >> 1)) * (p.Kc / 16) + (pt & 1) * 8;
             if (pt >= 64 && pt < 96 && pt - 64 < ti.w) fdx = p.xd + (long)(p.rowmap ? __ldg(p.rowmap + ti.z + pt - 64) : ti.z + pt - 64) * nblk;
             const int row = ti.y + r;
             if (FMT == 0) fw = p.w + (long)ti.x * p.expert_bytes + (long)row * nblk * SZ_Q4_K + 16 + part * 32;   // this thread's qs of block 0, first half
-            else if (IQ) fw = p.w + (long)ti.x * p.expert_bytes + (long)row * nblk * BS;                         // block 0 of the row
+            else if (FMT == 5) fw = p.w + (long)ti.x * p.expert_bytes + (long)row * nblk * SZ_Q5_K + 48 + part * 32;
+            else if (IQ || FMT >= 6) fw = p.w + (long)ti.x * p.expert_bytes + (long)row * nblk * BS;              // block 0 of the row
             else {
                 fitem = p.w + (long)ti.x * p.expert_bytes + (long)(row >> 2) * 4 * nblk * SZ_Q6_K;
                 ffi = (row & 3) * nblk;
@@ -187,11 +211,39 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
         auto issue = [&](uint32_t dst) {
             if (ftile < total_tiles) {
                 const int hh = fst & 1;
-                if (FMT == 0) {
+                if (K4) {
                     const uint8_t* q = fw + hh * 64;
                     cp_async16(dst, q);
                     cp_async16(dst + 16, q + 16);
-                    if (part == 0 || hh == 1) cp_async16(dst + 32, fw - 16 - part * 32);
+                    if (part == 0 || hh == 1) cp_async16(dst + 32, fw - (FMT == 5 ? 48 : 16) - part * 32);
+                    if (FMT == 5) {   // qh[0..31]
+                        cp_async16(dst + 80, fw - 32 - part * 32);
+                        cp_async16(dst + 96, fw - 16 - part * 32);
+                    }
+                } else if (FMT == 6) {
+                    // the words covering hmask[l] and qs[32 hh + l] (l = 16 part + 0..15): a fifth one only when the block starts
+                    // mid-word; part 0 the four covering scales[12] and d (bytes 96-109)
+                    const bool odd = (reinterpret_cast<uintptr_t>(fw) & 2) != 0;
+                    const uint8_t* hm = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(fw + 16 * part) & ~(uintptr_t)3);
+                    const uint8_t* qs = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(fw + 32 + 32 * hh + 16 * part) & ~(uintptr_t)3);
+#pragma unroll
+                    for (int i = 0; i < 4; i++) { cp_async4(dst + 16 + 4 * i, hm + 4 * i); cp_async4(dst + 36 + 4 * i, qs + 4 * i); }
+                    if (odd) { cp_async4(dst + 32, hm + 16); cp_async4(dst + 52, qs + 16); }
+                    if (part == 0) {
+                        const uint8_t* sc = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(fw + 96) & ~(uintptr_t)3);
+#pragma unroll
+                        for (int i = 0; i < 4; i++) cp_async4(dst + 4 * i, sc + 4 * i);
+                    }
+                } else if (FMT == 7) {
+                    // qs[32 hh + l] (l = 16 part + 0..15); scales[16] where this thread needs them (part 1: its mins); d | dmin
+                    const uint8_t* q = fw + 16 + 32 * hh + 16 * part;
+#pragma unroll
+                    for (int i = 0; i < 4; i++) cp_async4(dst + 16 + 4 * i, q + 4 * i);
+                    if (part == 0 || hh == 1) {
+#pragma unroll
+                        for (int i = 0; i < 4; i++) cp_async4(dst + 4 * i, fw + 4 * i);
+                    }
+                    if (part == 0) cp_async4(dst + 32, fw + 80);
                 } else if (IQ) {
                     // every word fetched holds at least one byte this thread needs (so it lies inside the tensor's pages);
                     // the last word of a field is only needed when the block starts on a word (the fields then start mid-word)
@@ -221,11 +273,11 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                         cp_async4(dst + 72, fitem + (long)13 * c16 + (ffi >> 1) * 4);
                     }
                 }
-                if (fxq) { cp_async16(dst + (IQ ? 32 : 48), fxq); fxq += 128; }
+                if (fxq) { cp_async16(dst + (IQ ? 32 : FMT == 6 ? 64 : 48), fxq); fxq += 128; }
                 if (hh == 1) {
-                    if (FMT == 0 && fbs) { cp_async16(dst + 64, fbs); fbs += 16; }
-                    if (fdx) { cp_async4(dst + (FMT == 0 ? 64 : IQ ? 24 : 76), fdx); fdx += 1; }
-                    fw += FMT == 0 ? SZ_Q4_K : IQ ? BS : 16;
+                    if (MINS && fbs) { cp_async16(dst + 64, fbs); fbs += 16; }
+                    if (fdx) { cp_async4(dst + (MINS ? 64 : IQ ? 24 : FMT == 6 ? 56 : 76), fdx); fdx += 1; }
+                    fw += FMT == 0 ? SZ_Q4_K : FMT == 5 ? SZ_Q5_K : (IQ || FMT >= 6) ? BS : 16;
                     ffi++;
                 }
                 if (++fst == nst) { fst = 0; ftile += gridDim.x; enter_tile(); }
@@ -233,39 +285,56 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
             cp_async_commit();
         };
         enter_tile();
-        for (int i = 0; i < kGRaw; i++) issue(raw_dst + i * rawSlot);
+        for (int i = 0; i < nRaw; i++) issue(raw_dst + i * rawSlot);
         int slot = 0;
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int4 ti = __ldg(p.tinfo + tile);
             const int n_valid = ti.w;
             int dsel = ((ti.y + r) & 3) * nblk;   // Q6_K: which half of the fetched word holds this block's d
-            // IQ: 16 when the current block starts on a word (its fields then start mid-word), else 0; 50 and 66 are 2 mod 4,
-            // so it alternates block by block
-            uint32_t ish = IQ ? ((reinterpret_cast<uintptr_t>(p.w + (long)ti.x * p.expert_bytes + (long)(ti.y + r) * nblk * BS) & 2) ? 0u : 16u) : 0u;
+            // IQ: 16 when the current block starts on a word (its fields then start mid-word), else 0; Q3_K (fields at word
+            // offsets of the block): 16 when it starts mid-word.  50, 66 and 110 are 2 mod 4, so it alternates block by block
+            uint32_t ish = IQ ? ((reinterpret_cast<uintptr_t>(p.w + (long)ti.x * p.expert_bytes + (long)(ti.y + r) * nblk * BS) & 2) ? 0u : 16u)
+                         : FMT == 6 ? ((reinterpret_cast<uintptr_t>(p.w + (long)ti.x * p.expert_bytes + (long)(ti.y + r) * nblk * BS) & 2) ? 16u : 0u) : 0u;
             for (int st = 0; st < nst; st++) {
                 const int hh = st & 1;
                 const bool tr = p.trace && blockIdx.x == 0 && tid == 0 && tile == 0 && st < 96;
                 if (tr) p.trace[(0 * 96 + st) * 4 + 0] = clock64();
-                cp_async_wait<kGRaw - 1>();
+                cp_async_wait<nRaw - 1>();
                 if (tr) p.trace[(0 * 96 + st) * 4 + 1] = clock64();
                 const uint4* rs = reinterpret_cast<const uint4*>(raw_src + slot * rawSlot);
-                const uint4 f0 = rs[0], f1 = rs[1], f2 = rs[2], f3 = rs[IQ ? 2 : 3], f4 = rs[IQ ? 1 : 4];
+                const uint4 f0 = rs[0], f1 = rs[1], f2 = rs[2], f3 = rs[IQ ? 2 : FMT == 6 ? 4 : 3], f4 = rs[IQ ? 1 : FMT == 6 ? 3 : 4];
+                const uint4 f5 = rs[FMT == 5 ? 5 : 0], f6 = rs[FMT == 5 ? 6 : 0];   // Q5_K: qh
                 issue(raw_dst + slot * rawSlot);   // refill the slot just read (thread-private bytes: no barrier involved)
-                slot = slot == kGRaw - 1 ? 0 : slot + 1;
+                slot = slot == nRaw - 1 ? 0 : slot + 1;
                 bar_wait(smem_u32(&misc.smem_free[stage]), sphase ^ 1);
                 bar_wait(smem_u32(&misc.hdr_free[hs]), hphase ^ 1);
                 if (tr) p.trace[(0 * 96 + st) * 4 + 2] = clock64();
                 uint8_t* arow = smem + stage * kGA + r * 128;
                 const uint4 z = make_uint4(0, 0, 0, 0);
-                if (FMT == 0) {
+                if (K4) {
                     // chunk c = 2 hh + part (32 bytes of qs): low nibbles = sub-block 2c (elements 64c .. 64c+31), high nibbles = sub-block 2c+1
                     const int pi = 4 * part;
-                    *reinterpret_cast<uint4*>(arow + (((pi + 0) ^ sw) << 4)) = make_uint4(f0.x & 0x0F0F0F0Fu, f0.y & 0x0F0F0F0Fu, f0.z & 0x0F0F0F0Fu, f0.w & 0x0F0F0F0Fu);
-                    *reinterpret_cast<uint4*>(arow + (((pi + 1) ^ sw) << 4)) = make_uint4(f1.x & 0x0F0F0F0Fu, f1.y & 0x0F0F0F0Fu, f1.z & 0x0F0F0F0Fu, f1.w & 0x0F0F0F0Fu);
-                    *reinterpret_cast<uint4*>(arow + (((pi + 2) ^ sw) << 4)) =
-                        make_uint4((f0.x >> 4) & 0x0F0F0F0Fu, (f0.y >> 4) & 0x0F0F0F0Fu, (f0.z >> 4) & 0x0F0F0F0Fu, (f0.w >> 4) & 0x0F0F0F0Fu);
-                    *reinterpret_cast<uint4*>(arow + (((pi + 3) ^ sw) << 4)) =
-                        make_uint4((f1.x >> 4) & 0x0F0F0F0Fu, (f1.y >> 4) & 0x0F0F0F0Fu, (f1.z >> 4) & 0x0F0F0F0Fu, (f1.w >> 4) & 0x0F0F0F0Fu);
+                    if (FMT == 0) {
+                        *reinterpret_cast<uint4*>(arow + (((pi + 0) ^ sw) << 4)) = make_uint4(f0.x & 0x0F0F0F0Fu, f0.y & 0x0F0F0F0Fu, f0.z & 0x0F0F0F0Fu, f0.w & 0x0F0F0F0Fu);
+                        *reinterpret_cast<uint4*>(arow + (((pi + 1) ^ sw) << 4)) = make_uint4(f1.x & 0x0F0F0F0Fu, f1.y & 0x0F0F0F0Fu, f1.z & 0x0F0F0F0Fu, f1.w & 0x0F0F0F0Fu);
+                        *reinterpret_cast<uint4*>(arow + (((pi + 2) ^ sw) << 4)) =
+                            make_uint4((f0.x >> 4) & 0x0F0F0F0Fu, (f0.y >> 4) & 0x0F0F0F0Fu, (f0.z >> 4) & 0x0F0F0F0Fu, (f0.w >> 4) & 0x0F0F0F0Fu);
+                        *reinterpret_cast<uint4*>(arow + (((pi + 3) ^ sw) << 4)) =
+                            make_uint4((f1.x >> 4) & 0x0F0F0F0Fu, (f1.y >> 4) & 0x0F0F0F0Fu, (f1.z >> 4) & 0x0F0F0F0Fu, (f1.w >> 4) & 0x0F0F0F0Fu);
+                    } else {   // Q5_K: bit 2c (low nibbles) or 2c + 1 (high nibbles) of qh[l] as bit 4
+                        const int hb = 2 * (2 * hh + part);
+                        const uint32_t q[8] = {f0.x, f0.y, f0.z, f0.w, f1.x, f1.y, f1.z, f1.w}, h[8] = {f5.x, f5.y, f5.z, f5.w, f6.x, f6.y, f6.z, f6.w};
+                        uint32_t lo[8], hi[8];
+#pragma unroll
+                        for (int i = 0; i < 8; i++) {
+                            lo[i] = (q[i] & 0x0F0F0F0Fu) | (((h[i] >> hb) << 4) & 0x10101010u);
+                            hi[i] = ((q[i] >> 4) & 0x0F0F0F0Fu) | (((h[i] >> hb) << 3) & 0x10101010u);
+                        }
+                        *reinterpret_cast<uint4*>(arow + (((pi + 0) ^ sw) << 4)) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+                        *reinterpret_cast<uint4*>(arow + (((pi + 1) ^ sw) << 4)) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
+                        *reinterpret_cast<uint4*>(arow + (((pi + 2) ^ sw) << 4)) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+                        *reinterpret_cast<uint4*>(arow + (((pi + 3) ^ sw) << 4)) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
+                    }
                     if (part == 0) misc.hdr[hs][r] = f2;
                     if (hh == 1) {   // A2 row: [m_0 m_0 m_1 m_1 ... m_7 m_7] against the sixteen 16-value activation sums; 4 mins per part
                         const uint32_t hw[4] = {f2.x, f2.y, f2.z, f2.w};
@@ -317,6 +386,53 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                     hrow[part] = ls[0] | (ls[1] << 16);
                     if (part == 0) hrow[2] = __float_as_uint(iq_d8((uint16_t)dbits));
                     if (hh == 1) ish ^= 16u;
+                } else if (FMT == 6) {
+                    // element 32 j + l of the half (l = 16 part + 0..15): (qs[32 hh + l] >> 2j & 3) - 4 unless bit 4 hh + j of
+                    // hmask[l] is set, built as (q | h << 2) - 4 per byte (flip bit 2, copy it into bits 3-7: no carries)
+                    const uint32_t hw5[5] = {f1.x, f1.y, f1.z, f1.w, f2.x}, qw5[5] = {f2.y, f2.z, f2.w, f4.x, f4.y};
+                    uint32_t m[4], q[4];
+#pragma unroll
+                    for (int i = 0; i < 4; i++) {
+                        m[i] = __funnelshift_r(hw5[i], hw5[i + 1], ish) >> (4 * hh);
+                        q[i] = __funnelshift_r(qw5[i], qw5[i + 1], ish);
+                    }
+#pragma unroll
+                    for (int j = 0; j < 4; j++) {
+                        uint32_t v[4];
+#pragma unroll
+                        for (int i = 0; i < 4; i++) {
+                            const uint32_t tt = (((q[i] >> (2 * j)) & 0x03030303u) | (((m[i] >> j) & 0x01010101u) << 2)) ^ 0x04040404u;
+                            v[i] = tt + (tt & 0x04040404u) * 62u;
+                        }
+                        *reinterpret_cast<uint4*>(arow + (((2 * j + part) ^ sw) << 4)) = make_uint4(v[0], v[1], v[2], v[3]);
+                    }
+                    if (part == 0) {   // the header of Q6_K: the half's 8 scales (6-bit, - 32) as int8, d as f32
+                        const uint32_t s0 = __funnelshift_r(f0.x, f0.y, ish), s1 = __funnelshift_r(f0.y, f0.z, ish), s2 = __funnelshift_r(f0.z, f0.w, ish);
+                        const uint32_t dbits = ish ? (f0.w >> 16) : (f0.w & 0xffffu);
+                        uint32_t c[2] = {((s0 >> (4 * hh)) & 0x0F0F0F0Fu) | (((s2 >> (4 * hh)) & 0x03030303u) << 4),
+                                         ((s1 >> (4 * hh)) & 0x0F0F0F0Fu) | (((s2 >> (4 * hh + 2)) & 0x03030303u) << 4)};
+#pragma unroll
+                        for (int i = 0; i < 2; i++) {   // - 32 as for Q6_K's quants
+                            const uint32_t tt = c[i] ^ 0x20202020u;
+                            c[i] = tt + (tt & 0x20202020u) * 6u;
+                        }
+                        misc.hdr[hs][r] = make_uint4(c[0], c[1], __float_as_uint(fp16_bits_to_f32((uint16_t)dbits)), 0);
+                    }
+                    if (hh == 1) ish ^= 16u;
+                } else if (FMT == 7) {
+                    // element 32 j + l of the half (l = 16 part + 0..15): qs[32 hh + l] >> 2j & 3
+#pragma unroll
+                    for (int j = 0; j < 4; j++)
+                        *reinterpret_cast<uint4*>(arow + (((2 * j + part) ^ sw) << 4)) =
+                            make_uint4((f1.x >> (2 * j)) & 0x03030303u, (f1.y >> (2 * j)) & 0x03030303u, (f1.z >> (2 * j)) & 0x03030303u, (f1.w >> (2 * j)) & 0x03030303u);
+                    // header: the half's 8 scales (low nibbles), d | dmin; A2 row (second half): the 16 mins (high nibbles), 8 per part
+                    if (part == 0) misc.hdr[hs][r] = make_uint4((hh ? f0.z : f0.x) & 0x0F0F0F0Fu, (hh ? f0.w : f0.y) & 0x0F0F0F0Fu, f2.x, 0);
+                    if (hh == 1) {
+                        const uint32_t m0 = part ? f0.z : f0.x, m1 = part ? f0.w : f0.y;
+                        uint8_t* a2 = smem + kOffA2 + stage * kGA2 + (r >> 3) * 256 + (r & 7) * 16 + part * 128;
+                        *reinterpret_cast<uint4*>(a2) = make_uint4(h2((m0 >> 4) & 15, (m0 >> 12) & 15), h2((m0 >> 20) & 15, m0 >> 28),
+                                                                   h2((m1 >> 4) & 15, (m1 >> 12) & 15), h2((m1 >> 20) & 15, m1 >> 28));
+                    }
                 } else {
                     // element 32 g + l of the half (l = 16 part + 0..15): g = 0 ql[l] & 15 | (qh & 3) << 4, g = 1 ql[32 + l] & 15 | (qh >> 2 & 3) << 4,
                     // g = 2 ql[l] >> 4 | (qh >> 4 & 3) << 4, g = 3 ql[32 + l] >> 4 | (qh >> 6 & 3) << 4; stored as q - 32 in int8
@@ -347,15 +463,15 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                 // activations: piece (bn, pc)
                 uint8_t* Bs = smem + offB + stage * strideB;
                 const uint4 bv = bn < n_valid ? f3 : z;
-                if (FMT != 1) {
+                if (!SUB16) {
                     *reinterpret_cast<uint4*>(Bs + bn * 128 + ((pc ^ (bn & 7)) << 4)) = bv;
-                } else {   // a 16-byte piece is one Q6_K sub-block: rows 0-31 keep the even pieces, rows 32-63 the odd ones
+                } else {   // a 16-byte piece is one 16-value sub-block: rows 0-31 keep the even pieces, rows 32-63 the odd ones
                     *reinterpret_cast<uint4*>(Bs + bn * 128 + ((pc ^ (bn & 7)) << 4)) = (pc & 1) ? z : bv;
                     *reinterpret_cast<uint4*>(Bs + (kGN + bn) * 128 + ((pc ^ (bn & 7)) << 4)) = (pc & 1) ? bv : z;
                 }
-                if (hh == 1 && pt < 96) {   // token scales, and (Q4_K) the sixteen 16-value sums of the super-block as fp16
-                    if (pt >= 64) misc.dxs[hs][pt - 64] = pt - 64 < n_valid ? __uint_as_float(FMT == 0 ? f4.x : IQ ? f4.z : f4.w) : 0.f;
-                    else if (FMT == 0) {
+                if (hh == 1 && pt < 96) {   // token scales, and (formats with mins) the sixteen 16-value sums of the super-block as fp16
+                    if (pt >= 64) misc.dxs[hs][pt - 64] = pt - 64 < n_valid ? __uint_as_float(MINS ? f4.x : (IQ || FMT == 6) ? f4.z : f4.w) : 0.f;
+                    else if (MINS) {
                         const int n2 = pt >> 1, kg = pt & 1;
                         uint4 vv = z;
                         if (n2 < n_valid) {
@@ -402,7 +518,7 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                     const uint4 hd = misc.hdr[hs][ra + 8 * h];
                     hw[h][0] = hd.x; hw[h][1] = hd.y; hw[h][2] = hd.z; hw[h][3] = hd.w;
                 }
-                if (FMT == 0) {
+                if (K4) {
                     int sc[2][4], mn;
 #pragma unroll
                     for (int h = 0; h < 2; h++) {   // (compile-time byte indices: no local-memory copy of the header)
@@ -426,23 +542,6 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                         fence_regs(v1);
 #pragma unroll
                         for (int i = 0; i < 16; i++) isum[i] += sc[(i >> 1) & 1][c] * (int)v0[i] + sc[(i >> 1) & 1][c + 1] * (int)v1[i];
-                    }
-                    if (hh == 1) {
-                        float ms[16];
-                        fence();
-                        mma_f16_m64n32(ms, smem_desc(base + kOffA2 + stage * kGA2 + g * (kGA2 / 2), 128, 256, kLayoutNone),
-                                       smem_desc(base + kOffB2 + stage * kGB2, 128, 256, kLayoutNone), 0);
-                        commit();
-                        wait<0>();
-                        fence_regs(ms);
-#pragma unroll
-                        for (int i = 0; i < 16; i++) {
-                            const __half2 dm = *reinterpret_cast<const __half2*>(&hw[(i >> 1) & 1][0]);
-                            const float dw = __low2float(dm), dmin = __high2float(dm);
-                            const float dx = misc.dxs[hs][8 * (i >> 2) + cq + (i & 1)];
-                            acc[i] += (dw * dx) * (float)isum[i] - (dmin * dx) * ms[i];
-                            isum[i] = 0;
-                        }
                     }
                 } else if (IQ) {
                     // sub-block c of the stage: one MMA into its own accumulator, times its ls (header word c / 2, half c % 2)
@@ -482,12 +581,29 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
 #pragma unroll
                         for (int i = 0; i < 32; i++) isum[i & 15] += sb8(hw[(i >> 1) & 1], 2 * c + (i >> 4)) * (int)v[i];
                     }
-                    if (hh == 1) {
+                    if (!MINS && hh == 1) {
 #pragma unroll
                         for (int i = 0; i < 16; i++) {
                             acc[i] += (__uint_as_float(hw[(i >> 1) & 1][2]) * misc.dxs[hs][8 * (i >> 2) + cq + (i & 1)]) * (float)isum[i];
                             isum[i] = 0;
                         }
+                    }
+                }
+                if (MINS && hh == 1) {   // the mins MMA and the finish; d | dmin in header word 0 (Q4_K, Q5_K) or 2 (Q2_K)
+                    float ms[16];
+                    fence();
+                    mma_f16_m64n32(ms, smem_desc(base + kOffA2 + stage * kGA2 + g * (kGA2 / 2), 128, 256, kLayoutNone),
+                                   smem_desc(base + kOffB2 + stage * kGB2, 128, 256, kLayoutNone), 0);
+                    commit();
+                    wait<0>();
+                    fence_regs(ms);
+#pragma unroll
+                    for (int i = 0; i < 16; i++) {
+                        const __half2 dm = *reinterpret_cast<const __half2*>(&hw[(i >> 1) & 1][FMT == 7 ? 2 : 0]);
+                        const float dw = __low2float(dm), dmin = __high2float(dm);
+                        const float dx = misc.dxs[hs][8 * (i >> 2) + cq + (i & 1)];
+                        acc[i] += (dw * dx) * (float)isum[i] - (dmin * dx) * ms[i];
+                        isum[i] = 0;
                     }
                 }
                 if (tr) p.trace[(1 * 96 + st) * 4 + 2] = clock64();
@@ -866,6 +982,9 @@ static int grouped_fmt(int type, int layout) {
     if (type == KTB200_TYPE_IQ1_S) return 2;
     if (type == KTB200_TYPE_IQ2_XXS) return 3;
     if (type == KTB200_TYPE_RAWINT4_G32) return 4;   // grouped_i4_kernel (NP picked per launch), never mixed with the others
+    if (type == KTB200_TYPE_Q5_K) return 5;
+    if (type == KTB200_TYPE_Q3_K) return 6;
+    if (type == KTB200_TYPE_Q2_K) return 7;
     return -1;
 }
 static void grouped_i4(int np, const GrpI4Params& p, int grid, cudaStream_t s) {
@@ -877,12 +996,15 @@ static void grouped_gemm(int fmt, const GrpGemmParams& p, int grid, cudaStream_t
         case 0: grouped_gemm_kernel<0><<<grid, kGThreads, kGSmem, s>>>(p); break;
         case 1: grouped_gemm_kernel<1><<<grid, kGThreads, kGSmem, s>>>(p); break;
         case 2: grouped_gemm_kernel<2><<<grid, kGThreads, kGSmemI, s>>>(p); break;
-        default: grouped_gemm_kernel<3><<<grid, kGThreads, kGSmemI, s>>>(p); break;
+        case 3: grouped_gemm_kernel<3><<<grid, kGThreads, kGSmemI, s>>>(p); break;
+        case 5: grouped_gemm_kernel<5><<<grid, kGThreads, kGSmem, s>>>(p); break;
+        case 6: grouped_gemm_kernel<6><<<grid, kGThreads, kGSmem, s>>>(p); break;
+        default: grouped_gemm_kernel<7><<<grid, kGThreads, kGSmem, s>>>(p); break;
     }
 }
 
-// true when ktb200_moe_forward may take the grouped tensor-core path for this handle: gate and up Q4_K, IQ1_S or IQ2_XXS (each
-// on its own), down any of those or Q6_K in the tile layout; or all three RAWINT4_G32
+// true when ktb200_moe_forward may take the grouped tensor-core path for this handle: gate and up Q4_K, Q5_K, Q3_K, Q2_K, IQ1_S
+// or IQ2_XXS (each on its own), down any of those or Q6_K in the tile layout; or all three RAWINT4_G32
 bool grouped_ok(const ktb200_moe* m, int k) {
     const ktb200_moe_config& c = m->cfg;
     const int fg = grouped_fmt(c.gate_type, LAYOUT_RAW), fu = grouped_fmt(c.up_type, LAYOUT_RAW), fd = grouped_fmt(c.down_type, m->down_layout);
@@ -908,6 +1030,9 @@ int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, cons
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmemI));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmemI));
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem));
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem));
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_i4_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, I4Plan<1>::kSmem));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_i4_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, I4Plan<3>::kSmem));
         attr[dev & 63] = true;

@@ -77,7 +77,8 @@ class KExpertsBase(ABC):
 
 
 class KExpertsB200(KExpertsBase):
-    """GPU-resident GGUF experts on the hand-written sm_90a kernels."""
+    """GPU-resident GGUF experts on the hand-written sm_90a kernels: per-pair GEMV kernels for decode batches, and the grouped
+    tensor-core GEMM from 48 tokens up for Q2_K / Q3_K / Q4_K / Q5_K / Q6_K experts (80 with an IQ1_S / IQ2_XXS tensor)."""
 
     # graph-safe output buffers per device, like KExpertsCPU.output_gpu_map (experts.py:147)
     output_gpu_map: dict = {}
@@ -337,7 +338,8 @@ class KTransformersExperts(BaseInjectedModule, KExpertsBase):
 class KTransformersExpertsV2(KTransformersExperts):
     """experts.py:1273-1350: the balance-serve variant whose forward carries `bsz_tensor` (device-side live batch size) and a
     CUDA-graph slot.  With `prefill_op: None` the generate experts serve both phases (one GPU-resident KExpertsB200: per-pair
-    GEMV kernels for decode batches, the grouped tensor-core path from 48 tokens up, 80 for IQ1_S / IQ2_XXS experts)."""
+    GEMV kernels for decode batches, the grouped tensor-core path from 48 tokens up for Q2_K-Q6_K experts, 80 for IQ1_S /
+    IQ2_XXS experts)."""
 
     def forward(self, input_tensor, expert_ids, weights, bsz_tensor=None, cuda_graph_idx=0):
         if self.mode == InferenceState.GENERATE or (self.mode == InferenceState.PREFILL and self.prefill_experts is None):

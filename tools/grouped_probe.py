@@ -1,5 +1,7 @@
 """Times the grouped (prefill) MoE path at DeepSeek-V3 shapes (E 256, H 7168, I 2048, k 8, BF16) against the per-pair kernels,
-for three expert type sets: Q4_K/Q4_K/Q6_K and DeepSeek-R1's IQ1_S x3 and IQ1_S/IQ1_S/IQ2_XXS; and set "i4" at Kimi-K2's shapes
+for the expert type sets Q4_K/Q4_K/Q6_K, DeepSeek-R1's IQ1_S x3 and IQ1_S/IQ1_S/IQ2_XXS, and the K-quant mixes "q5k" (Q5_K/Q5_K/Q6_K,
+Q5_K_M), "q3k" (Q3_K/Q3_K/Q4_K, Q3_K_M), "q2k" (Q2_K/Q2_K/Q3_K, Q2_K) and "q2k_q6k" (Q2_K/Q2_K/Q6_K: the per-pair kernels refuse
+a Q3_K down projection at these shapes, so this set gives Q2_K gate / up a per-pair time); and set "i4" at Kimi-K2's shapes
 (RAWINT4_G32 x3, E 384, 60 MoE layers), packed with ktb200_rawint4_pack from seeded words and scales as tools/rawint4_probe.py.
 
 Every (type set, arm) runs in an interpreter of its own on the same seeded weights and inputs: arm "grouped" as shipped,
@@ -11,6 +13,7 @@ size: per-pair against grouped within assert_bf16_close's bound, baseline agains
 the same kernels (else within that bound).
 
     python tools/grouped_probe.py                       TYPES=q4k,iq1x3,iq1_iq1_iq2  QLENS=48,64,256,1024,4096  REPS=2
+    TYPES=q5k,q3k,q2k python tools/grouped_probe.py
     TYPES=i4 QLENS=8,16,24,32,48,64,128,256,1024,4096 python tools/grouped_probe.py
     TRACE=1 python tools/grouped_probe.py               clock64 stamps of the gate and down GEMMs' CTA 0 (grouped arm)
 """
@@ -18,12 +21,14 @@ import json, os, subprocess, sys, tempfile
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-Q4_K, Q6_K, IQ2_XXS, IQ1_S, BF16, I4 = 12, 14, 16, 19, 30, 256
-TYPE_SETS = {"q4k": (Q4_K, Q4_K, Q6_K), "iq1x3": (IQ1_S,) * 3, "iq1_iq1_iq2": (IQ1_S, IQ1_S, IQ2_XXS), "i4": (I4,) * 3}
-NAMES = {Q4_K: "Q4_K", Q6_K: "Q6_K", IQ1_S: "IQ1_S", IQ2_XXS: "IQ2_XXS", I4: "RAWINT4_G32"}
-BLOCK = {Q4_K: 144, Q6_K: 210, IQ1_S: 50, IQ2_XXS: 66, I4: 144}
+Q2_K, Q3_K, Q4_K, Q5_K, Q6_K, IQ2_XXS, IQ1_S, BF16, I4 = 10, 11, 12, 13, 14, 16, 19, 30, 256
+TYPE_SETS = {"q4k": (Q4_K, Q4_K, Q6_K), "iq1x3": (IQ1_S,) * 3, "iq1_iq1_iq2": (IQ1_S, IQ1_S, IQ2_XXS), "i4": (I4,) * 3,
+             "q5k": (Q5_K, Q5_K, Q6_K), "q3k": (Q3_K, Q3_K, Q4_K), "q2k": (Q2_K, Q2_K, Q3_K), "q2k_q6k": (Q2_K, Q2_K, Q6_K)}
+NAMES = {Q2_K: "Q2_K", Q3_K: "Q3_K", Q4_K: "Q4_K", Q5_K: "Q5_K", Q6_K: "Q6_K", IQ1_S: "IQ1_S", IQ2_XXS: "IQ2_XXS", I4: "RAWINT4_G32"}
+BLOCK = {Q2_K: 84, Q3_K: 110, Q4_K: 144, Q5_K: 176, Q6_K: 210, IQ1_S: 50, IQ2_XXS: 66, I4: 144}
 KERNEL = {Q4_K: "grouped_gemm_kernel<0>", Q6_K: "grouped_gemm_kernel<1>", IQ1_S: "grouped_gemm_kernel<2>", IQ2_XXS: "grouped_gemm_kernel<3>",
-          I4: "grouped_i4_kernel<1> (gate, BF16) / <3> (down)"}
+          I4: "grouped_i4_kernel<1> (gate, BF16) / <3> (down)", Q5_K: "grouped_gemm_kernel<5>", Q3_K: "grouped_gemm_kernel<6>",
+          Q2_K: "grouped_gemm_kernel<7>"}
 k, H, I, HBM = 8, 7168, 2048, 3.35e12
 # (experts, MoE layers) per type set: DeepSeek-V3/R1 256 and 58, Kimi-K2 384 and 60; E in the environment overrides the experts
 SHAPE = {"i4": (384, 60)}
@@ -44,7 +49,7 @@ def weights(t, n, seed, cols=H):
         native.check(native.lib().ktb200_rawint4_pack(packed.data_ptr(), scale.data_ptr(), n // cols, cols, blocks.data_ptr(),
                                                       torch.cuda.current_stream().cuda_stream))
         return blocks
-    if t in (Q4_K, Q6_K):
+    if t in (Q2_K, Q3_K, Q4_K, Q5_K, Q6_K):
         from ktransformers_b200.util.synth import synth_blocks
         return synth_blocks(t, n, "cuda", seed)
     g = torch.Generator(device="cuda").manual_seed(seed)
@@ -126,7 +131,7 @@ def main():
     tmp = tempfile.mkdtemp(prefix="grouped_probe_")
     ok = True
     for tset in tsets:
-        best = {}
+        best, refused = {}, {}
         for rep in range(reps):
             for arm, env in arms.items():
                 d = os.path.join(tmp, tset, arm)
@@ -138,6 +143,11 @@ def main():
                                    env=env, capture_output=True, text=True)
                 lines = r.stdout.splitlines()
                 if r.returncode:
+                    err = [l[12:] for l in r.stderr.splitlines() if l.startswith("ValueError: ")]
+                    if arm != "grouped" and err:   # the library refuses the handle on this arm's route (per-pair kernels)
+                        refused[arm] = err[-1]
+                        print(f"{tset} {arm}: refused: {err[-1]}")
+                        continue
                     print(r.stdout[-2000:], r.stderr[-3000:])
                     raise SystemExit(f"{tset} {arm}: worker failed")
                 print("\n".join(l for l in lines if not l.startswith("RESULT ")), end="" if len(lines) < 2 else "\n")
@@ -153,13 +163,18 @@ def main():
         tl = f"tok/s/{LAYERS}L"
         print(f"{'qlen':>6} | {'grouped ms':>22} {tl:>9} {'HBM share':>9} | {'per-pair ms':>22} {tl:>9} | {'speed-up':>8} | outputs")
         for q in qlens:
-            gr, pp = best[("grouped", q)], best[("per-pair", q)]
+            gr, pp = best[("grouped", q)], best.get(("per-pair", q))
             tile_bytes = sum(gr["tiles"]) * sum(eb)
-            a, b = (np.load(os.path.join(tmp, tset, arm, f"{q}.npy")).view(np.uint16) for arm in ("grouped", "per-pair"))
-            close, exact = bf16_close(b, a)
-            cmp = f"per-pair {'within' if close else 'OUTSIDE'} bf16 bound ({exact:.2%} bit-identical)"
-            ok &= close
-            if "baseline" in arms:
+            a = np.load(os.path.join(tmp, tset, "grouped", f"{q}.npy")).view(np.uint16)
+            if pp:
+                close, exact = bf16_close(np.load(os.path.join(tmp, tset, "per-pair", f"{q}.npy")).view(np.uint16), a)
+                cmp = f"per-pair {'within' if close else 'OUTSIDE'} bf16 bound ({exact:.2%} bit-identical)"
+                ok &= close
+            else:
+                cmp = f"per-pair refused ({refused['per-pair']})"
+            if "baseline" in refused:
+                cmp += "; baseline refused"
+            elif "baseline" in arms:
                 # bit-identical where both builds take the same kernels; otherwise (a route the baseline build lacks) the
                 # per-pair bound
                 bl = best[("baseline", q)]
@@ -170,8 +185,8 @@ def main():
                 verdict = "bit-identical" if same else "within bf16 bound" if close else "OUTSIDE bf16 bound"
                 cmp += f"; baseline {verdict}, {bl['ms']:.3f} ms [{' '.join(f'{v:.3f}' for v in bl['all'])}]"
             fmt = lambda v: f"{v['ms']:8.3f} [{' '.join(f'{x:.2f}' for x in v['all'])}]"
-            print(f"{q:6d} | {fmt(gr):>22} {q / (LAYERS * gr['ms']) * 1e3:9.0f} {tile_bytes / HBM * 1e3 / gr['ms']:9.1%} | {fmt(pp):>22} "
-                  f"{q / (LAYERS * pp['ms']) * 1e3:9.0f} | {pp['ms'] / gr['ms']:7.2f}x | {cmp}", flush=True)
+            ppc = f"{fmt(pp):>22} {q / (LAYERS * pp['ms']) * 1e3:9.0f} | {pp['ms'] / gr['ms']:7.2f}x" if pp else f"{'-':>22} {'-':>9} | {'-':>8}"
+            print(f"{q:6d} | {fmt(gr):>22} {q / (LAYERS * gr['ms']) * 1e3:9.0f} {tile_bytes / HBM * 1e3 / gr['ms']:9.1%} | {ppc} | {cmp}", flush=True)
     print("all outputs agree" if ok else "OUTPUT MISMATCH")
     sys.exit(0 if ok else 1)
 
