@@ -418,6 +418,11 @@ void ktb200_debug_grouped(long long* trace_dev);
  *     (de-interleaved pairs, modeling_deepseek_v3.py:339-373) on k_pe and on every head's q_pe, and the paged cache write
  *     (custom_cache.py:147-193): q [T][heads][nope+64], kv_a_out [T][576], cos/sin fp32 [T][64], page_idx/page_offset
  *     int32 [T]; q_pe_out [T][heads][64].
+ * Both take dense rows: residual, delta and out are [T][hidden], q is [T][heads][nope+64] and kv_a_out is [T][576], each
+ * row right after the previous one.  A view of one projection output whose rows are wider (q_a and kv_a stacked in one
+ * [T][q_lora + 576] buffer) is therefore only valid at T = 1.
+ * add_rmsnorm: hidden even and <= 8192; residual, delta, weight and out 4-byte aligned (bf16 pairs), else KTB200_EINVAL
+ * before any device work (n_tokens = 0 included).
  * ------------------------------------------------------------------------------------------ */
 int ktb200_add_rmsnorm(void* residual_dev, const void* delta_dev, const void* weight_dev, float eps, void* out_dev, int n_tokens,
                        int hidden, void* stream);
@@ -427,14 +432,18 @@ int ktb200_mla_prep(const void* q_dev, int num_heads, int qk_nope_head_dim, cons
 
 /* The two absorb products of MLA decode (attention.py:428-431, 470-472): batches of one-row GEMVs over the per-head bf16
  * halves of kv_b_proj — q_abs[t][h][:] = q_nope[t][h][:] . W_UK[h] ([heads][nope][512]; q addressed by element strides so the
- * q_nope slice of the q_b output needs no copy) and out[t][h][:] = attn_latent[t][h][:] . W_UV[h]^T ([heads][v][512]). */
+ * q_nope slice of the q_b output needs no copy) and out[t][h][:] = attn_latent[t][h][:] . W_UV[h]^T ([heads][v][512]).
+ * qk_nope_head_dim <= 512, kv_lora_rank a multiple of 8.  absorb_q: w_uk 16-byte aligned, q_abs_out 4-byte aligned;
+ * absorb_o: attn_latent and w_uv 16-byte aligned.  Other arguments give KTB200_EINVAL before any device work
+ * (n_tokens = 0 included).  Any n_tokens runs (one launch per 65535 tokens). */
 int ktb200_mla_absorb_q(const void* q_dev, long q_head_stride, long q_token_stride, const void* w_uk_dev, int num_heads, int qk_nope_head_dim,
                         int kv_lora_rank, void* q_abs_out_dev, int n_tokens, void* stream);
 int ktb200_mla_absorb_o(const void* attn_latent_dev, const void* w_uv_dev, int num_heads, int v_head_dim, int kv_lora_rank, void* out_dev,
                         int n_tokens, void* stream);
 
 /* paged latent KV write: StaticCache.update (archive/ktransformers/models/custom_cache.py:147-200)
- * kv_cache[page_idx[t]][page_offset[t]][0:512] = ckv[t], [512:576] = k_pe[t] */
+ * kv_cache[page_idx[t]][page_offset[t]][0:512] = ckv[t], [512:576] = k_pe[t]; kv_cache, ckv and k_pe 16-byte aligned
+ * (KTB200_EINVAL otherwise) */
 int ktb200_mla_kv_write(void* kv_cache, int page_size, const void* ckv, const void* k_pe, const int* page_idx,
                         const int* page_offset, int n_tokens, void* stream);
 

@@ -111,8 +111,16 @@ __global__ void __launch_bounds__(256) mla_prep_kernel(const __nv_bfloat16* q, i
 
 using namespace ktb;
 
+static bool misaligned(const void* p, uintptr_t bytes) { return ((uintptr_t)p & (bytes - 1)) != 0; }
+
 extern "C" int ktb200_add_rmsnorm(void* residual, const void* delta, const void* weight, float eps, void* out, int n_tokens, int hidden, void* stream) {
-    if (!residual || !weight || !out || n_tokens < 0 || hidden <= 0 || hidden % 2 || hidden > 2 * kNormPairs * kNormThreads) { set_error("add_rmsnorm: bad argument (bf16, even hidden <= 8192)"); return KTB200_EINVAL; }
+    if (!residual || !weight || !out || n_tokens < 0) { set_error("add_rmsnorm: null pointer / negative n_tokens"); return KTB200_EINVAL; }
+    if (hidden <= 0 || hidden % 2 || hidden > 2 * kNormPairs * kNormThreads) { set_error("add_rmsnorm: hidden %d must be even and <= 8192 (bf16)", hidden); return KTB200_EINVAL; }
+    // bf16x2 loads and stores
+    if (misaligned(residual, 4)) { set_error("add_rmsnorm: residual must be 4-byte aligned"); return KTB200_EINVAL; }
+    if (misaligned(delta, 4)) { set_error("add_rmsnorm: delta must be 4-byte aligned"); return KTB200_EINVAL; }
+    if (misaligned(weight, 4)) { set_error("add_rmsnorm: weight must be 4-byte aligned"); return KTB200_EINVAL; }
+    if (misaligned(out, 4)) { set_error("add_rmsnorm: out must be 4-byte aligned"); return KTB200_EINVAL; }
     if (n_tokens == 0) return KTB200_OK;
     KTB_CUDA_CHECK(launch_pdl(add_rmsnorm_kernel, dim3(n_tokens), dim3(kNormThreads), 0, (cudaStream_t)stream, (__nv_bfloat16*)residual, (const __nv_bfloat16*)delta,
                               (const __nv_bfloat16*)weight, eps, (__nv_bfloat16*)out, hidden, (long)hidden, (long)hidden, (long)hidden));
@@ -141,6 +149,8 @@ extern "C" int ktb200_mla_prep(const void* q, int num_heads, int qk_nope_head_di
 //   mode 0  q_abs[t][h][c] = sum_d q_nope[t][h][d] * W_UK[h][d][c]     W [heads][D][C] read along c (contiguous)
 //   mode 1  o[t][h][v]     = sum_c lat[t][h][c]   * W_UV[h][v][c]     W [heads][V][C] read along c (contiguous): one warp per (h, v)
 namespace ktb {
+
+constexpr int kMaxGridZ = 65535;   // the tokens of one absorb launch (gridDim.z)
 
 // grid (C / 512, heads, tokens), 256 threads = 4 groups of 64: a group owns a quarter of the d range, a thread 8 columns of
 // the 512-column slab (16-byte loads, 8 rows in flight); the four partial sums meet in shared memory in group order
@@ -213,19 +223,35 @@ __global__ void __launch_bounds__(256) absorb_o_kernel(const __nv_bfloat16* lat,
 
 extern "C" int ktb200_mla_absorb_q(const void* q, long q_head_stride, long q_token_stride, const void* w_uk, int num_heads, int nope_dim, int kv_lora_rank,
                                    void* q_abs_out, int n_tokens, void* stream) {
-    if (!q || !w_uk || !q_abs_out || num_heads <= 0 || nope_dim <= 0 || nope_dim > 512 || kv_lora_rank <= 0 || kv_lora_rank % 8) { set_error("mla_absorb_q: bad argument"); return KTB200_EINVAL; }
+    if (!q || !w_uk || !q_abs_out || num_heads <= 0) { set_error("mla_absorb_q: null pointer / bad num_heads"); return KTB200_EINVAL; }
+    if (nope_dim <= 0 || nope_dim > 512) { set_error("mla_absorb_q: qk_nope_head_dim %d must be in 1..512", nope_dim); return KTB200_EINVAL; }   // qs[512]
+    if (kv_lora_rank <= 0 || kv_lora_rank % 8) { set_error("mla_absorb_q: kv_lora_rank %d must be a positive multiple of 8", kv_lora_rank); return KTB200_EINVAL; }
+    if (misaligned(w_uk, 16)) { set_error("mla_absorb_q: w_uk must be 16-byte aligned"); return KTB200_EINVAL; }          // uint4 weight loads
+    if (misaligned(q_abs_out, 4)) { set_error("mla_absorb_q: q_abs_out must be 4-byte aligned"); return KTB200_EINVAL; }  // bf16x2 stores
     if (n_tokens <= 0) return KTB200_OK;
-    KTB_CUDA_CHECK(launch_pdl(ktb::absorb_q_kernel, dim3((kv_lora_rank + 511) / 512, num_heads, n_tokens), dim3(256), 0, (cudaStream_t)stream, (const __nv_bfloat16*)q,
-                              q_head_stride, q_token_stride, (const __nv_bfloat16*)w_uk, nope_dim, kv_lora_rank, (__nv_bfloat16*)q_abs_out));
-    count_launch();
+    for (int t0 = 0; t0 < n_tokens; t0 += kMaxGridZ) {   // tokens are grid.z: one launch per 65535
+        const int nt = n_tokens - t0 < kMaxGridZ ? n_tokens - t0 : kMaxGridZ;
+        KTB_CUDA_CHECK(launch_pdl(ktb::absorb_q_kernel, dim3((kv_lora_rank + 511) / 512, num_heads, nt), dim3(256), 0, (cudaStream_t)stream,
+                                  (const __nv_bfloat16*)q + t0 * q_token_stride, q_head_stride, q_token_stride, (const __nv_bfloat16*)w_uk, nope_dim,
+                                  kv_lora_rank, (__nv_bfloat16*)q_abs_out + (long)t0 * num_heads * kv_lora_rank));
+        count_launch();
+    }
     return KTB200_OK;
 }
 
 extern "C" int ktb200_mla_absorb_o(const void* attn_latent, const void* w_uv, int num_heads, int v_head_dim, int kv_lora_rank, void* out, int n_tokens, void* stream) {
-    if (!attn_latent || !w_uv || !out || num_heads <= 0 || v_head_dim <= 0 || kv_lora_rank <= 0 || kv_lora_rank % 8) { set_error("mla_absorb_o: bad argument"); return KTB200_EINVAL; }
+    if (!attn_latent || !w_uv || !out || num_heads <= 0 || v_head_dim <= 0) { set_error("mla_absorb_o: null pointer / bad shape"); return KTB200_EINVAL; }
+    if (kv_lora_rank <= 0 || kv_lora_rank % 8) { set_error("mla_absorb_o: kv_lora_rank %d must be a positive multiple of 8", kv_lora_rank); return KTB200_EINVAL; }
+    // uint4 loads of both operands
+    if (misaligned(attn_latent, 16)) { set_error("mla_absorb_o: attn_latent must be 16-byte aligned"); return KTB200_EINVAL; }
+    if (misaligned(w_uv, 16)) { set_error("mla_absorb_o: w_uv must be 16-byte aligned"); return KTB200_EINVAL; }
     if (n_tokens <= 0) return KTB200_OK;
-    KTB_CUDA_CHECK(launch_pdl(ktb::absorb_o_kernel, dim3((v_head_dim + 7) / 8, num_heads, n_tokens), dim3(256), 0, (cudaStream_t)stream, (const __nv_bfloat16*)attn_latent,
-                              (const __nv_bfloat16*)w_uv, v_head_dim, kv_lora_rank, (__nv_bfloat16*)out));
-    count_launch();
+    for (int t0 = 0; t0 < n_tokens; t0 += kMaxGridZ) {
+        const int nt = n_tokens - t0 < kMaxGridZ ? n_tokens - t0 : kMaxGridZ;
+        KTB_CUDA_CHECK(launch_pdl(ktb::absorb_o_kernel, dim3((v_head_dim + 7) / 8, num_heads, nt), dim3(256), 0, (cudaStream_t)stream,
+                                  (const __nv_bfloat16*)attn_latent + (long)t0 * num_heads * kv_lora_rank, (const __nv_bfloat16*)w_uv, v_head_dim,
+                                  kv_lora_rank, (__nv_bfloat16*)out + (long)t0 * num_heads * v_head_dim));
+        count_launch();
+    }
     return KTB200_OK;
 }

@@ -418,6 +418,10 @@ int ktb200_mla_kv_write(void* kv_cache, int page_size, const void* ckv, const vo
                         const int* page_offset, int n_tokens, void* stream) {
     using namespace ktb;
     if (!kv_cache || !ckv || !k_pe || !page_idx || !page_offset) { set_error("mla_kv_write: null pointer"); return KTB200_EINVAL; }
+    // 16-byte row pieces
+    if ((uintptr_t)kv_cache & 15) { set_error("mla_kv_write: kv_cache must be 16-byte aligned"); return KTB200_EINVAL; }
+    if ((uintptr_t)ckv & 15) { set_error("mla_kv_write: ckv must be 16-byte aligned"); return KTB200_EINVAL; }
+    if ((uintptr_t)k_pe & 15) { set_error("mla_kv_write: k_pe must be 16-byte aligned"); return KTB200_EINVAL; }
     if (n_tokens <= 0) return KTB200_OK;
     mla_kv_write_kernel<<<n_tokens, 72, 0, (cudaStream_t)stream>>>((__nv_bfloat16*)kv_cache, page_size, (const __nv_bfloat16*)ckv,
                                                                    (const __nv_bfloat16*)k_pe, page_idx, page_offset);

@@ -210,53 +210,6 @@ def test_kdeepseek_v2_attention_absorbed_paged_decode_matches_plain_attention(he
     assert cache.get_seq_length(0) == steps
 
 
-def test_fused_rmsnorm_and_mla_prep_match_the_module_code():
-    """ktb200_add_rmsnorm / ktb200_mla_prep (csrc/elementwise.cu) against DeepseekV3RMSNorm, apply_rotary_pos_emb and the
-    cache layout they replace (models/modeling_deepseek_v3.py restating the reference's :65-80, :339-373)."""
-    import ctypes as C
-    from ktransformers_b200 import native
-    from ktransformers_b200.models.modeling_deepseek_v3 import DeepseekV3RMSNorm, DeepseekV3RotaryEmbedding, apply_rotary_pos_emb
-    lib = native.lib()
-    s = torch.cuda.current_stream().cuda_stream
-    torch.manual_seed(5)
-    T, Hd = 3, 7168
-    norm = DeepseekV3RMSNorm(Hd).to("cuda", torch.bfloat16)
-    with torch.no_grad():
-        norm.weight.copy_((1 + 0.1 * torch.randn(Hd)).to(torch.bfloat16))
-    x = torch.randn(T, Hd, device="cuda").to(torch.bfloat16)
-    d = torch.randn(T, Hd, device="cuda").to(torch.bfloat16)
-    res, out = x.clone(), torch.zeros_like(x)
-    native.check(lib.ktb200_add_rmsnorm(res.data_ptr(), d.data_ptr(), norm.weight.data_ptr(), 1e-6, out.data_ptr(), T, Hd, s))
-    torch.cuda.synchronize()
-    assert torch.equal(res, x + d)
-    want = norm(x + d)
-    assert (out.float() - want.float()).abs().max() <= 2.0 ** -7 * want.float().abs().max()
-    assert (out == want).float().mean() > 0.99
-    # MLA prep
-    heads, page = 16, 64
-    q = torch.randn(T, heads, 192, device="cuda").to(torch.bfloat16)
-    kva = torch.randn(T, 576, device="cuda").to(torch.bfloat16)
-    kvn = DeepseekV3RMSNorm(512).to("cuda", torch.bfloat16)
-    with torch.no_grad():
-        kvn.weight.copy_((1 + 0.1 * torch.randn(512)).to(torch.bfloat16))
-    rot = DeepseekV3RotaryEmbedding(64).to("cuda")
-    pos = torch.tensor([[5, 70, 131]], device="cuda")
-    cos, sin = rot(torch.zeros(1, device="cuda", dtype=torch.float32), pos)            # fp32 tables [1, T, 64]
-    cache = torch.zeros(4, page, 576, dtype=torch.bfloat16, device="cuda")
-    pidx = (pos[0] // page).to(torch.int32).contiguous(); poff = (pos[0] % page).to(torch.int32).contiguous()
-    q_pe_out = torch.zeros(T, heads, 64, dtype=torch.bfloat16, device="cuda")
-    native.check(lib.ktb200_mla_prep(q.data_ptr(), heads, 128, kva.data_ptr(), kvn.weight.data_ptr(), 1e-6, cos[0].contiguous().data_ptr(), sin[0].contiguous().data_ptr(),
-                                     cache.data_ptr(), page, pidx.data_ptr(), poff.data_ptr(), q_pe_out.data_ptr(), T, s))
-    torch.cuda.synchronize()
-    qpe_w, kpe_w = apply_rotary_pos_emb(q[None, :, :, 128:], kva[None, :, None, 512:], cos.to(torch.bfloat16), sin.to(torch.bfloat16), unsqueeze_dim=2)
-    tol = lambda w: 2.0 ** -6 * w.float().abs().max()
-    assert (q_pe_out.float() - qpe_w[0].float()).abs().max() <= tol(qpe_w)
-    rows = cache[pidx.long(), poff.long()]
-    assert (rows[:, 512:].float() - kpe_w[0, :, 0].float()).abs().max() <= tol(kpe_w)
-    ckv_w = kvn(kva[:, :512])
-    assert (rows[:, :512].float() - ckv_w.float()).abs().max() <= tol(ckv_w)
-
-
 def test_serve_rule_file_v2_classes_carry_bsz_tensor(tmp_path):
     """balance-serve flavour (experts.py:1172-1350): KDeepseekV3MoEV2 / KTransformersExpertsV2 with a device-side batch size; rows
     below bsz equal the V1 forward bit for bit, through the block kernel (3 tokens), the per-pair kernels (12) and the grouped path (64)."""

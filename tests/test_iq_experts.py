@@ -255,25 +255,63 @@ def test_moe_forward_type_mixes(oracle, mix, qlen):
     m.close()
 
 
-def _kernels_of(fn):
-    """names of the CUDA kernels `fn` launches"""
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    return [e.key for e in prof.key_averages() if "kernel" in e.key]
-
-
 # (H, I): which kernels a same-type all-IQ handle takes
 PATHS = {(1024, 512): ("rows_bulk_iq_kernel", "reduce_bulk_kernel<ktb::BulkIQ"),     # both on the bulk-copy ring
+         (2048, 1024): ("rows_bulk_iq_kernel", "reduce_bulk_kernel<ktb::BulkIQ"),    # the same with 8 / 4 blocks per row
          (512, 256): ("rows_kernel<ktb::FmtGenK", "reduce_kernel<ktb::FmtGenK")}     # 2 blocks per row, 1 per down row
+KERNEL_MIXES = ["iq1x3", "iq2x3"]
+
+# every (mix, shape) of test_kernels_that_ran in ONE torch.profiler session, in an interpreter of its own: after other
+# profiler sessions in the same process a session can come back without some of its kernels.  Kernels are attributed to
+# the call that launched them by launch order.
+_CENSUS = r"""
+import json, sys
+import numpy as np, torch
+sys.path[:0] = sys.argv[1:]
+from torch.profiler import ProfilerActivity, profile
+from ktransformers_b200 import native
+from test_iq_experts import KERNEL_MIXES, PATHS, TYPE_MIXES, _Experts, _ids, _x
+cases = []
+for mix in KERNEL_MIXES:
+    for H, I in sorted(PATHS):
+        ex = _Experts(8, H, I, *TYPE_MIXES[mix], 60)
+        rng = np.random.default_rng(61)
+        cases.append((f"{mix} {H} {I}", ex, ex.moe(4, 0), _ids(3, 8, 4, rng), rng.random((3, 4)).astype(np.float32), _x(3, H, 62, 0)[0]))
+torch.cuda.synchronize()
+counts = []
+with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    for _, _, m, ids, w, x in cases:
+        n0 = native.launch_count()
+        m.forward(ids, w, x)
+        torch.cuda.synchronize()
+        counts.append(native.launch_count() - n0)
+names = [e.name for e in sorted((e for e in prof.events() if "ktb::" in e.name), key=lambda e: e.time_range.start)]
+assert len(names) == sum(counts), f"{len(names)} library kernels recorded, {sum(counts)} launched: {names}"
+res, i = {}, 0
+for (key, *_), n in zip(cases, counts):
+    res[key] = (n, names[i:i + n])
+    i += n
+print("CENSUS " + json.dumps(res))
+"""
+
+
+@pytest.fixture(scope="module")
+def kernel_census():
+    import json
+    import subprocess
+    import sys
+    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", _CENSUS, os.path.join(ROOT, "tests"), ROOT]
+    r = subprocess.run(cmd, capture_output=True, text=True, timeout=600, cwd=ROOT)
+    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
+    return json.loads(next(l for l in r.stdout.splitlines() if l.startswith("CENSUS "))[7:])
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", sorted(PATHS))
-@pytest.mark.parametrize("mix", ["iq1x3", "iq2x3"])
-def test_kernels_that_ran(oracle, shape, mix):
-    """the bulk-copy kernels take shapes whose 2-row units / 4-row items are 16-byte aligned; other shapes the generic ones"""
+@pytest.mark.parametrize("mix", KERNEL_MIXES)
+def test_kernels_that_ran(oracle, kernel_census, shape, mix):
+    """the bulk-copy kernels take shapes whose 2-row units / 4-row items are 16-byte aligned; other shapes the generic ones
+    (kernel names from the census above; the launch count and the result checked here as well)"""
     H, I = shape
     E, k, T = 8, 4, 3
     ex = _Experts(E, H, I, *TYPE_MIXES[mix], 60)
@@ -281,16 +319,18 @@ def test_kernels_that_ran(oracle, shape, mix):
     rng = np.random.default_rng(61)
     ids, w = _ids(T, E, k, rng), rng.random((T, k)).astype(np.float32)
     x, xf = _x(T, H, 62, F32)
+    launched, names = kernel_census[f"{mix} {H} {I}"]
+    assert launched == 2
     n0 = native.launch_count()
-    names = _kernels_of(lambda: m.forward(ids, w, x))
+    got = m.forward(ids, w, x)
     assert native.launch_count() - n0 == 2
     fmt = "BulkIQ1S" if mix == "iq1x3" else "BulkIQ2XXS"
     gu, dn = PATHS[shape]
     assert any(gu in n and (fmt in n or "FmtGenK" in n) for n in names), names
     assert any(dn in n for n in names), names
-    if shape == (1024, 512):
+    if gu == "rows_bulk_iq_kernel":
         assert any(fmt in n for n in names) and not any("FmtGenK" in n for n in names), names
-    _check(m.forward(ids, w, x), oq.moe_forward(oracle, xf, ids, w, ex.expert, E), F32)
+    _check(got, oq.moe_forward(oracle, xf, ids, w, ex.expert, E), F32)
     m.close()
 
 
