@@ -13,7 +13,7 @@
 //       out[t][h] = sum_j w[t][j] * ( W[e_tj][h,:] . aq_tj )   — aq quantised in the prologue
 //
 // grid = (gx, T): blockIdx.y is the token, blockIdx.x splits that token's work into contiguous,
-// equally sized ranges (gx is chosen so gx*T ~ MINB CTAs per SM).
+// equally sized ranges (gx is chosen so gx*T ~ kGemvCtasPerSm CTAs per SM).
 //
 // A warp walks a row in "steps" (32 lanes = Fmt::kBlocksPerStep super-blocks).  Steps are consumed in
 // batches of NB: all global loads of a batch (RW rows x NM matrices x NB steps) are issued before the
@@ -25,6 +25,7 @@
 namespace ktb {
 
 constexpr int kGemvThreads = 256;
+constexpr int kGemvCtasPerSm = 2;   // rows_kernel / reduce_kernel: launch bounds and grid size
 
 struct RowsParams {
     const void* w0;         // [E][rows][ncols] blocks
@@ -111,8 +112,8 @@ __device__ __forceinline__ float warp_reduce4(float v0, float v1, float v2, floa
     return c;
 }
 
-template <class Fmt, bool PAIR, int RW, int NB, int MINB>
-__global__ void __launch_bounds__(kGemvThreads, MINB) rows_kernel(const RowsParams p) {
+template <class Fmt, bool PAIR, int RW, int NB>
+__global__ void __launch_bounds__(kGemvThreads, kGemvCtasPerSm) rows_kernel(const RowsParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int t = blockIdx.y;
     if (p.bsz && t >= *p.bsz) return;
@@ -216,8 +217,8 @@ struct ReduceParams {
 
 // Work item of a warp = (slot j, 4 consecutive output rows): the 4 rows share slot j's int8 activations,
 // one ids lookup and one 6-shuffle reduction.
-template <class Fmt, int NB, int MINB>
-__global__ void __launch_bounds__(kGemvThreads, MINB) reduce_kernel(const ReduceParams p) {
+template <class Fmt, int NB>
+__global__ void __launch_bounds__(kGemvThreads, kGemvCtasPerSm) reduce_kernel(const ReduceParams p) {
     constexpr int RW = 4;
     extern __shared__ __align__(16) uint8_t smem[];
     const int t = blockIdx.y;

@@ -124,7 +124,7 @@ namespace ktb {
 // in the SoA layout the item is four contiguous pieces (ql 4x128nb | qh 4x64nb | scales 4x16nb | d 4x2nb),
 // streamed into a warp-private 2-slot ring with cp.async while the previous item is reduced from shared memory.
 // CTA row ranges are multiples of 4 rows; requires rows % 4 == 0 and nb even.
-template <int WARPS, int SLOTS>
+template <int WARPS>
 __global__ void __launch_bounds__(WARPS * 32, 1) reduce_pipe_q6k8_kernel(const ReduceParams p, int slot_bytes) {
     using Fmt = FmtQ6K8;
     constexpr int RW = 4;
@@ -146,7 +146,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) reduce_pipe_q6k8_kernel(const R
     const int nquads = q1 - q0;
     size_t off = (size_t)ns * p.ncols + (size_t)ns * nb * 4 + (size_t)ns * (p.ncols / 16) * 2 + (size_t)(nrows > 0 ? nrows : 1) * ns * 4;
     off = (off + 15) & ~(size_t)15;
-    uint8_t* ring = smem + off + (size_t)warp * SLOTS * slot_bytes;
+    uint8_t* ring = smem + off + (size_t)warp * 2 * slot_bytes;
     const uint32_t ring_u32 = (uint32_t)__cvta_generic_to_shared(ring);
 
     unsigned skip = 0;
@@ -192,14 +192,9 @@ __global__ void __launch_bounds__(WARPS * 32, 1) reduce_pipe_q6k8_kernel(const R
     const Fmt::Lane L = Fmt::lane(lane);
     const int nsteps = (nb + Fmt::kBlocksPerStep - 1) / Fmt::kBlocksPerStep;
     for (int it = 0; item < total; item += WARPS, it++) {
-        const int slot = (SLOTS == 2) ? (it & 1) : 0;
-        bool next_ok = false;
-        if (SLOTS == 2) {
-            next_ok = issue(item + WARPS, slot ^ 1);
-            cp_async_wait_group<1>();
-        } else {
-            cp_async_wait_group<0>();
-        }
+        const int slot = it & 1;
+        const bool next_ok = issue(item + WARPS, slot ^ 1);
+        cp_async_wait_group<1>();
         __syncwarp();
         const int j = item / nquads, quad = item - j * nquads;
         float res = 0.f;
@@ -228,8 +223,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) reduce_pipe_q6k8_kernel(const R
         }
         if ((lane & 7) == 0) partial[(quad * RW + (lane >> 3)) * ns + j] = res;
         __syncwarp();
-        if (SLOTS == 2) cur_ok = next_ok;
-        else cur_ok = issue(item + WARPS, 0);
+        cur_ok = next_ok;
     }
     cp_async_wait_group<0>();
     __syncthreads();

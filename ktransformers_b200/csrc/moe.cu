@@ -4,6 +4,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <new>
+#include <type_traits>
 
 #define KTB_IQ_CODEBOOKS
 #include "gemv_bulk.cuh"
@@ -133,46 +134,60 @@ static int set_smem_attr(K kernel, size_t smem) {
     return KTB200_OK;
 }
 
-// Tuning knobs (read once): KTB200_MINB = CTAs per SM the main kernels are compiled/launched for (2 or 3),
-// KTB200_NB = steps per load batch for the long-row gate/up kernel (2 or 4).
-static int env_int(const char* name, int dflt) {
-    const char* v = getenv(name);
-    return v ? atoi(v) : dflt;
-}
-static int cfg_minb() { static int v = env_int("KTB200_MINB", 2); return v == 3 ? 3 : 2; }
-static int cfg_pipe() { static int v = env_int("KTB200_PIPE", 2); return v; }   // 0 off, 1 chunk-per-lane, 2 block-per-lane
-static int cfg_nb() { static int v = env_int("KTB200_NB", 2); return v == 4 ? 4 : 2; }
-// bulk-copy generation (gemv_bulk.cuh): KTB200_BULK=0 disables it, *_SLOTS_* = ring depth, KTB200_BULK_WARPS caps the CTA
-static int cfg_bulk() { static int v = env_int("KTB200_BULK", 1); return v; }
-static int cfg_bulk_slots_up() { static int v = env_int("KTB200_BULK_SLOTS_UP", 3); return v == 2 ? 2 : (v == 4 ? 4 : 3); }
-static int cfg_bulk_slots_down() { static int v = env_int("KTB200_BULK_SLOTS_DOWN", 2); return v == 3 ? 3 : 2; }
-static int cfg_bulk_warps() { static int v = env_int("KTB200_BULK_WARPS", kBulkMaxWarps); return v < 1 ? 1 : (v > kBulkMaxWarps ? kBulkMaxWarps : v); }
 constexpr size_t kSmemCap = 232448 - 512;   // 227 KB opt-in limit minus the kernels' static shared variables
 
+// one CTA per SM, at most one per unit of work
+static int grid_x(long units, int device) {
+    int gx = num_sms(device);
+    if (gx > units) gx = (int)units;
+    return gx < 1 ? 1 : gx;
+}
+
+// Shared-memory plan of a bulk-copy ring kernel (gemv_bulk.cuh, dense_bulk.cuh, iq.cuh, rawint4.cuh): a head of `chunk`
+// staged units (tokens for gate/up, (token, slot) pairs for down) of `unit_bytes` each, padded to 16 bytes, then W warps of
+// `slots` ring slots of `slot_bytes` with an 8-byte mbarrier per slot, within the opt-in limit less the format's static
+// tables (`table_bytes`).  The chunk is the largest in [lo, hi] whose head leaves room for `room_warps` warps plus `spare`
+// bytes (lo when none does); W is as many warps as fit next to it, at most max_warps.  W = 0: fewer than min_warps fit.
+struct RingPlan { int chunk, W; size_t smem; };
+static RingPlan plan_ring(size_t unit_bytes, int lo, int hi, int room_warps, size_t spare, size_t slot_bytes, int slots,
+                          int min_warps, int max_warps, int table_bytes) {
+    const size_t cap = kSmemCap - table_bytes, ring = (size_t)slots * (slot_bytes + 8);
+    auto head = [&](int chunk) { return ((size_t)chunk * unit_bytes + 15) & ~(size_t)15; };
+    RingPlan pl{hi, 0, 0};
+    while (pl.chunk > lo && head(pl.chunk) + 16 + spare + room_warps * ring > cap) pl.chunk--;
+    const size_t h = head(pl.chunk);
+    if (h + 16 >= cap) return pl;
+    int W = (int)((cap - h - 16) / ring);
+    if (W > max_warps) W = max_warps;
+    if (W < min_warps) return pl;
+    pl.W = W;
+    pl.smem = h + (((size_t)W * slots * 8 + 15) & ~(size_t)15) + (size_t)W * slots * slot_bytes;
+    return pl;
+}
+
+constexpr size_t kGateUpSpare = 48;   // plan_ring `spare` of the gate/up kernels' token chunks
+
 template <class Fmt, bool PAIR>
-static int launch_rows_fmt(const RowsParams& p, int T, int device, cudaStream_t stream, bool tunable) {
+static int launch_rows_fmt(const RowsParams& p, int T, int device, cudaStream_t stream) {
     const int nblk = p.ncols / QK_K;
     const int nsteps = (nblk + Fmt::kBlocksPerStep - 1) / Fmt::kBlocksPerStep;
     const size_t smem = (size_t)p.ncols + (size_t)nblk * 4 + (size_t)p.ncols / 8;
-    const int minb = tunable ? cfg_minb() : 2;
-    int gx = (minb * num_sms(device) + T - 1) / T;
+    int gx = (kGemvCtasPerSm * num_sms(device) + T - 1) / T;
     const long total = (long)(p.slots + (p.x0 ? 1 : 0)) * p.rows;
     if (total >= (1L << 31) / 2) { set_error("rows kernel: slots x rows too large"); return KTB200_EINVAL; }
     if (gx > total) gx = (int)total;
     if (gx < 1) gx = 1;
     dim3 grid(gx, T);
-#define KTB_ROWS(RW, NB, MINB)                                                             \
+    constexpr int kLongRowNB = std::is_same<Fmt, FmtQ4K>::value ? 2 : 4;   // steps per load batch on rows of >= 4 steps
+#define KTB_ROWS(RW, NB)                                                                   \
     do {                                                                                   \
-        int rc = set_smem_attr(rows_kernel<Fmt, PAIR, RW, NB, MINB>, smem);                \
+        int rc = set_smem_attr(rows_kernel<Fmt, PAIR, RW, NB>, smem);                      \
         if (rc) return rc;                                                                 \
-        rows_kernel<Fmt, PAIR, RW, NB, MINB><<<grid, kGemvThreads, smem, stream>>>(p);     \
+        rows_kernel<Fmt, PAIR, RW, NB><<<grid, kGemvThreads, smem, stream>>>(p);           \
     } while (0)
-    if (nsteps >= 4) {
-        if (tunable && minb == 3) KTB_ROWS(1, 2, 3);
-        else if (tunable && cfg_nb() == 2) KTB_ROWS(1, 2, 2);
-        else KTB_ROWS(1, 4, 2);
-    } else if (nsteps >= 2) KTB_ROWS(2, 2, 2);
-    else KTB_ROWS(4, 1, 2);
+    if (nsteps >= 4) KTB_ROWS(1, kLongRowNB);
+    else if (nsteps >= 2) KTB_ROWS(2, 2);
+    else KTB_ROWS(4, 1);
 #undef KTB_ROWS
     KTB_LAUNCH_CHECK();
     return KTB200_OK;
@@ -182,7 +197,6 @@ static int launch_rows_fmt(const RowsParams& p, int T, int device, cudaStream_t 
 // Returns 1 when the shape does not suit it (caller falls back to rows_kernel).
 template <class Fmt, bool PAIR>
 static int launch_rows_pipe(const RowsParams& p, int T, int device, cudaStream_t stream) {
-    if (!cfg_pipe()) return 1;
     const int nblk = p.ncols / QK_K;
     const int row_bytes = nblk * Fmt::kBlockBytes;
     const int slot = row_bytes * (PAIR ? 2 : 1);
@@ -212,42 +226,26 @@ static int launch_rows_pipe(const RowsParams& p, int T, int device, cudaStream_t
 // Q4_K rows through the bulk-copy ring (rows_bulk_q4k_kernel).  Returns 1 when the shape does not suit it.
 template <bool PAIR>
 static int launch_rows_bulk_q4k(const RowsParams& p, int T, int device, cudaStream_t stream) {
-    if (!cfg_bulk()) return 1;
+    constexpr int S = 3;
     const int nblk = p.ncols / QK_K;
-    const int row_bytes = nblk * SZ_Q4_K;
     if (nblk < 16) return 1;                             // needs >= 16 blocks per row to keep most lanes busy
     const int nslots = p.slots + (p.x0 ? 1 : 0);
     const long total = (long)nslots * p.rows;
     if (total >= (1L << 26) || nslots > 200) return 1;
     const int act_tok = (nblk * kActBlkStride + nblk * 16 + nblk * 4 + 15) & ~15;
-    const int S = cfg_bulk_slots_up();
-    // tokens per chunk: as many (<= 8) as fit next to 12 rings; then as many warps as fit
-    int tc = T < 8 ? T : 8;
-    while (tc > 1 && (size_t)tc * (act_tok + nslots * 4) + 64 + (size_t)12 * S * (row_bytes + 8) > kSmemCap) tc--;
-    const size_t head = (((size_t)tc * act_tok + (size_t)tc * nslots * 4 + 15) & ~(size_t)15);
-    if (head + 64 >= kSmemCap) return 1;
-    int W = (int)((kSmemCap - head - 16) / ((size_t)S * (row_bytes + 8)));
-    if (W > cfg_bulk_warps()) W = cfg_bulk_warps();
-    if (W < 4) return 1;
-    const size_t smem = head + (((size_t)W * S * 8 + 15) & ~(size_t)15) + (size_t)W * S * row_bytes;
-    int gx = num_sms(device);            // one CTA per SM walks all T tokens
-    if (gx > total) gx = (int)total;
-    if (gx < 1) gx = 1;
-#define KTB_BULK_ROWS(SL)                                                                                              \
-    do {                                                                                                               \
-        KTB_CUDA_CHECK(cudaFuncSetAttribute(rows_bulk_q4k_kernel<PAIR, SL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        rows_bulk_q4k_kernel<PAIR, SL><<<gx, W * 32, smem, stream>>>(p, act_tok, tc);                                  \
-    } while (0)
-    if (S == 2) KTB_BULK_ROWS(2); else if (S == 4) KTB_BULK_ROWS(4); else KTB_BULK_ROWS(3);
-#undef KTB_BULK_ROWS
+    // tokens per chunk: as many (<= 8) as leave room for 12 warps; then 4 to kBulkMaxWarps warps
+    const RingPlan pl = plan_ring(act_tok + nslots * 4, 1, T < 8 ? T : 8, 12, kGateUpSpare, (size_t)nblk * SZ_Q4_K, S, 4,
+                                  kBulkMaxWarps, 0);
+    if (!pl.W) return 1;
+    KTB_CUDA_CHECK(cudaFuncSetAttribute(rows_bulk_q4k_kernel<PAIR, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
+    rows_bulk_q4k_kernel<PAIR, S><<<grid_x(total, device), pl.W * 32, pl.smem, stream>>>(p, act_tok, pl.chunk);
     KTB_LAUNCH_CHECK();
     return KTB200_OK;
 }
 
 // Dense Q4_K linear on the segment ring (dense_bulk.cuh).  Returns 1 when the shape does not suit it.
 static int launch_dense_q4k(const RowsParams& p, int T, int device, cudaStream_t stream) {
-    static const int on = env_int("KTB200_DENSE_BULK", 1);
-    if (!on || p.ids || p.slots != 1 || p.x0 || !p.out_hidden || p.out_f32 || T > kDenseMaxTokens) return 1;
+    if (p.ids || p.slots != 1 || p.x0 || !p.out_hidden || p.out_f32 || T > kDenseMaxTokens) return 1;
     const int nblk = p.ncols / QK_K;
     DenseParams d{};
     d.w = reinterpret_cast<const uint8_t*>(p.w0); d.x = p.x; d.out = p.out_hidden; d.bias = p.bias; d.bsz = p.bsz;
@@ -257,22 +255,15 @@ static int launch_dense_q4k(const RowsParams& p, int T, int device, cudaStream_t
     else { d.R = 1; d.G = (nblk + 31) / 32; if (nblk % d.G) return 1; d.segb = nblk / d.G; }
     d.act_tok = (nblk * kActBlkStride + nblk * 16 + nblk * 4 + 15) & ~15;
     constexpr int SL = 4;
-    const size_t head = (((size_t)T * d.act_tok + 15) & ~(size_t)15);
-    const size_t seg = (size_t)d.segb * SZ_Q4_K;
-    if (head + 64 >= kSmemCap) return 1;
-    int W = (int)((kSmemCap - head - 16) / (SL * (seg + 8)));
-    if (W > kDenseWarps) W = kDenseWarps;
-    if (W < 4) return 1;
-    const size_t smem = head + (((size_t)W * SL * 8 + 15) & ~(size_t)15) + (size_t)W * SL * seg;
-    const int nunits = (p.rows + d.R - 1) / d.R;
-    int gx = num_sms(device);
-    if (gx > nunits) gx = nunits;
+    const RingPlan pl = plan_ring(d.act_tok, T, T, 0, 0, (size_t)d.segb * SZ_Q4_K, SL, 4, kDenseWarps, 0);
+    if (!pl.W) return 1;
     static size_t limit[64] = {};
-    if (limit[device & 63] < smem) {
-        KTB_CUDA_CHECK(cudaFuncSetAttribute(dense_q4k_kernel<SL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        limit[device & 63] = smem;
+    if (limit[device & 63] < pl.smem) {
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(dense_q4k_kernel<SL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
+        limit[device & 63] = pl.smem;
     }
-    KTB_CUDA_CHECK(launch_pdl(dense_q4k_kernel<SL>, dim3(gx), dim3(W * 32), smem, stream, d));
+    KTB_CUDA_CHECK(launch_pdl(dense_q4k_kernel<SL>, dim3(grid_x((p.rows + d.R - 1) / d.R, device)), dim3(pl.W * 32), pl.smem,
+                              stream, d));
     count_launch();
     return KTB200_OK;
 }
@@ -287,19 +278,11 @@ static int launch_rows_i4(const RowsParams& p, int T, int device, cudaStream_t s
     const size_t act_tok = (size_t)nblk * kI4ActStride;
     const long total = (long)p.slots * p.rows;
     if (p.x0 || p.shared_token >= 0 || p.slots > 200 || total >= (1L << 26)) { set_error("RAWINT4 gate/up: unsupported launch"); return KTB200_EINVAL; }
-    auto head = [&](int tc) { return ((size_t)tc * act_tok + (size_t)tc * p.slots * 4 + 15) & ~(size_t)15; };
-    int tc = T < kI4MaxChunkTokens ? T : kI4MaxChunkTokens;
-    while (tc > 1 && head(tc) + 64 + (size_t)8 * S * (slot + 8) > kSmemCap) tc--;
-    if (head(tc) + 64 >= kSmemCap) { set_error("RAWINT4 gate/up: hidden_size %d does not fit shared memory", p.ncols); return KTB200_EINVAL; }
-    int W = (int)((kSmemCap - head(tc) - 16) / (S * (slot + 8)));
-    if (W > cfg_bulk_warps()) W = cfg_bulk_warps();
-    if (W < 1) { set_error("RAWINT4 gate/up: hidden_size %d does not fit shared memory", p.ncols); return KTB200_EINVAL; }
-    const size_t smem = head(tc) + (((size_t)W * S * 8 + 15) & ~(size_t)15) + (size_t)W * S * slot;
-    int gx = num_sms(device);
-    if (gx > total) gx = (int)total;
-    if (gx < 1) gx = 1;
-    KTB_CUDA_CHECK(cudaFuncSetAttribute(rows_bulk_i4_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    rows_bulk_i4_kernel<S><<<gx, W * 32, smem, stream>>>(p, tc);
+    const RingPlan pl = plan_ring(act_tok + p.slots * 4, 1, T < kI4MaxChunkTokens ? T : kI4MaxChunkTokens, 8, kGateUpSpare,
+                                  slot, S, 1, kBulkMaxWarps, 0);
+    if (!pl.W) { set_error("RAWINT4 gate/up: hidden_size %d does not fit shared memory", p.ncols); return KTB200_EINVAL; }
+    KTB_CUDA_CHECK(cudaFuncSetAttribute(rows_bulk_i4_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
+    rows_bulk_i4_kernel<S><<<grid_x(total, device), pl.W * 32, pl.smem, stream>>>(p, pl.chunk);
     KTB_LAUNCH_CHECK();
     return KTB200_OK;
 }
@@ -310,28 +293,16 @@ static int launch_rows_i4(const RowsParams& p, int T, int device, cudaStream_t s
 template <class Fmt>
 static int launch_rows_bulk_iq(const RowsParams& p, int T, int device, cudaStream_t stream) {
     constexpr int S = 2;
-    if (!cfg_bulk()) return 1;
     const int nblk = p.ncols / QK_K;
     if (p.type0 != Fmt::kType || p.type1 != Fmt::kType || p.x0 || !p.ids || nblk % 4 || p.rows % 2 || p.slots > 200) return 1;
     const long total = (long)p.slots * (p.rows / 2);
     if (total >= (1L << 26)) return 1;
-    const size_t slot = (size_t)4 * nblk * Fmt::kBlockBytes;
     const int act_tok = (nblk * kActBlkStride + nblk * 16 + nblk * 4 + 15) & ~15;
-    const size_t cap = kSmemCap - Fmt::kTableBytes;
-    auto head = [&](int tc) { return ((size_t)tc * act_tok + (size_t)tc * p.slots * 4 + 15) & ~(size_t)15; };
-    int tc = T < 8 ? T : 8;
-    while (tc > 1 && head(tc) + 64 + (size_t)8 * S * (slot + 8) > cap) tc--;
-    if (head(tc) + 64 >= cap) return 1;
-    int W = (int)((cap - head(tc) - 16) / (S * (slot + 8)));
-    if (W > kIqMaxWarps) W = kIqMaxWarps;
-    if (W > cfg_bulk_warps()) W = cfg_bulk_warps();
-    if (W < 4) return 1;
-    const size_t smem = head(tc) + (((size_t)W * S * 8 + 15) & ~(size_t)15) + (size_t)W * S * slot;
-    int gx = num_sms(device);
-    if (gx > total) gx = (int)total;
-    if (gx < 1) gx = 1;
-    KTB_CUDA_CHECK(cudaFuncSetAttribute(rows_bulk_iq_kernel<Fmt, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    rows_bulk_iq_kernel<Fmt, S><<<gx, W * 32, smem, stream>>>(p, act_tok, tc);
+    const RingPlan pl = plan_ring(act_tok + p.slots * 4, 1, T < 8 ? T : 8, 8, kGateUpSpare, (size_t)4 * nblk * Fmt::kBlockBytes,
+                                  S, 4, kIqMaxWarps, Fmt::kTableBytes);
+    if (!pl.W) return 1;
+    KTB_CUDA_CHECK(cudaFuncSetAttribute(rows_bulk_iq_kernel<Fmt, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
+    rows_bulk_iq_kernel<Fmt, S><<<grid_x(total, device), pl.W * 32, pl.smem, stream>>>(p, act_tok, pl.chunk);
     KTB_LAUNCH_CHECK();
     return KTB200_OK;
 }
@@ -358,26 +329,33 @@ static int launch_rows(FmtId f, const RowsParams& p_in, int T, int device, cudaS
         if (rcb != 1) return rcb;
     }
     if (p.x0 && p.shared_token >= 0) { set_error("per-token shared slot: only the bulk-copy kernels implement it"); return KTB200_EINVAL; }
-    if (f == FMT_Q4K || f == FMT_Q5K) {
-        const int rc = (f == FMT_Q4K) ? launch_rows_pipe<FmtQ4K32, PAIR>(p, T, device, stream) : launch_rows_pipe<FmtQ5K, PAIR>(p, T, device, stream);
+    if (f == FMT_Q5K) {
+        const int rc = launch_rows_pipe<FmtQ5K, PAIR>(p, T, device, stream);
         if (rc != 1) return rc;
     }
+    // Q4_K rows without a pair do not reach the pipe kernel: the bulk kernel above takes every such row of >= 16 blocks
+    // that fits the pipe's 8 warps x 2 slots, and shorter rows are under its 4096 bytes.
+    if constexpr (PAIR) {
+        if (f == FMT_Q4K) {
+            const int rc = launch_rows_pipe<FmtQ4K32, PAIR>(p, T, device, stream);
+            if (rc != 1) return rc;
+        }
+    }
     switch (f) {
-        case FMT_Q4K: return launch_rows_fmt<FmtQ4K, PAIR>(p, T, device, stream, true);
-        case FMT_Q5K: return launch_rows_fmt<FmtQ5K, PAIR>(p, T, device, stream, false);
-        case FMT_Q6K8: return launch_rows_fmt<FmtQ6K8, PAIR>(p, T, device, stream, false);
-        case FMT_GENK: return launch_rows_fmt<FmtGenK, PAIR>(p, T, device, stream, false);
+        case FMT_Q4K: return launch_rows_fmt<FmtQ4K, PAIR>(p, T, device, stream);
+        case FMT_Q5K: return launch_rows_fmt<FmtQ5K, PAIR>(p, T, device, stream);
+        case FMT_Q6K8: return launch_rows_fmt<FmtQ6K8, PAIR>(p, T, device, stream);
+        case FMT_GENK: return launch_rows_fmt<FmtGenK, PAIR>(p, T, device, stream);
         default: set_error("unsupported weight type"); return KTB200_EINVAL;
     }
 }
 
 template <class Fmt, int NBMAX>
-static int launch_reduce_fmt(const ReduceParams& p, int T, int device, cudaStream_t stream, bool tunable) {
+static int launch_reduce_fmt(const ReduceParams& p, int T, int device, cudaStream_t stream) {
     const int nblk = p.ncols / QK_K;
     const int nsteps = (nblk + Fmt::kBlocksPerStep - 1) / Fmt::kBlocksPerStep;
-    const int minb = tunable ? cfg_minb() : 2;
     const int ns = p.slots + (p.xw ? 1 : 0);
-    int gx = (minb * num_sms(device) + T - 1) / T;
+    int gx = (kGemvCtasPerSm * num_sms(device) + T - 1) / T;
     if (gx > p.rows) gx = p.rows;
     if (gx < 1) gx = 1;
     const int nrows_max = (p.rows + gx - 1) / gx + 1;
@@ -388,25 +366,21 @@ static int launch_reduce_fmt(const ReduceParams& p, int T, int device, cudaStrea
         return KTB200_EINVAL;
     }
     dim3 grid(gx, T);
-#define KTB_RED(NB, MINB)                                                                  \
+#define KTB_RED(NB)                                                                        \
     do {                                                                                   \
-        int rc = set_smem_attr(reduce_kernel<Fmt, NB, MINB>, smem);                        \
+        int rc = set_smem_attr(reduce_kernel<Fmt, NB>, smem);                              \
         if (rc) return rc;                                                                 \
-        reduce_kernel<Fmt, NB, MINB><<<grid, kGemvThreads, smem, stream>>>(p);             \
+        reduce_kernel<Fmt, NB><<<grid, kGemvThreads, smem, stream>>>(p);                   \
     } while (0)
-    if (NBMAX >= 2 && nsteps >= 2) {
-        if (minb == 3) KTB_RED((NBMAX >= 2 ? 2 : 1), 3); else KTB_RED((NBMAX >= 2 ? 2 : 1), 2);
-    } else {
-        if (minb == 3) KTB_RED(1, 3); else KTB_RED(1, 2);
-    }
+    if (nsteps >= 2) KTB_RED(NBMAX);
+    else KTB_RED(1);
 #undef KTB_RED
     KTB_LAUNCH_CHECK();
     return KTB200_OK;
 }
 
-// cp.async-pipelined Q6_K (SoA) reduce: returns 1 when the shape does not suit it
+// cp.async-pipelined Q6_K (SoA) reduce, 12 warps x 2 ring slots: returns 1 when the shape does not suit it
 static int launch_reduce_pipe_q6k8(const ReduceParams& p, int T, int device, cudaStream_t stream) {
-    if (!cfg_pipe()) return 1;
     const int nb = p.ncols / QK_K;
     if (p.rows % 4 || nb % 2) return 1;
     const int ns = p.slots + (p.xw ? 1 : 0);
@@ -417,131 +391,74 @@ static int launch_reduce_pipe_q6k8(const ReduceParams& p, int T, int device, cud
     if (gx > quads) gx = quads;
     if (gx < 1) gx = 1;
     const int nrows_max = ((quads + gx - 1) / gx + 1) * 4;
-    size_t base = (size_t)ns * p.ncols + (size_t)ns * nb * 4 + (size_t)ns * (p.ncols / 16) * 2 + (size_t)nrows_max * ns * 4 + 16;
-    static const int want_slots = env_int("KTB200_PIPE_SLOTS", 2);
-    dim3 grid(gx, T);
-    if (want_slots != 2 && base + (size_t)24 * slot <= 220 * 1024) {
-        const size_t smem = base + (size_t)24 * slot;
-        KTB_CUDA_CHECK(cudaFuncSetAttribute(reduce_pipe_q6k8_kernel<24, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        reduce_pipe_q6k8_kernel<24, 1><<<grid, 24 * 32, smem, stream>>>(p, slot);
-    } else if (base + (size_t)12 * 2 * slot <= 220 * 1024) {
-        const size_t smem = base + (size_t)12 * 2 * slot;
-        KTB_CUDA_CHECK(cudaFuncSetAttribute(reduce_pipe_q6k8_kernel<12, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        reduce_pipe_q6k8_kernel<12, 2><<<grid, 12 * 32, smem, stream>>>(p, slot);
-    } else {
-        return 1;
-    }
+    const size_t smem = (size_t)ns * p.ncols + (size_t)ns * nb * 4 + (size_t)ns * (p.ncols / 16) * 2 + (size_t)nrows_max * ns * 4 + 16 +
+                        (size_t)12 * 2 * slot;
+    if (smem > 220 * 1024) return 1;
+    KTB_CUDA_CHECK(cudaFuncSetAttribute(reduce_pipe_q6k8_kernel<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    reduce_pipe_q6k8_kernel<12><<<dim3(gx, T), 12 * 32, smem, stream>>>(p, slot);
     KTB_LAUNCH_CHECK();
     return KTB200_OK;
 }
 
-// Shared-memory plan of reduce_bulk_kernel<Fmt, S> for `pcap` staged (token, slot) pairs: returns the warp count
-// (0 = does not fit)
-template <class Fmt>
-static int reduce_bulk_plan(int rows, int ncols, int pcap, int S, int device, int* gx_out, int* nrows_max_out, size_t* smem_out) {
-    const int nb = ncols / QK_K;
-    if (rows % 4 || nb < 1 || pcap > 200) return 0;
-    const size_t item = (size_t)4 * nb * Fmt::kBlockBytes;
-    if (item % 16) return 0;
+// Plan of the bulk-copy down kernels (reduce_bulk_kernel, reduce_bulk_i4_kernel): one CTA per SM over 4-row items of
+// `item` bytes; a token chunk stages `pcap` (token, slot) pairs of `act_pair` activation bytes and a partial sum per row.
+// pcap: one token's worth (ns) at least; up to 2 tokens' worth (<= 18) when several tokens share the launch and >= 10
+// warps still fit.  W = 0: does not fit.
+struct DownPlan { int gx, nrows_max, pcap, W; size_t smem; };
+static DownPlan plan_down(int rows, int nb, int ns, int T, size_t act_pair, size_t item, int slots, int min_warps,
+                          int table_bytes, int device) {
+    DownPlan d{};
+    if (rows % 4 || nb < 1 || ns > 200 || item % 16) return d;
     const int quads = rows / 4;
-    int gx = num_sms(device);
-    if (gx > quads) gx = quads;
-    if (gx < 1) gx = 1;
-    const int nrows_max = ((quads + gx - 1) / gx) * 4;
-    size_t base = (size_t)pcap * nb * (kActBlkStride + 2 * Fmt::kBs + 4) + (size_t)nrows_max * pcap * 4 + (size_t)pcap * 4;
-    base = (base + 15) & ~(size_t)15;
-    const size_t cap = kSmemCap - Fmt::kTableBytes;
-    if (base + 16 >= cap) return 0;
-    int W = (int)((cap - base - 16) / ((size_t)S * (item + 8)));
-    if (W > cfg_bulk_warps()) W = cfg_bulk_warps();
-    if (W > kBulkMaxWarpsDown) W = kBulkMaxWarpsDown;
-    if (W < 2) return 0;
-    if (gx_out) *gx_out = gx;
-    if (nrows_max_out) *nrows_max_out = nrows_max;
-    if (smem_out) *smem_out = base + (((size_t)W * S * 8 + 15) & ~(size_t)15) + (size_t)W * S * item;
-    return W;
+    d.gx = grid_x(quads, device);
+    d.nrows_max = (quads + d.gx - 1) / d.gx * 4;
+    int want = ns;
+    if (T > 1) {
+        want = 2 * ns < 18 ? 2 * ns : (ns > 18 ? ns : 18);
+        if ((long)T * ns < want) want = T * ns;
+    }
+    const RingPlan pl = plan_ring(act_pair + (size_t)d.nrows_max * 4 + 4, ns, want, 10, 0, item, slots, min_warps,
+                                  kBulkMaxWarpsDown, table_bytes);
+    d.pcap = pl.chunk;
+    d.W = pl.W;
+    d.smem = pl.smem;
+    return d;
 }
 
 // Down projection through the bulk-copy ring.  Returns 1 when the shape does not suit it.
 template <class Fmt>
 static int launch_reduce_bulk(const ReduceParams& p, int T, int device, cudaStream_t stream) {
-    if (!cfg_bulk()) return 1;
-    const int ns = p.slots + (p.xw ? 1 : 0);
-    const int S = cfg_bulk_slots_down();
-    // pair capacity of a token chunk: one token's worth at least; up to 2 tokens' worth (<= 18) when several tokens
-    // share the launch and >= 10 warps still fit
-    int pcap = ns;
-    if (T > 1) {
-        int want = 2 * ns < 18 ? 2 * ns : (ns > 18 ? ns : 18);
-        if ((long)T * ns < want) want = T * ns;
-        while (want > ns && reduce_bulk_plan<Fmt>(p.rows, p.ncols, want, S, device, nullptr, nullptr, nullptr) < 10) want--;
-        pcap = want;
-    }
-    int gx = 0, nrows_max = 0;
-    size_t smem = 0;
-    const int W = reduce_bulk_plan<Fmt>(p.rows, p.ncols, pcap, S, device, &gx, &nrows_max, &smem);
-    if (!W) return 1;
-    if (S == 3) {
-        KTB_CUDA_CHECK(cudaFuncSetAttribute(reduce_bulk_kernel<Fmt, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        reduce_bulk_kernel<Fmt, 3><<<gx, W * 32, smem, stream>>>(p, nrows_max, pcap);
-    } else {
-        KTB_CUDA_CHECK(cudaFuncSetAttribute(reduce_bulk_kernel<Fmt, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        reduce_bulk_kernel<Fmt, 2><<<gx, W * 32, smem, stream>>>(p, nrows_max, pcap);
-    }
+    constexpr int S = 2;
+    const int nb = p.ncols / QK_K;
+    const DownPlan d = plan_down(p.rows, nb, p.slots + (p.xw ? 1 : 0), T, (size_t)nb * (kActBlkStride + 2 * Fmt::kBs + 4),
+                                 (size_t)4 * nb * Fmt::kBlockBytes, S, 2, Fmt::kTableBytes, device);
+    if (!d.W) return 1;
+    KTB_CUDA_CHECK(cudaFuncSetAttribute(reduce_bulk_kernel<Fmt, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d.smem));
+    reduce_bulk_kernel<Fmt, S><<<d.gx, d.W * 32, d.smem, stream>>>(p, d.nrows_max, d.pcap);
     KTB_LAUNCH_CHECK();
     return KTB200_OK;
 }
 
 // Load-time decision: can a Q6_K down tensor [rows][ncols] take the T4 tile layout (and therefore ONLY the bulk
 // kernel) for up to ns_max slots per token?
+constexpr int kQ6K4TPlanSlots = 3;   // one ring slot more than the launch uses: an accepted tensor launches with warps to spare
 static bool q6k4t_eligible(int rows, int ncols, int ns_max, int device) {
-    if (!cfg_bulk()) return false;
     const int nb = ncols / QK_K;
     if (nb % 2 || rows % 4) return false;
-    return reduce_bulk_plan<BulkQ6K4T>(rows, ncols, ns_max, 3, device, nullptr, nullptr, nullptr) >= 4;
+    using F = BulkQ6K4T;
+    return plan_down(rows, nb, ns_max, 1, (size_t)nb * (kActBlkStride + 2 * F::kBs + 4), (size_t)4 * nb * F::kBlockBytes,
+                     kQ6K4TPlanSlots, 4, F::kTableBytes, device).W > 0;
 }
 
-// Shared-memory plan of reduce_bulk_i4_kernel<S> for `pcap` staged pairs: returns the warp count (0 = does not fit)
-static int reduce_i4_plan(int rows, int ncols, int pcap, int S, int device, int* gx_out, int* nrows_max_out, size_t* smem_out) {
-    const int nb = ncols / QK_K;
-    if (rows % 4 || nb < 1 || pcap > 200) return 0;
-    const size_t item = (size_t)4 * nb * SZ_RAWINT4;
-    const int quads = rows / 4;
-    int gx = num_sms(device);
-    if (gx > quads) gx = quads;
-    if (gx < 1) gx = 1;
-    const int nrows_max = ((quads + gx - 1) / gx) * 4;
-    size_t base = (size_t)pcap * nb * kI4ActStride + (size_t)nrows_max * pcap * 4 + (size_t)pcap * 4;
-    base = (base + 15) & ~(size_t)15;
-    if (base + 16 >= kSmemCap) return 0;
-    int W = (int)((kSmemCap - base - 16) / ((size_t)S * (item + 8)));
-    if (W > cfg_bulk_warps()) W = cfg_bulk_warps();
-    if (W > kBulkMaxWarpsDown) W = kBulkMaxWarpsDown;
-    if (W < 1) return 0;
-    if (gx_out) *gx_out = gx;
-    if (nrows_max_out) *nrows_max_out = nrows_max;
-    if (smem_out) *smem_out = base + (((size_t)W * S * 8 + 15) & ~(size_t)15) + (size_t)W * S * item;
-    return W;
-}
-
-// RAWINT4 down projection (reduce_bulk_i4_kernel): pair capacity of a token chunk as in launch_reduce_bulk.
+// RAWINT4 down projection (reduce_bulk_i4_kernel): the only kernel for the format, so a shape it cannot take is an error.
 static int launch_reduce_i4(const ReduceParams& p, int T, int device, cudaStream_t stream) {
     constexpr int S = 2;
     if (p.xw) { set_error("RAWINT4 down: the shared expert cannot ride in the routed launch"); return KTB200_EINVAL; }
-    const int ns = p.slots;
-    int pcap = ns;
-    if (T > 1) {
-        int want = 2 * ns < 18 ? 2 * ns : (ns > 18 ? ns : 18);
-        if ((long)T * ns < want) want = T * ns;
-        while (want > ns && reduce_i4_plan(p.rows, p.ncols, want, S, device, nullptr, nullptr, nullptr) < 10) want--;
-        pcap = want;
-    }
-    int gx = 0, nrows_max = 0;
-    size_t smem = 0;
-    const int W = reduce_i4_plan(p.rows, p.ncols, pcap, S, device, &gx, &nrows_max, &smem);
-    if (!W) { set_error("RAWINT4 down: k=%d x intermediate_size=%d does not fit shared memory", ns, p.ncols); return KTB200_EINVAL; }
-    KTB_CUDA_CHECK(cudaFuncSetAttribute(reduce_bulk_i4_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    reduce_bulk_i4_kernel<S><<<gx, W * 32, smem, stream>>>(p, nrows_max, pcap);
+    const int nb = p.ncols / QK_K;
+    const DownPlan d = plan_down(p.rows, nb, p.slots, T, (size_t)nb * kI4ActStride, (size_t)4 * nb * SZ_RAWINT4, S, 1, 0, device);
+    if (!d.W) { set_error("RAWINT4 down: k=%d x intermediate_size=%d does not fit shared memory", p.slots, p.ncols); return KTB200_EINVAL; }
+    KTB_CUDA_CHECK(cudaFuncSetAttribute(reduce_bulk_i4_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d.smem));
+    reduce_bulk_i4_kernel<S><<<d.gx, d.W * 32, d.smem, stream>>>(p, d.nrows_max, d.pcap);
     KTB_LAUNCH_CHECK();
     return KTB200_OK;
 }
@@ -570,10 +487,10 @@ static int launch_reduce(FmtId f, const ReduceParams& p_in, int T, int device, c
         if (rc != 1) return rc;
     }
     switch (f) {
-        case FMT_Q4K: return launch_reduce_fmt<FmtQ4K, 2>(p, T, device, stream, true);
-        case FMT_Q5K: return launch_reduce_fmt<FmtQ5K, 1>(p, T, device, stream, false);
-        case FMT_Q6K8: return launch_reduce_fmt<FmtQ6K8, 1>(p, T, device, stream, true);
-        case FMT_GENK: return launch_reduce_fmt<FmtGenK, 1>(p, T, device, stream, false);
+        case FMT_Q4K: return launch_reduce_fmt<FmtQ4K, 2>(p, T, device, stream);
+        case FMT_Q5K: return launch_reduce_fmt<FmtQ5K, 1>(p, T, device, stream);
+        case FMT_Q6K8: return launch_reduce_fmt<FmtQ6K8, 1>(p, T, device, stream);
+        case FMT_GENK: return launch_reduce_fmt<FmtGenK, 1>(p, T, device, stream);
         default: set_error("unsupported weight type"); return KTB200_EINVAL;
     }
 }

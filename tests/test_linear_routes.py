@@ -79,7 +79,7 @@ def linear_route(t, n_in, n_out, T):
 
 
 def _bulk_down_warps(rows, ncols, block_bytes, bs, slots, pcap, sms):
-    """reduce_bulk_plan: warps of reduce_bulk_kernel for `pcap` staged pairs (0: does not fit)"""
+    """plan_down: warps of reduce_bulk_kernel for `pcap` staged pairs (0: does not fit)"""
     nb = ncols // QK
     item = 4 * nb * block_bytes
     if rows % 4 or item % 16 or pcap > 200:
