@@ -153,9 +153,15 @@ __device__ __forceinline__ float warp_sum(float v) {
 __device__ __forceinline__ float fp16_bits_to_f32(uint16_t h) { return __half2float(__ushort_as_half(h)); }
 
 // ------------------------------------------------------------------ IQ1_S / IQ2_XXS arithmetic shared by iq.cuh and grouped.cu
-// a super-block's fp32 term (DESIGN.md §2): ((d / 8) * dx) * S with the exact integer S of the super-block
+// a super-block's fp32 term (DESIGN.md §2): ((d / 8) * dx) * S with the exact integer S of the super-block; also the term
+// (d * dx) * isum of Q3_K and Q6_K (gemv_bulk.cuh BulkQ3K, grouped.cu)
 __device__ __forceinline__ float iq_d8(uint16_t d_bits) { return fp16_bits_to_f32(d_bits) * 0.125f; }
 __device__ __forceinline__ float iq_term(float d8, float dx, int isum) { return (d8 * dx) * (float)isum; }
+// the term of a K-quant with mins (gemv_bulk.cuh BulkQ2K; grouped.cu's Q4_K, Q5_K and Q2_K finish): (d * dx) * isum -
+// (dmin * dx) * msum, msum the exact sum of the mins times the activation sums
+__device__ __forceinline__ float kq_min_term(float d, float dmin, float dx, int isum, float msum) {
+    return (d * dx) * (float)isum - (dmin * dx) * msum;
+}
 // an IQ2_XXS sign pattern (ksigns_iq2xs byte) as byte masks: value = (grid ^ m) - m per byte
 __device__ __forceinline__ uint2 iq2_sign_masks(uint32_t s) {
     uint32_t lo = 0, hi = 0;

@@ -319,6 +319,116 @@ struct BulkQ6K4T {   // chunk-major 4-row tiles (see the header comment)
     }
 };
 
+// Raw Q2_K and Q3_K super-blocks, one per lane: the down items of reduce_bulk_kernel (4 rows x nb blocks, block f at
+// f * kBlockBytes) and the gate/up formats of rows_bulk_iq_kernel (iq.cuh).  No load-time re-layout: the grouped GEMM reads the
+// same tensors.  Value 128 n + 32 j + l (n < 2, j < 4, l < 32) is bits 2j..2j+1 of qs[32 n + l] and lies in 16-value group
+// g = 8 n + 2 j + (l >= 16).  Integer sums per super-block are exact; the fp32 finish is the grouped GEMM's (common.cuh).
+struct BulkQ2K {   // {scales[16] (scale | min << 4), qs[64], d, dmin} = 84 B: 4-byte aligned
+    static constexpr int kType = KTB200_TYPE_Q2_K;
+    static constexpr int kBlockBytes = SZ_Q2_K;
+    static constexpr int kBs = 16;          // the mins need the 16-value activation sums
+    static constexpr int kTableBytes = 0;
+    static constexpr bool kSharedSlot = true;   // rows_bulk_iq_kernel: a shared expert of this type can ride as slot `slots`
+    __device__ static __forceinline__ void stage_tables() {}
+    // isum = sum_g sc_g * sum q * q8 (q 0..3), msum = sum_g m_g * bsum16_g
+    __device__ static __forceinline__ float block_dot(const uint8_t* wb, const uint8_t* aq, const int16_t* bs16, float dxb) {
+        const uint32_t* w = reinterpret_cast<const uint32_t*>(wb);
+        const uint32_t sm[4] = {w[0], w[1], w[2], w[3]};   // byte g of the 16: group g
+        int isum = 0;
+#pragma unroll
+        for (int n = 0; n < 2; n++) {
+            uint32_t q[8];
+#pragma unroll
+            for (int i = 0; i < 8; i++) q[i] = w[4 + 8 * n + i];
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                const uint4 a0 = *reinterpret_cast<const uint4*>(aq + 128 * n + 32 * j);
+                const uint4 a1 = *reinterpret_cast<const uint4*>(aq + 128 * n + 32 * j + 16);
+                int s0 = dp4a_s8s8((q[0] >> (2 * j)) & 0x03030303u, a0.x, 0);
+                s0 = dp4a_s8s8((q[1] >> (2 * j)) & 0x03030303u, a0.y, s0);
+                s0 = dp4a_s8s8((q[2] >> (2 * j)) & 0x03030303u, a0.z, s0);
+                s0 = dp4a_s8s8((q[3] >> (2 * j)) & 0x03030303u, a0.w, s0);
+                int s1 = dp4a_s8s8((q[4] >> (2 * j)) & 0x03030303u, a1.x, 0);
+                s1 = dp4a_s8s8((q[5] >> (2 * j)) & 0x03030303u, a1.y, s1);
+                s1 = dp4a_s8s8((q[6] >> (2 * j)) & 0x03030303u, a1.z, s1);
+                s1 = dp4a_s8s8((q[7] >> (2 * j)) & 0x03030303u, a1.w, s1);
+                const uint32_t scw = sm[2 * n + (j >> 1)] >> (16 * (j & 1));   // groups 8n + 2j, 8n + 2j + 1 in bytes 0, 1
+                isum += (int)(scw & 0xf) * s0 + (int)((scw >> 8) & 0xf) * s1;
+            }
+        }
+        const uint4 b0 = *reinterpret_cast<const uint4*>(bs16), b1 = *reinterpret_cast<const uint4*>(bs16 + 8);
+        const uint32_t m0 = (sm[0] >> 4) & 0x0f0f0f0fu, m1 = (sm[1] >> 4) & 0x0f0f0f0fu;
+        const uint32_t m2 = (sm[2] >> 4) & 0x0f0f0f0fu, m3 = (sm[3] >> 4) & 0x0f0f0f0fu;
+        int msum = __dp2a_lo((int)b0.x, (int)m0, 0);
+        msum = __dp2a_hi((int)b0.y, (int)m0, msum);
+        msum = __dp2a_lo((int)b0.z, (int)m1, msum);
+        msum = __dp2a_hi((int)b0.w, (int)m1, msum);
+        msum = __dp2a_lo((int)b1.x, (int)m2, msum);
+        msum = __dp2a_hi((int)b1.y, (int)m2, msum);
+        msum = __dp2a_lo((int)b1.z, (int)m3, msum);
+        msum = __dp2a_hi((int)b1.w, (int)m3, msum);
+        const float2 dm = __half22float2(*reinterpret_cast<const __half2*>(w + 20));
+        return kq_min_term(dm.x, dm.y, dxb, isum, (float)msum);
+    }
+    __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int /*nrb*/, const uint8_t* aq, const int16_t* bs, float dxb) {
+        return block_dot(sl + f * SZ_Q2_K, aq, bs, dxb);
+    }
+};
+
+struct BulkQ3K {   // {hmask[32], qs[64], scales[12], d} = 110 B: 2-byte aligned, 4-byte aligned on even f
+    static constexpr int kType = KTB200_TYPE_Q3_K;
+    static constexpr int kBlockBytes = SZ_Q3_K;
+    static constexpr int kBs = 8;           // staged, not read
+    static constexpr int kTableBytes = 0;
+    static constexpr bool kSharedSlot = true;
+    __device__ static __forceinline__ void stage_tables() {}
+    // isum = sum_g (sc_g - 32) * sum (q - 4 [hmask bit clear]) * q8, the hmask term as a second dp4a on the clear bits.
+    // Words are read as the grouped producer reads them: the aligned words covering the block, funnel-shifted by 16 bits when
+    // the block starts mid-word.  The last word read (27) ends inside this block or the next one, which always exists: units
+    // and items hold an even number of blocks.
+    __device__ static __forceinline__ float block_dot(const uint8_t* wb, const uint8_t* aq, const int16_t* /*bs*/, float dxb) {
+        const uint32_t sh = (uint32_t)(reinterpret_cast<uintptr_t>(wb) & 2u) * 8u;
+        const uint32_t* w = reinterpret_cast<const uint32_t*>(wb - (sh >> 3));
+        auto word = [&](int i) { return __funnelshift_r(w[i], w[i + 1], sh); };
+        const uint32_t s0 = word(24), s1 = word(25), s2 = word(26);
+        const float d = fp16_bits_to_f32((uint16_t)(w[27] >> sh));
+        // 6-bit scales of groups 4c..4c+3 in word c: low nibbles from s0 / s1, high bit pairs from s2
+        const uint32_t sc[4] = {(s0 & 0x0f0f0f0fu) | ((s2 << 4) & 0x30303030u), (s1 & 0x0f0f0f0fu) | ((s2 << 2) & 0x30303030u),
+                                ((s0 >> 4) & 0x0f0f0f0fu) | (s2 & 0x30303030u), ((s1 >> 4) & 0x0f0f0f0fu) | ((s2 >> 2) & 0x30303030u)};
+        int isum = 0;
+#pragma unroll
+        for (int h = 0; h < 2; h++) {   // l < 16, l >= 16: a quarter of the words live at a time
+            uint32_t nh[4];   // hmask complemented: bit 4n + j of byte l set where value 128 n + 32 j + l takes the - 4
+#pragma unroll
+            for (int i = 0; i < 4; i++) nh[i] = ~word(4 * h + i);
+#pragma unroll
+            for (int n = 0; n < 2; n++) {
+                uint32_t q[4];
+#pragma unroll
+                for (int i = 0; i < 4; i++) q[i] = word(8 + 8 * n + 4 * h + i);
+#pragma unroll
+                for (int j = 0; j < 4; j++) {
+                    const uint4 a = *reinterpret_cast<const uint4*>(aq + 128 * n + 32 * j + 16 * h);
+                    const uint32_t ax[4] = {a.x, a.y, a.z, a.w};
+                    int s = 0, t = 0;
+#pragma unroll
+                    for (int i = 0; i < 4; i++) {
+                        s = dp4a_s8s8((q[i] >> (2 * j)) & 0x03030303u, ax[i], s);
+                        t = dp4a_s8s8((nh[i] >> (4 * n + j)) & 0x01010101u, ax[i], t);
+                    }
+                    // group 8n + 2j + h: byte 2 (j & 1) + h of scale word 2n + (j >> 1)
+                    const int sg = (int)((sc[2 * n + (j >> 1)] >> (16 * (j & 1) + 8 * h)) & 0xff) - 32;
+                    isum += sg * (s - 4 * t);
+                }
+            }
+        }
+        return iq_term(d, dxb, isum);
+    }
+    __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int /*nrb*/, const uint8_t* aq, const int16_t* bs, float dxb) {
+        return block_dot(sl + f * SZ_Q3_K, aq, bs, dxb);
+    }
+};
+
 // Down projection + weighted combine.  Work item of a warp = (pair, 4 consecutive output rows) = one bulk copy; every
 // CTA owns a contiguous range of row quads for ALL pairs so the combine over experts stays in the CTA.
 //

@@ -584,7 +584,7 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                     if (!MINS && hh == 1) {
 #pragma unroll
                         for (int i = 0; i < 16; i++) {
-                            acc[i] += (__uint_as_float(hw[(i >> 1) & 1][2]) * misc.dxs[hs][8 * (i >> 2) + cq + (i & 1)]) * (float)isum[i];
+                            acc[i] += iq_term(__uint_as_float(hw[(i >> 1) & 1][2]), misc.dxs[hs][8 * (i >> 2) + cq + (i & 1)], isum[i]);
                             isum[i] = 0;
                         }
                     }
@@ -602,7 +602,7 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                         const __half2 dm = *reinterpret_cast<const __half2*>(&hw[(i >> 1) & 1][FMT == 7 ? 2 : 0]);
                         const float dw = __low2float(dm), dmin = __high2float(dm);
                         const float dx = misc.dxs[hs][8 * (i >> 2) + cq + (i & 1)];
-                        acc[i] += (dw * dx) * (float)isum[i] - (dmin * dx) * ms[i];
+                        acc[i] += kq_min_term(dw, dmin, dx, isum[i], ms[i]);
                         isum[i] = 0;
                     }
                 }

@@ -6,7 +6,8 @@
 //   * gate/up: rows_bulk_iq_kernel.  A row is nblk * 50 B (IQ1_S) or nblk * 66 B (IQ2_XXS): 1400 B / 1848 B at H = 7168,
 //     not a multiple of 16, so a single row cannot be one bulk copy.  The unit is two consecutive rows (2800 B / 3696 B,
 //     16-byte aligned when nblk % 4 == 0): one ring slot holds the gate rows 2r, 2r+1 and the up rows 2r, 2r+1 (two copies
-//     on one mbarrier), so one read of x serves both matrices and the raw GGUF bytes are used as they are.
+//     on one mbarrier), so one read of x serves both matrices and the raw GGUF bytes are used as they are.  The same kernel
+//     takes Q2_K and Q3_K gate/up (formats BulkQ2K / BulkQ3K, gemv_bulk.cuh): 168 B / 220 B per block pair of a unit.
 //
 // Codebooks: IQ1_S's 2048 x 8 int8 grid as 16 KB of uint2 (one LDS.64 per 8 values, no unpacking); IQ2_XXS's 256 x 8
 // grid (2 KB) and its 128 sign patterns expanded to byte masks (1 KB: value = (g ^ m) - m per byte).  Both are copied from
@@ -34,6 +35,7 @@ struct BulkIQ1S {
     static constexpr int kBlockBytes = SZ_IQ1_S;
     static constexpr int kBs = 8;            // int16 activation sums per block (32-value groups)
     static constexpr int kTableBytes = 2048 * 8;
+    static constexpr bool kSharedSlot = false;   // shared experts are never i-quants (MLPs take K-quants only)
     __device__ static __forceinline__ void stage_tables() {
         uint2* g = iq1s_grid_smem();
         for (int i = threadIdx.x; i < 2048; i += blockDim.x) g[i] = *reinterpret_cast<const uint2*>(ktb_iq1s_grid[i]);
@@ -77,6 +79,7 @@ struct BulkIQ2XXS {
     static constexpr int kBlockBytes = SZ_IQ2_XXS;
     static constexpr int kBs = 8;
     static constexpr int kTableBytes = 256 * 8 + 128 * 8;
+    static constexpr bool kSharedSlot = false;
     __device__ static __forceinline__ void stage_tables() {
         uint2* g = iq2xxs_grid_smem();
         uint2* m = iq2xxs_signs_smem();
@@ -112,8 +115,9 @@ struct BulkIQ2XXS {
 };
 
 // ---------------------------------------------------------------------------------------------------------------
-// Gate/up pairs of IQ1_S or IQ2_XXS experts (gate and up of the same type).  Structure of rows_bulk_q4k_kernel (token
-// chunks, one (token, slot) work list per chunk, Q8_K activations staged side by side), with a 2-row unit per ring slot.
+// Gate/up pairs of IQ1_S, IQ2_XXS, Q2_K or Q3_K experts (gate and up of the same type).  Structure of rows_bulk_q4k_kernel
+// (token chunks, one (token, slot) work list per chunk, Q8_K activations staged side by side), with a 2-row unit per ring slot.
+// Fmt::kSharedSlot: a shared expert (p.x0 / p.x1, launcher: every token of the chunk) is slot p.slots of every token.
 constexpr int kIqMaxWarps = 16;
 template <class Fmt, int SLOTS>
 __global__ void __launch_bounds__(kIqMaxWarps * 32, 1) rows_bulk_iq_kernel(const RowsParams p, int act_tok, int tc) {
@@ -128,10 +132,12 @@ __global__ void __launch_bounds__(kIqMaxWarps * 32, 1) rows_bulk_iq_kernel(const
     const int unit_bytes = 2 * row_bytes;             // rows 2r, 2r+1 of one matrix
     const int slot_bytes = 2 * unit_bytes;            // gate unit | up unit
     const int nru = p.rows / 2;                       // row pairs per matrix
-    const int total_out = p.slots * p.rows;
-    // [tc activation rows: q8 [nblk][272] | bs32 [nblk][8] int16 | dx [nblk]] [pair list] [mbarriers] [rings]
+    const int nslots = p.slots + (Fmt::kSharedSlot && p.x0 ? 1 : 0);
+    const int total_out = nslots * p.rows;
+    // [tc activation rows: q8 [nblk][272] | bs [nblk][kBs] int16 | dx [nblk]] [pair list] [mbarriers] [rings]
     int* pairs = reinterpret_cast<int*>(smem + (size_t)tc * act_tok);
-    const size_t off = ((size_t)tc * act_tok + (size_t)tc * p.slots * 4 + 15) & ~(size_t)15;
+    // (p.slots spelled out, and the staging offsets below written per kBs, keep the i-quant instantiations' code as it was)
+    const size_t off = ((size_t)tc * act_tok + (size_t)tc * (Fmt::kSharedSlot ? nslots : p.slots) * 4 + 15) & ~(size_t)15;
     const int bar_bytes = (W * SLOTS * 8 + 15) & ~15;
     const uint32_t bar_u32 = (uint32_t)__cvta_generic_to_shared(smem + off) + warp * SLOTS * 8;
     uint8_t* ring = smem + off + bar_bytes + (size_t)warp * SLOTS * slot_bytes;
@@ -150,11 +156,13 @@ __global__ void __launch_bounds__(kIqMaxWarps * 32, 1) rows_bulk_iq_kernel(const
     __syncthreads();
     if (threadIdx.x == 0) {
         int np = 0;
-        for (int tl = 0; tl < nt; tl++)
+        for (int tl = 0; tl < nt; tl++) {
             for (int s = 0; s < p.slots; s++) {
                 const long e = (long)p.ids[(long)(t0 + tl) * p.slots + s] - p.id_offset;
                 if (e >= 0 && e < p.n_experts) pairs[np++] = (tl << 8) | s;
             }
+            if (Fmt::kSharedSlot && p.x0) pairs[np++] = (tl << 8) | p.slots;
+        }
         s_np = np;
     }
     __syncthreads();
@@ -170,12 +178,13 @@ __global__ void __launch_bounds__(kIqMaxWarps * 32, 1) rows_bulk_iq_kernel(const
         if (iss < nu) {
             if (lane == 0) {
                 const int pr = pairs[ipi];
-                const long e = (long)p.ids[(long)(t0 + (pr >> 8)) * p.slots + (pr & 0xff)] - p.id_offset;
+                const bool sh = Fmt::kSharedSlot && (pr & 0xff) == p.slots;
+                const long e = sh ? 0L : (long)p.ids[(long)(t0 + (pr >> 8)) * p.slots + (pr & 0xff)] - p.id_offset;
                 const long first = (e * p.rows + 2L * iru) * row_bytes;
                 const uint32_t bar = bar_u32 + 8 * slot_i, dst = ring_u32 + slot_i * slot_bytes;
                 mbar_expect_tx(bar, (uint32_t)slot_bytes);
-                bulk_g2s(dst, reinterpret_cast<const uint8_t*>(p.w0) + first, (uint32_t)unit_bytes, bar);
-                bulk_g2s(dst + unit_bytes, reinterpret_cast<const uint8_t*>(p.w1) + first, (uint32_t)unit_bytes, bar);
+                bulk_g2s(dst, reinterpret_cast<const uint8_t*>(sh ? p.x0 : p.w0) + first, (uint32_t)unit_bytes, bar);
+                bulk_g2s(dst + unit_bytes, reinterpret_cast<const uint8_t*>(sh ? p.x1 : p.w1) + first, (uint32_t)unit_bytes, bar);
             }
             iss++;
             iru += W;
@@ -198,8 +207,9 @@ __global__ void __launch_bounds__(kIqMaxWarps * 32, 1) rows_bulk_iq_kernel(const
             const int tl = g / nblk, b = g - tl * nblk;
             uint8_t* at = smem + (size_t)tl * act_tok;
             warp_quantize_q8k_block(cur, lane, reinterpret_cast<uint32_t*>(at + (size_t)b * kActBlkStride),
-                                    reinterpret_cast<float*>(at + (size_t)nblk * (kActBlkStride + 16)) + b, nullptr,
-                                    reinterpret_cast<int16_t*>(at + (size_t)nblk * kActBlkStride) + b * 8);
+                                    reinterpret_cast<float*>(at + (size_t)nblk * (kActBlkStride + 2 * Fmt::kBs)) + b,
+                                    Fmt::kBs == 16 ? reinterpret_cast<int16_t*>(at + (size_t)nblk * kActBlkStride) + b * 16 : nullptr,
+                                    Fmt::kBs == 8 ? reinterpret_cast<int16_t*>(at + (size_t)nblk * kActBlkStride) + b * 8 : nullptr);
 #pragma unroll
             for (int i = 0; i < 8; i++) cur[i] = nxt[i];
             g = gn;
@@ -213,14 +223,14 @@ __global__ void __launch_bounds__(kIqMaxWarps * 32, 1) rows_bulk_iq_kernel(const
         const uint8_t* sl = ring + slot_u * slot_bytes;
         const int pr = pairs[cpi];
         const uint8_t* at = smem + (size_t)(pr >> 8) * act_tok;
-        const int16_t* bs32 = reinterpret_cast<const int16_t*>(at + (size_t)nblk * kActBlkStride);
-        const float* dx = reinterpret_cast<const float*>(at + (size_t)nblk * (kActBlkStride + 16));
+        const int16_t* bs = reinterpret_cast<const int16_t*>(at + (size_t)nblk * kActBlkStride);
+        const float* dx = reinterpret_cast<const float*>(at + (size_t)nblk * (kActBlkStride + 2 * Fmt::kBs));
         float g0 = 0.f, g1 = 0.f, v0 = 0.f, v1 = 0.f;
         for (int f = lane; f < 2 * nblk; f += 32) {   // (row, block) of the unit: f = rw * nblk + blk
             const int rw = f >= nblk, blk = f - rw * nblk;
             const uint8_t* aq = at + (size_t)blk * kActBlkStride;
-            const float g = Fmt::block_dot(sl + f * Fmt::kBlockBytes, aq, bs32 + blk * 8, dx[blk]);
-            const float u = Fmt::block_dot(sl + unit_bytes + f * Fmt::kBlockBytes, aq, bs32 + blk * 8, dx[blk]);
+            const float g = Fmt::block_dot(sl + f * Fmt::kBlockBytes, aq, bs + blk * Fmt::kBs, dx[blk]);
+            const float u = Fmt::block_dot(sl + unit_bytes + f * Fmt::kBlockBytes, aq, bs + blk * Fmt::kBs, dx[blk]);
             if (rw) { g1 += g; v1 += u; } else { g0 += g; v0 += u; }
         }
         const float r = warp_reduce4(g0, g1, v0, v1, lane);   // lane 0: g0, 8: g1, 16: u0, 24: u1

@@ -287,18 +287,21 @@ static int launch_rows_i4(const RowsParams& p, int T, int device, cudaStream_t s
     return KTB200_OK;
 }
 
-// IQ1_S / IQ2_XXS gate/up pairs through the bulk-copy ring (rows_bulk_iq_kernel, iq.cuh): 2-row units, 2 slots per warp,
-// tokens per chunk as many (<= 8) as leave room for >= 8 warps.  Returns 1 when the launch does not suit it (gate and up
-// of different types, rows not 16-byte aligned in pairs, a shared-expert slot): the generic kernels take it then.
+// IQ1_S / IQ2_XXS / Q2_K / Q3_K gate/up pairs of routed experts through the bulk-copy ring (rows_bulk_iq_kernel, iq.cuh):
+// 2-row units, 2 slots per warp, tokens per chunk as many (<= 8) as leave room for >= 8 warps.  Returns 1 when the launch
+// does not suit it (no expert ids, gate and up of different types, rows not 16-byte aligned in pairs, a shared-expert slot
+// the format has no room for or of one token only): the generic kernels take it then.
 template <class Fmt>
 static int launch_rows_bulk_iq(const RowsParams& p, int T, int device, cudaStream_t stream) {
     constexpr int S = 2;
     const int nblk = p.ncols / QK_K;
-    if (p.type0 != Fmt::kType || p.type1 != Fmt::kType || p.x0 || !p.ids || nblk % 4 || p.rows % 2 || p.slots > 200) return 1;
-    const long total = (long)p.slots * (p.rows / 2);
+    if (p.type0 != Fmt::kType || p.type1 != Fmt::kType || !p.ids || nblk % 4 || p.rows % 2 || p.slots > 200) return 1;
+    if (p.x0 && (!Fmt::kSharedSlot || p.shared_token >= 0)) return 1;
+    const int nslots = p.slots + (p.x0 ? 1 : 0);
+    const long total = (long)nslots * (p.rows / 2);
     if (total >= (1L << 26)) return 1;
-    const int act_tok = (nblk * kActBlkStride + nblk * 16 + nblk * 4 + 15) & ~15;
-    const RingPlan pl = plan_ring(act_tok + p.slots * 4, 1, T < 8 ? T : 8, 8, kGateUpSpare, (size_t)4 * nblk * Fmt::kBlockBytes,
+    const int act_tok = (nblk * (kActBlkStride + 2 * Fmt::kBs + 4) + 15) & ~15;
+    const RingPlan pl = plan_ring(act_tok + nslots * 4, 1, T < 8 ? T : 8, 8, kGateUpSpare, (size_t)4 * nblk * Fmt::kBlockBytes,
                                   S, 4, kIqMaxWarps, Fmt::kTableBytes);
     if (!pl.W) return 1;
     KTB_CUDA_CHECK(cudaFuncSetAttribute(rows_bulk_iq_kernel<Fmt, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
@@ -315,9 +318,14 @@ static int launch_rows(FmtId f, const RowsParams& p_in, int T, int device, cudaS
         if (!PAIR) { set_error("RAWINT4: routed experts only"); return KTB200_EINVAL; }
         return launch_rows_i4(p, T, device, stream);
     }
-    if (PAIR && f == FMT_GENK && is_iquant(p.type0)) {
-        const int rci = p.type0 == KTB200_TYPE_IQ1_S ? launch_rows_bulk_iq<BulkIQ1S>(p, T, device, stream)
-                                                     : launch_rows_bulk_iq<BulkIQ2XXS>(p, T, device, stream);
+    if (PAIR && f == FMT_GENK) {
+        int rci = 1;
+        switch (p.type0) {
+            case KTB200_TYPE_IQ1_S: rci = launch_rows_bulk_iq<BulkIQ1S>(p, T, device, stream); break;
+            case KTB200_TYPE_IQ2_XXS: rci = launch_rows_bulk_iq<BulkIQ2XXS>(p, T, device, stream); break;
+            case KTB200_TYPE_Q2_K: rci = launch_rows_bulk_iq<BulkQ2K>(p, T, device, stream); break;
+            case KTB200_TYPE_Q3_K: rci = launch_rows_bulk_iq<BulkQ3K>(p, T, device, stream); break;
+        }
         if (rci != 1) return rci;
     }
     if (!PAIR && f == FMT_Q4K) {
@@ -481,6 +489,14 @@ static int launch_reduce(FmtId f, const ReduceParams& p_in, int T, int device, c
                                                    : launch_reduce_bulk<BulkIQ2XXS>(p, T, device, stream);
         if (rc != 1) return rc;
     }
+    // Q2_K / Q3_K down items of routed experts, with a shared expert of every token at most (gemv_bulk.cuh); a Q3_K item is
+    // 16-byte aligned for an even nb only (plan_down declines it otherwise)
+    if (f == FMT_GENK && (p.type == KTB200_TYPE_Q2_K || p.type == KTB200_TYPE_Q3_K) && p.ids &&
+        !(p.xw && (p.shared_token >= 0 || p.xw_out))) {
+        const int rc = p.type == KTB200_TYPE_Q2_K ? launch_reduce_bulk<BulkQ2K>(p, T, device, stream)
+                                                  : launch_reduce_bulk<BulkQ3K>(p, T, device, stream);
+        if (rc != 1) return rc;
+    }
     if (p.xw && (p.shared_token >= 0 || p.xw_out)) { set_error("per-token shared slot: only the bulk-copy kernels implement it"); return KTB200_EINVAL; }
     if (f == FMT_Q6K8) {
         const int rc = launch_reduce_pipe_q6k8(p, T, device, stream);
@@ -629,8 +645,8 @@ void grouped_set_trace(long long* t);
 }
 // qlen from which the per-expert tensor-core GEMMs (grouped.cu) replace the per-pair GEMV kernels: the reference makes the
 // same split between MOE::forward_one and MOE::forward_many (moe.cpp:367-377, threshold group_min_len).  48 tokens for the
-// K-quants (Q5_K's per-pair kernels stay faster only below about 40 tokens at DeepSeek-V3's shapes, Q3_K's and Q2_K's at no
-// measured size; DESIGN.md §5); 80 for a
+// K-quants (Q5_K's per-pair kernels stay faster only below about 40 tokens at DeepSeek-V3's shapes; Q3_K's and Q2_K's bulk-copy
+// per-pair kernels up to about 100 / 150 tokens, a crossover this threshold does not follow yet: DESIGN.md §5, §8); 80 for a
 // handle with an IQ1_S or IQ2_XXS tensor, whose per-pair kernels stay faster up to about 68 tokens at DeepSeek-R1's shapes;
 // 96 for RAWINT4_G32, whose per-pair kernels stay faster up to 88 tokens at Kimi-K2's shapes (DESIGN.md §5).  KTB200_GROUPED_MIN, when set, is the threshold of every handle (0: never).
 void ktb200_debug_grouped(long long* trace_dev) { ktb::grouped_set_trace(trace_dev); }
