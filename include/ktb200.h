@@ -41,11 +41,15 @@ enum ktb200_ggml_type {
      *            four 7-bit indices into ksigns_iq2xs and the 4-bit scale s in bits 28..31; value = d*(2s+1)/8 * grid * sign
      *   IQ1_S    50 B: fp16 d, qs[32], qh uint16[8]; sub-block ib has ls = 2*((qh>>12)&7)+1, delta = qh bit 15 ? -1/8 : +1/8,
      *            group l = iq1s_grid[qs[4ib+l] | ((qh >> 3l) & 7) << 8]; value = d*ls*(grid + delta)
+     *   IQ1_M    56 B: qs[32], qh[16], scales uint16[4]; 8-value group l (0..31) has the nibble of qh byte l/2 (low for even
+     *            l): bits 0-2 the high bits of its iq1s_grid index qs[l] | (nibble & 7) << 8, bit 3 the sign of its
+     *            delta (+-1/8); 16-value half h (0..15) has ls = 2*((scales[h/4] >> 3(h%4)) & 7)+1; the fp16 d is the
+     *            four top nibbles, scales[0] >> 12 lowest; value = d*ls*(grid + delta)
      * vec_dot_type Q8_K.  Routed experts only (ktb200_moe_create, any mix with the K-quants); linears, MLP handles and the
      * one-token expert-parallel entry points reject them.  ktb200_moe_forward runs them per (token, expert) pair below 80
      * tokens and on the grouped tensor-core GEMM from 80 (gate, up and down each in its own format).  The codebooks are
      * ktransformers_b200/csrc/iq_tables.h. */
-    KTB200_TYPE_IQ2_XXS = 16, KTB200_TYPE_IQ1_S = 19,
+    KTB200_TYPE_IQ2_XXS = 16, KTB200_TYPE_IQ1_S = 19, KTB200_TYPE_IQ1_M = 29,
     /* Not a ggml type: ggml's ids stay below 64, so 256 cannot collide with one.
      * Symmetric INT4 in groups of 32 with bf16 scales (compressed-tensors "pack-quantized", kt-kernel's RAWINT4; Kimi-K2's
      * routed experts), in the device layout ktb200_rawint4_pack writes: 144 B per 256 values of a row,

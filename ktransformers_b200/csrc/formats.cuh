@@ -13,7 +13,7 @@
 //   FmtQ4K    raw GGUF block_q4_K (144 B, already 16-byte aligned)   unit = 16 B of qs = 32 weights, 4 blocks/step
 //   FmtQ5K    raw GGUF block_q5_K (176 B, 16-byte aligned)           unit = 16 B qs + qh   = 32 weights, 4 blocks/step
 //   FmtQ6K8   block_q6_K re-laid as "8-row SoA" (moe.cu repack)      unit = 48 B           = 64 weights, 8 blocks/step
-//   FmtGenK   any raw K-quant / IQ4_XS / IQ2_XXS / IQ1_S through byte loads (fallback)
+//   FmtGenK   any raw K-quant / IQ4_XS / IQ2_XXS / IQ1_S / IQ1_M through byte loads (fallback)
 //                                                                    unit = 16 weights,              2 blocks/step
 #pragma once
 #include "common.cuh"
@@ -418,6 +418,21 @@ __device__ inline void unpack_group16(int type, const uint8_t* b, int g, GroupK&
             const int delta = (qh & 0x8000u) ? -1 : 1;
             for (int l = 0; l < 2; l++) {
                 const int idx = ldg_u8(b + 2 + 4 * ib + l0 + l) | (int)(((qh >> (3 * (l0 + l))) & 7) << 8);
+                for (int j = 0; j < 8; j++) v[8 * l + j] = (int8_t)(8 * (int)(int8_t)ldg_u8(&ktb_iq1s_grid[idx][j]) + delta);
+            }
+            break;
+        }
+        case KTB200_TYPE_IQ1_M: {
+            // IQ1_S's form with the scale per 16 values and the delta per 8: 8*grid + delta (-9..9) with d/8
+            const uint32_t s01 = (uint32_t)ldg_u16(b + 48) | ((uint32_t)ldg_u16(b + 50) << 16);
+            const uint32_t s23 = (uint32_t)ldg_u16(b + 52) | ((uint32_t)ldg_u16(b + 54) << 16);
+            o.d = fp16_bits_to_f32(iq1m_d_bits(s01, s23)) * 0.125f;
+            o.isc = 2 * (int)((ldg_u16(b + 48 + 2 * (g >> 2)) >> (3 * (g & 3))) & 7) + 1;
+            const uint32_t qh = ldg_u8(b + 32 + g);   // low nibble: 8-value group 2g, high nibble: 2g + 1
+            for (int l = 0; l < 2; l++) {
+                const uint32_t nib = (qh >> (4 * l)) & 15;
+                const int idx = ldg_u8(b + 2 * g + l) | (int)((nib & 7) << 8);
+                const int delta = (nib & 8) ? -1 : 1;
                 for (int j = 0; j < 8; j++) v[8 * l + j] = (int8_t)(8 * (int)(int8_t)ldg_u8(&ktb_iq1s_grid[idx][j]) + delta);
             }
             break;

@@ -329,6 +329,7 @@ struct BulkQ2K {   // {scales[16] (scale | min << 4), qs[64], d, dmin} = 84 B: 4
     static constexpr int kBs = 16;          // the mins need the 16-value activation sums
     static constexpr int kTableBytes = 0;
     static constexpr bool kSharedSlot = true;   // rows_bulk_iq_kernel: a shared expert of this type can ride as slot `slots`
+    static constexpr int kNblkMultiple = 4;
     __device__ static __forceinline__ void stage_tables() {}
     // isum = sum_g sc_g * sum q * q8 (q 0..3), msum = sum_g m_g * bsum16_g
     __device__ static __forceinline__ float block_dot(const uint8_t* wb, const uint8_t* aq, const int16_t* bs16, float dxb) {
@@ -381,6 +382,7 @@ struct BulkQ3K {   // {hmask[32], qs[64], scales[12], d} = 110 B: 2-byte aligned
     static constexpr int kBs = 8;           // staged, not read
     static constexpr int kTableBytes = 0;
     static constexpr bool kSharedSlot = true;
+    static constexpr int kNblkMultiple = 4;
     __device__ static __forceinline__ void stage_tables() {}
     // isum = sum_g (sc_g - 32) * sum (q - 4 [hmask bit clear]) * q8, the hmask term as a second dp4a on the clear bits.
     // Words are read as the grouped producer reads them: the aligned words covering the block, funnel-shifted by 16 bits when

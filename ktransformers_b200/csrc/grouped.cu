@@ -41,6 +41,11 @@
 //         the Q4_K mins MMA (K = 16, one min per 16-value sum) and Q4_K's finish.  84-byte blocks: 4-byte cp.async words.
 // Q3_K / Q2_K split a row's stage between its two producer threads by byte position l (as Q6_K), so a thread converts 16 qs
 // (and 16 hmask) bytes and the 80-byte plan holds its share.
+// IQ1_M (FMT 8), the experts of DeepSeek-R1's 1.73-bit files: IQ1_S's codebook with an odd scale ls per 16 values and the delta
+// per 8, so FMT 2's producers (sub-blocks 4 hh + 2 part + {0, 1}, 8 * grid + delta from the staged codebook) feeding the Q6_K
+// MMAs (one K = 32 MMA per sub-block against the 64-row B, the two halves' ls as the header's signed bytes) and Q3_K's finish
+// with d / 8.  56-byte blocks are 8-byte aligned: a thread's 8 B of qs, 4 B of qh and the 8-byte scale field (which holds d) are
+// plain cp.async words in FMT 2's 48-byte raw slots; own plan constants (kGSmemM) for the 64-row B.
 #include <cuda_fp16.h>
 
 #include "act_quant.cuh"
@@ -81,6 +86,10 @@ constexpr int kGBI = kGN * 128, kRawPitchI = 48, kRawSlotI = 2 * kGM * kRawPitch
 constexpr int kOffBI = kGStages * kGA, kOffRawI = kOffBI + kGStages * kGBI, kOffTabI = kOffRawI + kGRaw * kRawSlotI, kOffMiscI = kOffTabI + kTabI;
 constexpr int kGSmemI = kOffMiscI + (int)sizeof(GrpMisc) + 1024;
 static_assert(kGSmemI <= 227 * 1024 && kOffBI % 1024 == 0 && kGBI % 1024 == 0, "IQ shared-memory plan");
+// IQ1_M plan: the IQ plan with the 64-row B of the 16-value sub-block formats (even / odd halves zeroed)
+constexpr int kOffBM = kGStages * kGA, kOffRawM = kOffBM + kGStages * kGB, kOffTabM = kOffRawM + kGRaw * kRawSlotI, kOffMiscM = kOffTabM + kTabI;
+constexpr int kGSmemM = kOffMiscM + (int)sizeof(GrpMisc) + 1024;
+static_assert(kGSmemM <= 227 * 1024 && kOffBM % 1024 == 0 && kGB % 1024 == 0, "IQ1_M shared-memory plan");
 
 struct GrpGemmParams {
     const uint8_t* w;          // expert weights
@@ -143,25 +152,29 @@ __global__ void grp_tiles_kernel(const int* nt_prefix, const int* offsets, int E
 //   Q3_K (l = 16 part + 0..15 of the half): bytes 0-15 the words covering scales[12] and d, 16-35 those covering hmask[l],
 //         36-55 those covering qs[32 hh + l], 56 token scale (threads 64-95), 4 activation piece
 //   Q2_K: 0 scales[16], 1 qs[32 hh + l], 2 d | dmin (bytes 32-35), 3 activation piece, 4 as Q4_K
+//   IQ1_M (the IQ slots, sub-blocks q = 2 hh + part times 2 + {0, 1}): bytes 0-7 qs[8 q .. + 8], 8-11 qh[4 q .. + 4], 16-23 the
+//         scale words (d and word q's ls), 24 token scale (threads 64-95), 2 activation piece
 template <int FMT>
 __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGemmParams p) {
     constexpr bool IQ = FMT == 2 || FMT == 3;
     constexpr bool K4 = FMT == 0 || FMT == 5;                 // 32-value sub-blocks with mins, u8 operands (Q4_K, Q5_K)
     constexpr bool MINS = K4 || FMT == 7;                     // the mins MMA and Q4_K's finish (Q4_K, Q5_K, Q2_K)
-    constexpr bool SUB16 = FMT == 1 || FMT == 6 || FMT == 7;  // 16-value sub-blocks on the 64-row B (Q6_K, Q3_K, Q2_K)
+    constexpr bool SUB16 = FMT == 1 || FMT == 6 || FMT == 7 || FMT == 8;  // 16-value sub-blocks on the 64-row B (Q6_K, Q3_K, Q2_K, IQ1_M)
+    constexpr bool IQM = FMT == 8;                            // IQ1_M: the IQ raw slots and codebook, the Q6_K MMAs
+    constexpr bool IQS = IQ || IQM;                           // the IQ raw-slot layout
     constexpr int nRaw = FMT == 5 ? kGRaw5 : kGRaw;
-    constexpr int offB = IQ ? kOffBI : kOffB, strideB = IQ ? kGBI : kGB, offRaw = IQ ? kOffRawI : kOffRaw,
-                  rawPitch = IQ ? kRawPitchI : FMT == 5 ? kRawPitch5 : kRawPitch, rawSlot = IQ ? kRawSlotI : FMT == 5 ? kRawSlot5 : kRawSlot,
-                  BS = FMT == 2 ? SZ_IQ1_S : FMT == 3 ? SZ_IQ2_XXS : FMT == 6 ? SZ_Q3_K : SZ_Q2_K;
+    constexpr int offB = IQ ? kOffBI : IQM ? kOffBM : kOffB, strideB = IQ ? kGBI : kGB, offRaw = IQ ? kOffRawI : IQM ? kOffRawM : kOffRaw,
+                  rawPitch = IQS ? kRawPitchI : FMT == 5 ? kRawPitch5 : kRawPitch, rawSlot = IQS ? kRawSlotI : FMT == 5 ? kRawSlot5 : kRawSlot,
+                  BS = FMT == 2 ? SZ_IQ1_S : FMT == 3 ? SZ_IQ2_XXS : FMT == 6 ? SZ_Q3_K : FMT == 8 ? SZ_IQ1_M : SZ_Q2_K;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base - raw);
-    GrpMisc& misc = *reinterpret_cast<GrpMisc*>(smem + (IQ ? kOffMiscI : kOffMiscG));
+    GrpMisc& misc = *reinterpret_cast<GrpMisc*>(smem + (IQ ? kOffMiscI : IQM ? kOffMiscM : kOffMiscG));
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nblk = p.Kc / QK_K, nst = 2 * nblk, MT = p.R / kGM;
-    uint2* tab = reinterpret_cast<uint2*>(smem + kOffTabI);   // IQ codebooks (read after the __syncthreads below)
-    if (FMT == 2) {
+    uint2* tab = reinterpret_cast<uint2*>(smem + (IQM ? kOffTabM : kOffTabI));   // IQ codebooks (read after the __syncthreads below)
+    if (FMT == 2 || IQM) {
         for (int i = tid; i < 2048; i += kGThreads) tab[i] = *reinterpret_cast<const uint2*>(ktb_iq1s_grid[i]);
     } else if (FMT == 3) {
         for (int i = tid; i < 256; i += kGThreads) tab[i] = *reinterpret_cast<const uint2*>(ktb_iq2xxs_grid[i]);
@@ -244,6 +257,12 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                         for (int i = 0; i < 4; i++) cp_async4(dst + 4 * i, fw + 4 * i);
                     }
                     if (part == 0) cp_async4(dst + 32, fw + 80);
+                } else if (IQM) {
+                    // sub-blocks 2 q, 2 q + 1: 8 bytes of qs, 4 of qh, the 8-byte scale field (d and their ls); 8-byte aligned blocks
+                    const int q = 2 * hh + part;
+                    cp_async8(dst, fw + 8 * q);
+                    cp_async4(dst + 8, fw + 32 + 4 * q);
+                    cp_async8(dst + 16, fw + 48);
                 } else if (IQ) {
                     // every word fetched holds at least one byte this thread needs (so it lies inside the tensor's pages);
                     // the last word of a field is only needed when the block starts on a word (the fields then start mid-word)
@@ -273,10 +292,10 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                         cp_async4(dst + 72, fitem + (long)13 * c16 + (ffi >> 1) * 4);
                     }
                 }
-                if (fxq) { cp_async16(dst + (IQ ? 32 : FMT == 6 ? 64 : 48), fxq); fxq += 128; }
+                if (fxq) { cp_async16(dst + (IQS ? 32 : FMT == 6 ? 64 : 48), fxq); fxq += 128; }
                 if (hh == 1) {
                     if (MINS && fbs) { cp_async16(dst + 64, fbs); fbs += 16; }
-                    if (fdx) { cp_async4(dst + (MINS ? 64 : IQ ? 24 : FMT == 6 ? 56 : 76), fdx); fdx += 1; }
+                    if (fdx) { cp_async4(dst + (MINS ? 64 : IQS ? 24 : FMT == 6 ? 56 : 76), fdx); fdx += 1; }
                     fw += FMT == 0 ? SZ_Q4_K : FMT == 5 ? SZ_Q5_K : (IQ || FMT >= 6) ? BS : 16;
                     ffi++;
                 }
@@ -302,7 +321,7 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                 cp_async_wait<nRaw - 1>();
                 if (tr) p.trace[(0 * 96 + st) * 4 + 1] = clock64();
                 const uint4* rs = reinterpret_cast<const uint4*>(raw_src + slot * rawSlot);
-                const uint4 f0 = rs[0], f1 = rs[1], f2 = rs[2], f3 = rs[IQ ? 2 : FMT == 6 ? 4 : 3], f4 = rs[IQ ? 1 : FMT == 6 ? 3 : 4];
+                const uint4 f0 = rs[0], f1 = rs[1], f2 = rs[2], f3 = rs[IQS ? 2 : FMT == 6 ? 4 : 3], f4 = rs[IQS ? 1 : FMT == 6 ? 3 : 4];
                 const uint4 f5 = rs[FMT == 5 ? 5 : 0], f6 = rs[FMT == 5 ? 6 : 0];   // Q5_K: qh
                 issue(raw_dst + slot * rawSlot);   // refill the slot just read (thread-private bytes: no barrier involved)
                 slot = slot == nRaw - 1 ? 0 : slot + 1;
@@ -349,6 +368,32 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                         uint8_t* a2 = smem + kOffA2 + stage * kGA2 + (r >> 3) * 256 + (r & 7) * 16 + part * 128;
                         *reinterpret_cast<uint4*>(a2) = make_uint4(h2(mn[0], mn[0]), h2(mn[1], mn[1]), h2(mn[2], mn[2]), h2(mn[3], mn[3]));
                     }
+                } else if (IQM) {
+                    // sub-block 4 hh + 2 part + j -> A chunks 4 part + 2 j, + 1 as FMT 2 with the delta per 8 values; header: the
+                    // stage's eight ls as bytes 0-7 (the Q6_K layout, byte 4 part + 2 j + half), word 2 = d / 8 as f32
+                    const uint32_t qs[2] = {f0.x, f0.y}, qh = f0.z;   // nibble 4 j + l of qh: group l of sub-block j, at bits 16 j + 4 l
+                    const uint32_t scw = (hh ? f1.y : f1.x) >> (16 * part);   // scale word 2 hh + part: ls of sub-block j at bits 6 j, 6 j + 3
+#pragma unroll
+                    for (int j = 0; j < 2; j++) {
+                        uint32_t v[8];
+#pragma unroll
+                        for (int l = 0; l < 4; l++) {
+                            const uint32_t nib = qh >> (16 * j + 4 * l);
+                            const uint2 g = tab[((qs[j] >> (8 * l)) & 0xffu) | ((nib & 7u) << 8)];
+                            const uint32_t dl = (nib & 8u) ? 0xffffffffu : 0x01010101u;
+                            v[2 * l] = __vadd4((g.x << 3) & 0xf8f8f8f8u, dl);
+                            v[2 * l + 1] = __vadd4((g.y << 3) & 0xf8f8f8f8u, dl);
+                        }
+                        const int c0 = 4 * part + 2 * j;
+                        *reinterpret_cast<uint4*>(arow + (((c0 + 0) ^ sw) << 4)) = make_uint4(v[0], v[1], v[2], v[3]);
+                        *reinterpret_cast<uint4*>(arow + (((c0 + 1) ^ sw) << 4)) = make_uint4(v[4], v[5], v[6], v[7]);
+                    }
+                    uint32_t ls = 0;
+#pragma unroll
+                    for (int i = 0; i < 4; i++) ls |= (2 * ((scw >> (3 * i)) & 7u) + 1) << (8 * i);
+                    uint32_t* hrow = reinterpret_cast<uint32_t*>(&misc.hdr[hs][r]);
+                    hrow[part] = ls;
+                    if (part == 0) hrow[2] = __float_as_uint(iq_d8(iq1m_d_bits(f1.x, f1.y)));
                 } else if (IQ) {
                     // sub-block 4 hh + 2 part + j -> A chunks 4 part + 2 j and 4 part + 2 j + 1; header word `part` = its two ls
                     // (16 bits each), word 2 = d / 8 as f32
@@ -470,7 +515,7 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                     *reinterpret_cast<uint4*>(Bs + (kGN + bn) * 128 + ((pc ^ (bn & 7)) << 4)) = (pc & 1) ? bv : z;
                 }
                 if (hh == 1 && pt < 96) {   // token scales, and (formats with mins) the sixteen 16-value sums of the super-block as fp16
-                    if (pt >= 64) misc.dxs[hs][pt - 64] = pt - 64 < n_valid ? __uint_as_float(MINS ? f4.x : (IQ || FMT == 6) ? f4.z : f4.w) : 0.f;
+                    if (pt >= 64) misc.dxs[hs][pt - 64] = pt - 64 < n_valid ? __uint_as_float(MINS ? f4.x : (IQS || FMT == 6) ? f4.z : f4.w) : 0.f;
                     else if (MINS) {
                         const int n2 = pt >> 1, kg = pt & 1;
                         uint4 vv = z;
@@ -985,6 +1030,7 @@ static int grouped_fmt(int type, int layout) {
     if (type == KTB200_TYPE_Q5_K) return 5;
     if (type == KTB200_TYPE_Q3_K) return 6;
     if (type == KTB200_TYPE_Q2_K) return 7;
+    if (type == KTB200_TYPE_IQ1_M) return 8;
     return -1;
 }
 static void grouped_i4(int np, const GrpI4Params& p, int grid, cudaStream_t s) {
@@ -999,12 +1045,13 @@ static void grouped_gemm(int fmt, const GrpGemmParams& p, int grid, cudaStream_t
         case 3: grouped_gemm_kernel<3><<<grid, kGThreads, kGSmemI, s>>>(p); break;
         case 5: grouped_gemm_kernel<5><<<grid, kGThreads, kGSmem, s>>>(p); break;
         case 6: grouped_gemm_kernel<6><<<grid, kGThreads, kGSmem, s>>>(p); break;
-        default: grouped_gemm_kernel<7><<<grid, kGThreads, kGSmem, s>>>(p); break;
+        case 7: grouped_gemm_kernel<7><<<grid, kGThreads, kGSmem, s>>>(p); break;
+        default: grouped_gemm_kernel<8><<<grid, kGThreads, kGSmemM, s>>>(p); break;
     }
 }
 
-// true when ktb200_moe_forward may take the grouped tensor-core path for this handle: gate and up Q4_K, Q5_K, Q3_K, Q2_K, IQ1_S
-// or IQ2_XXS (each on its own), down any of those or Q6_K in the tile layout; or all three RAWINT4_G32
+// true when ktb200_moe_forward may take the grouped tensor-core path for this handle: gate and up Q4_K, Q5_K, Q3_K, Q2_K, IQ1_S,
+// IQ1_M or IQ2_XXS (each on its own), down any of those or Q6_K in the tile layout; or all three RAWINT4_G32
 bool grouped_ok(const ktb200_moe* m, int k) {
     const ktb200_moe_config& c = m->cfg;
     const int fg = grouped_fmt(c.gate_type, LAYOUT_RAW), fu = grouped_fmt(c.up_type, LAYOUT_RAW), fd = grouped_fmt(c.down_type, m->down_layout);
@@ -1033,6 +1080,7 @@ int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, cons
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem));
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmemM));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_i4_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, I4Plan<1>::kSmem));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_i4_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, I4Plan<3>::kSmem));
         attr[dev & 63] = true;

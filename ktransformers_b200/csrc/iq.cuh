@@ -1,5 +1,6 @@
-// IQ1_S and IQ2_XXS routed experts on the bulk-copy ring (gemv_bulk.cuh): one lane per super-block, codebooks in shared
-// memory.
+// IQ1_S, IQ1_M and IQ2_XXS routed experts on the bulk-copy ring (gemv_bulk.cuh): one lane per super-block, codebooks in shared
+// memory.  IQ1_M (56-byte blocks, 8-byte aligned) takes every block count: its unit is 112 * nblk B and its item 224 * nb B, so
+// its launches skip the nblk % 4 (kNblkMultiple) condition of the 50 / 66-byte formats.
 //
 //   * down: item formats BulkIQ1S / BulkIQ2XXS of reduce_bulk_kernel — 4 rows x nb raw ggml blocks, one bulk copy
 //     (4 * nb * 50 B / 4 * nb * 66 B, a multiple of 16 when nb is even; 1600 B / 2112 B at I = 2048 = one block per lane);
@@ -9,7 +10,7 @@
 //     on one mbarrier), so one read of x serves both matrices and the raw GGUF bytes are used as they are.  The same kernel
 //     takes Q2_K and Q3_K gate/up (formats BulkQ2K / BulkQ3K, gemv_bulk.cuh): 168 B / 220 B per block pair of a unit.
 //
-// Codebooks: IQ1_S's 2048 x 8 int8 grid as 16 KB of uint2 (one LDS.64 per 8 values, no unpacking); IQ2_XXS's 256 x 8
+// Codebooks: IQ1_S's (and IQ1_M's) 2048 x 8 int8 grid as 16 KB of uint2 (one LDS.64 per 8 values, no unpacking); IQ2_XXS's 256 x 8
 // grid (2 KB) and its 128 sign patterns expanded to byte masks (1 KB: value = (g ^ m) - m per byte).  Both are copied from
 // the device tables of iq_tables.h once per CTA.
 //
@@ -36,6 +37,7 @@ struct BulkIQ1S {
     static constexpr int kBs = 8;            // int16 activation sums per block (32-value groups)
     static constexpr int kTableBytes = 2048 * 8;
     static constexpr bool kSharedSlot = false;   // shared experts are never i-quants (MLPs take K-quants only)
+    static constexpr int kNblkMultiple = 4;      // rows_bulk_iq_kernel: blocks per row for a 2-row unit of 16-byte size
     __device__ static __forceinline__ void stage_tables() {
         uint2* g = iq1s_grid_smem();
         for (int i = threadIdx.x; i < 2048; i += blockDim.x) g[i] = *reinterpret_cast<const uint2*>(ktb_iq1s_grid[i]);
@@ -74,12 +76,58 @@ struct BulkIQ1S {
     }
 };
 
+// IQ1_S's codebook with the scale per 16 values and the delta per 8.  The Q8_K sums cover 16 or 32 values, so the delta term is
+// summed per 8-value group: dp4a of the group's activations against 0x01010101 (+1) or 0xffffffff (-1).  56-byte blocks are
+// 8-byte aligned: words and the 8-byte scale field load whole.
+struct BulkIQ1M {
+    static constexpr int kType = KTB200_TYPE_IQ1_M;
+    static constexpr int kBlockBytes = SZ_IQ1_M;
+    static constexpr int kBs = 8;            // staged, not read
+    static constexpr int kTableBytes = 2048 * 8;
+    static constexpr bool kSharedSlot = false;
+    static constexpr int kNblkMultiple = 1;  // a 2-row unit is 112 * nblk B
+    __device__ static __forceinline__ void stage_tables() { BulkIQ1S::stage_tables(); }
+    // S = sum_h ls_h * sum_(8-groups l of h) (8 * sum grid * q8 + delta_l * sum q8); term = ((d/8) * dx) * S
+    __device__ static __forceinline__ float block_dot(const uint8_t* wb, const uint8_t* aq, const int16_t* /*bs*/, float dxb) {
+        const uint2* grid = iq1s_grid_smem();
+        const uint2 sc = *reinterpret_cast<const uint2*>(wb + 48);
+        const float d = iq_d8(iq1m_d_bits(sc.x, sc.y));
+        int isum = 0;
+#pragma unroll
+        for (int ib = 0; ib < 8; ib++) {
+            const uint32_t qs = *reinterpret_cast<const uint32_t*>(wb + 4 * ib);
+            const uint32_t qh = *reinterpret_cast<const uint16_t*>(wb + 32 + 2 * ib);   // nibble l (group 4 ib + l) at bits 4 l
+            const uint32_t sw = (ib < 4 ? sc.x : sc.y) >> (16 * ((ib >> 1) & 1) + 6 * (ib & 1));   // ls of the halves: bits 0-2, 3-5
+            const uint4 a0 = *reinterpret_cast<const uint4*>(aq + 32 * ib);
+            const uint4 a1 = *reinterpret_cast<const uint4*>(aq + 32 * ib + 16);
+            const uint32_t ax[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+            int v[2] = {0, 0};
+#pragma unroll
+            for (int l = 0; l < 4; l++) {
+                const uint2 g = grid[((qs >> (8 * l)) & 0xff) | (((qh >> (4 * l)) & 7) << 8)];
+                const uint32_t m = ((qh >> (4 * l + 3)) & 1) ? 0xffffffffu : 0x01010101u;
+                int s = dp4a_s8s8(g.x, ax[2 * l], 0);
+                s = dp4a_s8s8(g.y, ax[2 * l + 1], s);
+                int t = dp4a_s8s8(m, ax[2 * l], 0);
+                t = dp4a_s8s8(m, ax[2 * l + 1], t);
+                v[l >> 1] += 8 * s + t;
+            }
+            isum += (2 * (int)(sw & 7) + 1) * v[0] + (2 * (int)((sw >> 3) & 7) + 1) * v[1];
+        }
+        return iq_term(d, dxb, isum);
+    }
+    __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int /*nrb*/, const uint8_t* aq, const int16_t* bs, float dxb) {
+        return block_dot(sl + f * SZ_IQ1_M, aq, bs, dxb);
+    }
+};
+
 struct BulkIQ2XXS {
     static constexpr int kType = KTB200_TYPE_IQ2_XXS;
     static constexpr int kBlockBytes = SZ_IQ2_XXS;
     static constexpr int kBs = 8;
     static constexpr int kTableBytes = 256 * 8 + 128 * 8;
     static constexpr bool kSharedSlot = false;
+    static constexpr int kNblkMultiple = 4;
     __device__ static __forceinline__ void stage_tables() {
         uint2* g = iq2xxs_grid_smem();
         uint2* m = iq2xxs_signs_smem();

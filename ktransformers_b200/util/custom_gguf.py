@@ -67,7 +67,9 @@ GGML_BLOCK_SIZES = {t.name: GGML_QUANT_SIZES[t][1] for t in GGML_QUANT_SIZES}
 B200_WEIGHT_TYPES = {"Q2_K", "Q3_K", "Q4_K", "Q5_K", "Q6_K", "IQ4_XS"}
 # routed experts also take ggml's codebook i-quants (DeepSeek-R1's 1.5-2-bit GGUF files); linears and MLPs do not
 B200_EXPERT_TYPES = B200_WEIGHT_TYPES | {"IQ1_S", "IQ2_XXS"}
-B200_DEQUANT_TYPES = B200_EXPERT_TYPES | {"Q8_0", "F32", "F16", "BF16"}
+# what the routed-expert loaders accept: kept apart from B200_EXPERT_TYPES, whose value callers and tests rely on
+B200_ROUTED_EXPERT_TYPES = B200_EXPERT_TYPES | {"IQ1_M"}
+B200_DEQUANT_TYPES = B200_ROUTED_EXPERT_TYPES | {"Q8_0", "F32", "F16", "BF16"}
 # what the single-launch expert-parallel kernel takes: Q4_K gate/up, Q4_K or Q6_K down
 B200_EP_GATE_UP_TYPES = {"Q4_K"}
 B200_EP_DOWN_TYPES = {"Q4_K", "Q6_K"}
