@@ -35,65 +35,27 @@ __global__ void __launch_bounds__(kDenseWarps * 32, 1) dense_q4k_kernel(const De
     if (p.bsz) { griddep_wait(); T = min(T, *p.bsz); }
     const int nblk = p.ncols / QK_K;
     const int seg_bytes = p.segb * SZ_Q4_K;
-    const size_t off = ((size_t)p.T * p.act_tok + 15) & ~(size_t)15;
-    const int bar_bytes = (W * SLOTS * 8 + 15) & ~15;
-    const uint32_t bar_u32 = (uint32_t)__cvta_generic_to_shared(smem + off) + warp * SLOTS * 8;
-    const uint8_t* ring = smem + off + bar_bytes + (size_t)warp * SLOTS * seg_bytes;
-    const uint32_t ring_u32 = (uint32_t)__cvta_generic_to_shared(ring);
-    if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < SLOTS; s++) mbar_init(bar_u32 + 8 * s, 1);
-        mbar_fence_init();
-        fence_proxy_async_smem();
-    }
+    BulkRing<SLOTS> ring(smem, (size_t)p.T * p.act_tok, seg_bytes, lane, warp, W);
     // units: groups of R rows; this CTA's contiguous range, dealt round-robin to its warps
     const int nunits = (p.rows + p.R - 1) / p.R;
     const int u0 = (int)((long)nunits * blockIdx.x / gridDim.x), u1 = (int)((long)nunits * (blockIdx.x + 1) / gridDim.x);
-    int nu = u1 - u0 - warp;
-    nu = nu > 0 ? (nu + W - 1) / W : 0;
-    const int nseg = nu * p.G;                 // slots this warp consumes
-    int iu = u0 + warp, ig = 0, iss = 0;       // issue cursor: unit, segment of the unit, slots requested
-    int slot_i = 0, slot_u = 0;
-    uint32_t phase = 0;
+    const int nseg = warp_units(u0, u1, warp, W) * p.G;   // slots this warp consumes
+    int iu = u0 + warp, ig = 0, iss = 0;                  // issue cursor: unit, segment of the unit, slots requested
     auto issue_one = [&]() {
         if (iss < nseg) {
-            if (lane == 0) {
-                const int row0 = iu * p.R;
-                const int nrows = min(p.R, p.rows - row0);
-                const uint32_t bytes = (uint32_t)((p.G > 1 ? p.segb : nrows * nblk) * SZ_Q4_K);
-                const uint8_t* src = p.w + ((long)row0 * nblk + (long)ig * p.segb) * SZ_Q4_K;
-                const uint32_t bar = bar_u32 + 8 * slot_i;
-                mbar_expect_tx(bar, bytes);
-                bulk_g2s(ring_u32 + slot_i * seg_bytes, src, bytes, bar);
-            }
+            const int row0 = iu * p.R;
+            const int nrows = min(p.R, p.rows - row0);
+            const uint32_t bytes = (uint32_t)((p.G > 1 ? p.segb : nrows * nblk) * SZ_Q4_K);
+            ring.issue(lane, 1, bytes, [&](int) { return p.w + ((long)row0 * nblk + (long)ig * p.segb) * SZ_Q4_K; });
             iss++;
             if (++ig == p.G) { ig = 0; iu += W; }
-            slot_i = (slot_i + 1 == SLOTS) ? 0 : slot_i + 1;
         }
     };
 #pragma unroll
     for (int s = 0; s < SLOTS; s++) issue_one();   // weights do not depend on the previous kernel: requested before the wait
     griddep_wait();
 
-    {   // activations -> Q8_K, padded layout (as in rows_bulk_q4k_kernel): block g = (token, block of the row)
-        float cur[8], nxt[8];
-        const int totalb = T * nblk;
-        int g = warp;
-        if (g < totalb) load_block8(p.x, (long)(g / nblk) * p.ncols + (long)(g % nblk) * QK_K + lane * 8, p.hidden_type, cur);
-#pragma unroll 1
-        while (g < totalb) {
-            const int gn = g + W;
-            if (gn < totalb) load_block8(p.x, (long)(gn / nblk) * p.ncols + (long)(gn % nblk) * QK_K + lane * 8, p.hidden_type, nxt);
-            const int tl = g / nblk, b = g - tl * nblk;
-            uint8_t* at = smem + (size_t)tl * p.act_tok;
-            warp_quantize_q8k_block(cur, lane, reinterpret_cast<uint32_t*>(at + (size_t)b * kActBlkStride),
-                                    reinterpret_cast<float*>(at + (size_t)nblk * (kActBlkStride + 16)) + b, nullptr,
-                                    reinterpret_cast<int16_t*>(at + (size_t)nblk * kActBlkStride) + b * 8);
-#pragma unroll
-            for (int i = 0; i < 8; i++) cur[i] = nxt[i];
-            g = gn;
-        }
-    }
+    stage_q8k_rows<8>(p.x, p.hidden_type, 0, T, p.ncols, smem, p.act_tok, lane, warp, W);   // as in rows_bulk_q4k_kernel
     __syncthreads();
 
     float acc[kDenseMaxTokens];
@@ -101,9 +63,7 @@ __global__ void __launch_bounds__(kDenseWarps * 32, 1) dense_q4k_kernel(const De
     for (int t = 0; t < kDenseMaxTokens; t++) acc[t] = 0.f;
     int cu = u0 + warp, cg = 0;
     for (int n = 0; n < nseg; n++) {
-        mbar_wait(bar_u32 + 8 * slot_u, (phase >> slot_u) & 1u);
-        phase ^= 1u << slot_u;
-        const uint8_t* sl = ring + slot_u * seg_bytes;
+        const uint8_t* sl = ring.wait();
         const int row0 = cu * p.R;
         const int nrows = min(p.R, p.rows - row0);
         const int nact = p.G > 1 ? p.segb : nrows * nblk;            // blocks in this slot
@@ -119,8 +79,7 @@ __global__ void __launch_bounds__(kDenseWarps * 32, 1) dense_q4k_kernel(const De
                 }
             }
         }
-        __syncwarp();
-        slot_u = (slot_u + 1 == SLOTS) ? 0 : slot_u + 1;
+        ring.release();
         issue_one();
         if (++cg < p.G) continue;
         cg = 0;

@@ -17,44 +17,18 @@
 //
 // Arithmetic is unchanged from the earlier generations (bit-exact Q8_K activations, integer dot products, fp32
 // once per super-block): see DESIGN.md §2.
+//
+// Kernels on this ring: rows_bulk_q4k_kernel and reduce_bulk_kernel (here; the down item formats BulkQ4K, BulkQ6K4T,
+// BulkQ2K and BulkQ3K here, BulkIQ1S / BulkIQ1M / BulkIQ2XXS in iq.cuh, BulkI4 in rawint4.cuh), rows_bulk_iq_kernel (iq.cuh),
+// rows_bulk_i4_kernel (rawint4.cuh) and dense_q4k_kernel (dense_bulk.cuh).  The ring, work split, work lists and Q8_K
+// staging they share are in bulk_ring.cuh.
 #pragma once
-#include "gemv_pipe.cuh"
+#include "bulk_ring.cuh"
 
 namespace ktb {
 
-constexpr int kActBlkStride = QK_K + 16;   // int8 activation blocks padded to 272 B: 8 lanes x LDS.128 hit 32 distinct banks
 constexpr int kBulkMaxWarps = 18;        // gate/up kernel (<= 96 registers per thread)
 constexpr int kBulkMaxWarpsDown = 16;    // down kernel: 128 registers per thread, and shared memory caps it at 15 anyway
-
-// ---------------------------------------------------------------------------------------------------------------
-// mbarrier / bulk-copy PTX
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// global -> shared bulk copy (size and both addresses multiples of 16 B); completion is signalled on `bar`
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-                 "l"(src), "r"(bytes), "r"(bar)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred P1;\n"
-        "LAB_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n"
-        "@P1 bra DONE;\n"
-        "bra LAB_WAIT;\n"
-        "DONE:\n"
-        "}" ::"r"(bar),
-        "r"(parity)
-        : "memory");
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // One Q4_K super-block (144 B at `wb`, shared memory, 16-byte aligned) against one padded int8 activation block.
@@ -119,101 +93,46 @@ __global__ void __launch_bounds__(kBulkMaxWarps * 32, 1) rows_bulk_q4k_kernel(co
     constexpr int NM = PAIR ? 2 : 1;
     const int nslots = p.slots + (p.x0 ? 1 : 0);
     const int total_out = nslots * p.rows;
-    // [tc activation rows: q8 [nblk][272] | bs32 [nblk][8] int16 | dx [nblk]] [pair list: tc*nslots ints] [mbarriers] [rings]
+    // [tc activation rows: q8 [nblk][272] | bs32 [nblk][8] int16 | dx [nblk]] [pair list: tc*nslots ints] [ring]
     int* pairs = reinterpret_cast<int*>(smem + (size_t)tc * act_tok);                 // (token in chunk) << 8 | slot
-    const size_t off = ((size_t)tc * act_tok + (size_t)tc * nslots * 4 + 15) & ~(size_t)15;
-    const int bar_bytes = (W * SLOTS * 8 + 15) & ~15;
-    const uint32_t bar_u32 = (uint32_t)__cvta_generic_to_shared(smem + off) + warp * SLOTS * 8;
-    uint8_t* ring = smem + off + bar_bytes + (size_t)warp * SLOTS * row_bytes;
-    const uint32_t ring_u32 = (uint32_t)__cvta_generic_to_shared(ring);
-    if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < SLOTS; s++) mbar_init(bar_u32 + 8 * s, 1);
-        mbar_fence_init();
-        fence_proxy_async_smem();
-    }
-    int slot_i = 0, slot_u = 0;   // ring cursors (issue / use); they advance in lock step over the whole launch
-    uint32_t phase = 0;           // bit s = parity the next use of slot s waits for
+    BulkRing<SLOTS> ring(smem, (size_t)tc * act_tok + (size_t)tc * nslots * 4, row_bytes, lane, warp, W);
 
   for (int t0 = 0; t0 < Teff; t0 += tc) {
     const int nt = min(tc, Teff - t0);
     __syncthreads();   // previous chunk: everyone is done with the staging and the pair list (and the barriers are initialised)
-    if (threadIdx.x == 0) {
-        int np = 0;
-        for (int tl = 0; tl < nt; tl++) {
-            for (int s = 0; s < p.slots; s++) {
-                const long e = p.ids ? (long)p.ids[(long)(t0 + tl) * p.slots + s] - p.id_offset : 0;
-                if (e >= 0 && e < p.n_experts) pairs[np++] = (tl << 8) | s;
-            }
-            if (p.x0 && (p.shared_token < 0 || p.shared_token == t0 + tl)) pairs[np++] = (tl << 8) | p.slots;
-        }
-        s_np = np;
-    }
+    if (threadIdx.x == 0) s_np = gateup_pairs(p, t0, nt, p.x0 != nullptr, pairs);
     __syncthreads();
     const int total = s_np * p.rows;
     const int u0 = (int)((long)total * blockIdx.x / gridDim.x), u1 = (int)((long)total * (blockIdx.x + 1) / gridDim.x);
-    int nu = u1 - u0 - warp;
-    nu = nu > 0 ? (nu + W - 1) / W : 0;                     // units of this warp: u0 + warp + i*W
-    const int nsub = nu * NM;
-    // issue cursor: (pair index, row) of the next unit to request, and how many rows were requested
-    int ipi = 0, irr = 0, isub = 0;
-    if (nu > 0) { ipi = (u0 + warp) / p.rows; irr = (u0 + warp) - ipi * p.rows; }
-    int cpi = ipi, crr = irr;                               // consume cursor
+    const int nsub = warp_units(u0, u1, warp, W) * NM;
+    UnitCursor ic;                                          // (pair, row) of the next unit to request
+    if (nsub > 0) ic.start(u0 + warp, p.rows);
+    UnitCursor cc = ic;                                     // and of the unit being consumed
+    int isub = 0;                                           // rows requested
 
     auto issue_one = [&]() {
         if (isub < nsub) {
-            if (lane == 0) {
-                const int pr = pairs[ipi], s = pr & 0xff, tl = pr >> 8;
-                const bool second = PAIR && (isub & 1);
-                const uint8_t* src;
-                if (s == p.slots) {
-                    src = reinterpret_cast<const uint8_t*>(second ? p.x1 : p.x0) + (long)irr * row_bytes;
-                } else {
-                    const long e = p.ids ? (long)p.ids[(long)(t0 + tl) * p.slots + s] - p.id_offset : 0;
-                    src = reinterpret_cast<const uint8_t*>(second ? p.w1 : p.w0) + (e * p.rows + irr) * row_bytes;
-                }
-                const uint32_t bar = bar_u32 + 8 * slot_i;
-                mbar_expect_tx(bar, (uint32_t)row_bytes);
-                bulk_g2s(ring_u32 + slot_i * row_bytes, src, (uint32_t)row_bytes, bar);
-            }
+            const bool second = PAIR && (isub & 1);
+            ring.issue(lane, 1, (uint32_t)row_bytes, [&](int) -> const uint8_t* {
+                const int pr = pairs[ic.pi], s = pr & 0xff;
+                if (s == p.slots) return reinterpret_cast<const uint8_t*>(second ? p.x1 : p.x0) + (long)ic.r * row_bytes;
+                const long e = pair_expert(p, t0 + (pr >> 8), s);
+                return reinterpret_cast<const uint8_t*>(second ? p.w1 : p.w0) + (e * p.rows + ic.r) * row_bytes;
+            });
             isub++;
-            if (!PAIR || !(isub & 1)) {
-                irr += W;
-                while (irr >= p.rows) { irr -= p.rows; ipi++; }
-            }
-            slot_i = (slot_i + 1 == SLOTS) ? 0 : slot_i + 1;
+            if (!PAIR || !(isub & 1)) ic.step(W, p.rows);
         }
     };
 #pragma unroll
     for (int s = 0; s < SLOTS; s++) issue_one();
 
-    {   // quantise the chunk's activation rows into the padded layout: block g = (token in chunk, block of the row)
-        float cur[8], nxt[8];
-        const int totalb = nt * nblk;
-        int g = warp;
-        if (g < totalb) load_block8(p.x, (long)(t0 + g / nblk) * p.ncols + (long)(g % nblk) * QK_K + lane * 8, p.hidden_type, cur);
-#pragma unroll 1
-        while (g < totalb) {
-            const int gn = g + W;
-            if (gn < totalb) load_block8(p.x, (long)(t0 + gn / nblk) * p.ncols + (long)(gn % nblk) * QK_K + lane * 8, p.hidden_type, nxt);
-            const int tl = g / nblk, b = g - tl * nblk;
-            uint8_t* at = smem + (size_t)tl * act_tok;
-            warp_quantize_q8k_block(cur, lane, reinterpret_cast<uint32_t*>(at + (size_t)b * kActBlkStride),
-                                    reinterpret_cast<float*>(at + (size_t)nblk * (kActBlkStride + 16)) + b, nullptr,
-                                    reinterpret_cast<int16_t*>(at + (size_t)nblk * kActBlkStride) + b * 8);
-#pragma unroll
-            for (int i = 0; i < 8; i++) cur[i] = nxt[i];
-            g = gn;
-        }
-    }
+    stage_q8k_rows<8>(p.x, p.hidden_type, t0, nt, p.ncols, smem, act_tok, lane, warp, W);
     __syncthreads();
 
     float acc_first = 0.f;
     for (int n = 0; n < nsub; n++) {
-        mbar_wait(bar_u32 + 8 * slot_u, (phase >> slot_u) & 1u);
-        phase ^= 1u << slot_u;
-        const uint8_t* row0 = ring + slot_u * row_bytes;
-        const int pr = pairs[cpi];
+        const uint8_t* row0 = ring.wait();
+        const int pr = pairs[cc.pi];
         const uint8_t* at = smem + (size_t)(pr >> 8) * act_tok;
         const int16_t* bs32 = reinterpret_cast<const int16_t*>(at + (size_t)nblk * kActBlkStride);
         const float* dx = reinterpret_cast<const float*>(at + (size_t)nblk * (kActBlkStride + 16));
@@ -221,8 +140,7 @@ __global__ void __launch_bounds__(kBulkMaxWarps * 32, 1) rows_bulk_q4k_kernel(co
         for (int blk = lane; blk < nblk; blk += 32)
             acc += q4k_block_dot(row0 + blk * SZ_Q4_K, at + (size_t)blk * kActBlkStride,
                                  *reinterpret_cast<const uint4*>(bs32 + blk * 8), dx[blk]);
-        __syncwarp();                       // every lane is done reading the slot: hand it back to the copy engine
-        slot_u = (slot_u + 1 == SLOTS) ? 0 : slot_u + 1;
+        ring.release();
         issue_one();
         if (PAIR && !(n & 1)) { acc_first = acc; continue; }
         float g = PAIR ? acc_first : acc, uu = acc;
@@ -232,39 +150,49 @@ __global__ void __launch_bounds__(kBulkMaxWarps * 32, 1) rows_bulk_q4k_kernel(co
             if (PAIR) uu += __shfl_xor_sync(0xffffffffu, uu, o);
         }
         if (lane == 0) {
-            const int oidx = (pr & 0xff) * p.rows + crr;
+            const int oidx = (pr & 0xff) * p.rows + cc.r;
             const long o = (long)(t0 + (pr >> 8)) * total_out + oidx;
             if (PAIR) {
                 p.out_f32[o] = (p.use_silu ? act_silu(g) : act_relu(g)) * uu;
             } else {
-                if (p.bias) g += p.bias[crr];
+                if (p.bias) g += p.bias[cc.r];
                 if (p.out_f32) p.out_f32[o] = g;
                 if (p.out_hidden) store_hidden(p.out_hidden, o, p.hidden_type, g);
             }
         }
-        crr += W;
-        while (crr >= p.rows) { crr -= p.rows; cpi++; }
+        cc.step(W, p.rows);
     }
   }  // token chunks
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // Item formats of the down-projection kernel.  An item is 4 consecutive rows x nb super-blocks, f = rw*nb + blk.
-struct BulkQ4K {   // raw Q4_K rows: block f of the item at f*144
+// BulkFmt holds the defaults of these formats and of the gate/up units of rows_bulk_iq_kernel (iq.cuh).
+struct BulkFmt {
+    static constexpr bool kFp32Act = false;   // true: the format stages fp32 activations itself (stage_act), not Q8_K
+    static constexpr bool kSharedSlot = true; // a shared expert of the format can ride in the routed launch as slot `slots`
+    static constexpr int kMinWarps = 2;       // reduce_bulk_kernel: fewer warps per CTA do not launch
+    static constexpr int kTableBytes = 0;     // static shared memory of the format's tables (iq.cuh)
+    __device__ static __forceinline__ void stage_tables() {}
+};
+// staged bytes per activation block of a down item format: padded int8 block, kBs int16 sums and scale; or the fp32 block
+template <class Fmt>
+constexpr int act_block_bytes() {
+    if constexpr (Fmt::kFp32Act) return Fmt::kActBytes;
+    else return kActBlkStride + 2 * Fmt::kBs + 4;
+}
+
+struct BulkQ4K : BulkFmt {   // raw Q4_K rows: block f of the item at f*144
     static constexpr int kBlockBytes = SZ_Q4_K;
     static constexpr int kBs = 8;   // int16 activation sums per block (32-value groups)
-    static constexpr int kTableBytes = 0;   // static shared memory of the format's tables (iq.cuh)
-    __device__ static __forceinline__ void stage_tables() {}
     __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int /*nrb*/, const uint8_t* aq, const int16_t* bs, float dxb) {
         return q4k_block_dot(sl + f * SZ_Q4_K, aq, *reinterpret_cast<const uint4*>(bs), dxb);
     }
 };
 
-struct BulkQ6K4T {   // chunk-major 4-row tiles (see the header comment)
+struct BulkQ6K4T : BulkFmt {   // chunk-major 4-row tiles (see the header comment)
     static constexpr int kBlockBytes = SZ_Q6_K;
     static constexpr int kBs = 16;  // int16 activation sums per block (16-value groups)
-    static constexpr int kTableBytes = 0;
-    __device__ static __forceinline__ void stage_tables() {}
     __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int nrb, const uint8_t* aq, const int16_t* bs, float dxb) {
         const uint8_t* ql = sl + f * 16;                  // chunk c at ql + c*nrb*16
         const uint8_t* qh = sl + nrb * 128 + f * 16;      // chunk c at qh + c*nrb*16
@@ -323,14 +251,11 @@ struct BulkQ6K4T {   // chunk-major 4-row tiles (see the header comment)
 // f * kBlockBytes) and the gate/up formats of rows_bulk_iq_kernel (iq.cuh).  No load-time re-layout: the grouped GEMM reads the
 // same tensors.  Value 128 n + 32 j + l (n < 2, j < 4, l < 32) is bits 2j..2j+1 of qs[32 n + l] and lies in 16-value group
 // g = 8 n + 2 j + (l >= 16).  Integer sums per super-block are exact; the fp32 finish is the grouped GEMM's (common.cuh).
-struct BulkQ2K {   // {scales[16] (scale | min << 4), qs[64], d, dmin} = 84 B: 4-byte aligned
+struct BulkQ2K : BulkFmt {   // {scales[16] (scale | min << 4), qs[64], d, dmin} = 84 B: 4-byte aligned
     static constexpr int kType = KTB200_TYPE_Q2_K;
     static constexpr int kBlockBytes = SZ_Q2_K;
     static constexpr int kBs = 16;          // the mins need the 16-value activation sums
-    static constexpr int kTableBytes = 0;
-    static constexpr bool kSharedSlot = true;   // rows_bulk_iq_kernel: a shared expert of this type can ride as slot `slots`
     static constexpr int kNblkMultiple = 4;
-    __device__ static __forceinline__ void stage_tables() {}
     // isum = sum_g sc_g * sum q * q8 (q 0..3), msum = sum_g m_g * bsum16_g
     __device__ static __forceinline__ float block_dot(const uint8_t* wb, const uint8_t* aq, const int16_t* bs16, float dxb) {
         const uint32_t* w = reinterpret_cast<const uint32_t*>(wb);
@@ -376,14 +301,11 @@ struct BulkQ2K {   // {scales[16] (scale | min << 4), qs[64], d, dmin} = 84 B: 4
     }
 };
 
-struct BulkQ3K {   // {hmask[32], qs[64], scales[12], d} = 110 B: 2-byte aligned, 4-byte aligned on even f
+struct BulkQ3K : BulkFmt {   // {hmask[32], qs[64], scales[12], d} = 110 B: 2-byte aligned, 4-byte aligned on even f
     static constexpr int kType = KTB200_TYPE_Q3_K;
     static constexpr int kBlockBytes = SZ_Q3_K;
     static constexpr int kBs = 8;           // staged, not read
-    static constexpr int kTableBytes = 0;
-    static constexpr bool kSharedSlot = true;
     static constexpr int kNblkMultiple = 4;
-    __device__ static __forceinline__ void stage_tables() {}
     // isum = sum_g (sc_g - 32) * sum (q - 4 [hmask bit clear]) * q8, the hmask term as a second dp4a on the clear bits.
     // Words are read as the grouped producer reads them: the aligned words covering the block, funnel-shifted by 16 bits when
     // the block starts mid-word.  The last word read (27) ends inside this block or the next one, which always exists: units
@@ -437,8 +359,8 @@ struct BulkQ3K {   // {hmask[32], qs[64], scales[12], d} = 110 B: 2-byte aligned
 // Tokens are processed in chunks: as many consecutive tokens as have, together, at most `pcap` (token, slot) pairs
 // owned by this launch (launcher: pcap >= slots + 1, so a chunk always holds at least one token).  Within a chunk all
 // pairs form ONE work list (expert-parallel shards and decode batches do not drain the ring per token) and all their
-// activation rows are staged as Q8_K side by side.
-constexpr int kBulkMaxChunkTokens = 16;
+// activation rows are staged side by side: as Q8_K, or as the format's fp32 blocks (Fmt::kFp32Act, RAWINT4).
+// Fmt::kSharedSlot = false compiles the shared-expert slot out.
 template <class Fmt, int SLOTS>
 __global__ void __launch_bounds__(kBulkMaxWarpsDown * 32, 1) reduce_bulk_kernel(const ReduceParams p, int nrows_max, int pcap) {
     constexpr int RW = 4;
@@ -451,131 +373,94 @@ __global__ void __launch_bounds__(kBulkMaxWarpsDown * 32, 1) reduce_bulk_kernel(
     if (p.bsz) Teff = min(Teff, *p.bsz);
     const int nb = p.ncols / QK_K;
     const int k = p.slots;
-    const int ns = k + (p.xw ? 1 : 0);
+    const int ns = k + (Fmt::kSharedSlot && p.xw ? 1 : 0);
     const int nrb = RW * nb;                                  // (row, block) pairs per item
     const int item_bytes = nrb * Fmt::kBlockBytes;
-    // staging: q8 [pcap][nb][272] | bs [pcap][nb][kBs] int16 | dx [pcap][nb] | partial [nrows_max][pcap] | pair list [pcap] | mbarriers | rings
+    // staging: activations [pcap][nb] | partial [nrows_max][pcap] | pair list [pcap] | ring.  Q8_K activations are
+    // q8 [pcap][nb][272] | bs [pcap][nb][kBs] int16 | dx [pcap][nb]; fp32 ones [pcap][nb][Fmt::kActBytes].
+    const size_t nab = (size_t)pcap * nb;
     uint8_t* q8 = smem;
-    int16_t* bs = reinterpret_cast<int16_t*>(smem + (size_t)pcap * nb * kActBlkStride);
-    float* dx = reinterpret_cast<float*>(smem + (size_t)pcap * nb * (kActBlkStride + 2 * Fmt::kBs));
-    float* partial = dx + (size_t)pcap * nb;
+    int16_t* bs = reinterpret_cast<int16_t*>(smem + nab * kActBlkStride);
+    float* dx = reinterpret_cast<float*>(smem + nab * (kActBlkStride + 2 * Fmt::kBs));
+    float* partial = reinterpret_cast<float*>(smem + nab * act_block_bytes<Fmt>());
     int* pairs = reinterpret_cast<int*>(partial + (size_t)nrows_max * pcap);   // (token in chunk) << 8 | slot
-    size_t off = (size_t)pcap * nb * (kActBlkStride + 2 * Fmt::kBs + 4) + (size_t)nrows_max * pcap * 4 + (size_t)pcap * 4;
-    off = (off + 15) & ~(size_t)15;
-    const int bar_bytes = (W * SLOTS * 8 + 15) & ~15;
-    const uint32_t bar_u32 = (uint32_t)__cvta_generic_to_shared(smem + off) + warp * SLOTS * 8;
-    uint8_t* ring = smem + off + bar_bytes + (size_t)warp * SLOTS * item_bytes;
-    const uint32_t ring_u32 = (uint32_t)__cvta_generic_to_shared(ring);
-    if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < SLOTS; s++) mbar_init(bar_u32 + 8 * s, 1);
-        mbar_fence_init();
-        fence_proxy_async_smem();
-    }
-    int slot_i = 0, slot_u = 0;
-    uint32_t phase = 0;
+    BulkRing<SLOTS> ring(smem, nab * act_block_bytes<Fmt>() + (size_t)nrows_max * pcap * 4 + (size_t)pcap * 4, item_bytes,
+                         lane, warp, W);
     const int quads = p.rows / RW;
     const int q0 = (int)((long)quads * blockIdx.x / gridDim.x), q1 = (int)((long)quads * (blockIdx.x + 1) / gridDim.x);
     const int r0 = q0 * RW, nquads = q1 - q0, nrows = nquads * RW;
 
   for (int t0 = 0; t0 < Teff;) {
     __syncthreads();
-    if (threadIdx.x == 0) {   // greedy chunk: tokens t0.. while their owned pairs fit
-        int np = 0, nt = 0;
-        while (t0 + nt < Teff && nt < kBulkMaxChunkTokens) {
-            const bool sh_here = p.xw && (p.shared_token < 0 || p.shared_token == t0 + nt);
-            int cnt = sh_here ? 1 : 0;
-            for (int j = 0; j < k; j++) {
-                const long e = p.ids ? (long)p.ids[(long)(t0 + nt) * k + j] - p.id_offset : 0;
-                cnt += (e >= 0 && e < p.n_experts) ? 1 : 0;
-            }
-            if (nt > 0 && np + cnt > pcap) break;
-            s_first[nt] = np;
-            for (int j = 0; j < k; j++) {
-                const long e = p.ids ? (long)p.ids[(long)(t0 + nt) * k + j] - p.id_offset : 0;
-                if (e >= 0 && e < p.n_experts) pairs[np++] = (nt << 8) | j;
-            }
-            if (sh_here) pairs[np++] = (nt << 8) | k;
-            nt++;
-        }
-        s_first[nt] = np;
+    if (threadIdx.x == 0) {
+        int np;
+        s_nt = down_pairs(p, t0, Teff, pcap, Fmt::kSharedSlot && p.xw, pairs, s_first, np);
         s_np = np;
-        s_nt = nt;
     }
     __syncthreads();
     const int np = s_np, nt = s_nt;
-    const int total = nquads * np;   // item = pair * nquads + quad
-    int ni = total - warp;
-    ni = ni > 0 ? (ni + W - 1) / W : 0;
-    int ipi = 0, iq = 0, iss = 0;
-    if (ni > 0) { ipi = warp / nquads; iq = warp - ipi * nquads; }
-    int cpi = ipi, cq = iq;
+    const int ni = warp_units(0, nquads * np, warp, W);   // item = pair * nquads + quad
+    UnitCursor ic;
+    if (ni > 0) ic.start(warp, nquads);
+    UnitCursor cc = ic;
+    int iss = 0;
 
     auto issue_one = [&]() {
         if (iss < ni) {
-            if (lane == 0) {
-                const int pr = pairs[ipi], j = pr & 0xff;
-                long row = r0 + iq * RW;
+            ring.issue(lane, 1, (uint32_t)item_bytes, [&](int) {
+                const int pr = pairs[ic.pi], j = pr & 0xff;
+                long row = r0 + ic.r * RW;
                 const uint8_t* wbase = reinterpret_cast<const uint8_t*>(p.w);
-                if (j == k) wbase = reinterpret_cast<const uint8_t*>(p.xw);
-                else row += (p.ids ? (long)p.ids[(long)(t0 + (pr >> 8)) * k + j] - p.id_offset : 0L) * p.rows;
-                const uint8_t* src = wbase + (row >> 2) * item_bytes;
-                const uint32_t bar = bar_u32 + 8 * slot_i;
-                mbar_expect_tx(bar, (uint32_t)item_bytes);
-                bulk_g2s(ring_u32 + slot_i * item_bytes, src, (uint32_t)item_bytes, bar);
-            }
+                if (Fmt::kSharedSlot && j == k) wbase = reinterpret_cast<const uint8_t*>(p.xw);
+                else row += pair_expert(p, t0 + (pr >> 8), j) * p.rows;
+                return wbase + (row >> 2) * item_bytes;
+            });
             iss++;
-            iq += W;
-            while (iq >= nquads) { iq -= nquads; ipi++; }
-            slot_i = (slot_i + 1 == SLOTS) ? 0 : slot_i + 1;
+            ic.step(W, nquads);
         }
     };
 #pragma unroll
     for (int s = 0; s < SLOTS; s++) issue_one();
 
-    {   // quantise the pairs' activation rows (fp32 phase-1 output) into the padded layout: block g = (pair, block)
-        float cur[8], nxt[8];
-        const int totalb = np * nb;
-        auto src_of = [&](int g) -> long {
-            const int pi = g / nb, b = g - pi * nb, pr = pairs[pi];
-            return ((long)(t0 + (pr >> 8)) * ns + (pr & 0xff)) * p.ncols + (long)b * QK_K + lane * 8;
-        };
-        int g = warp;
-        if (g < totalb) load_block8(p.a, src_of(g), KTB200_TYPE_F32, cur);
-#pragma unroll 1
-        while (g < totalb) {
-            const int gn = g + W;
-            if (gn < totalb) load_block8(p.a, src_of(gn), KTB200_TYPE_F32, nxt);
-            warp_quantize_q8k_block(cur, lane, reinterpret_cast<uint32_t*>(q8 + (size_t)g * kActBlkStride), dx + g,
-                                    Fmt::kBs == 16 ? bs + g * 16 : nullptr, Fmt::kBs == 8 ? bs + g * 8 : nullptr);
-#pragma unroll
-            for (int i = 0; i < 8; i++) cur[i] = nxt[i];
-            g = gn;
-        }
+    // the pairs' activation rows (fp32 phase-1 output)
+    auto src_row = [&](int pi) {
+        const int pr = pairs[pi];
+        return ((long)(t0 + (pr >> 8)) * ns + (pr & 0xff)) * p.ncols;
+    };
+    if constexpr (Fmt::kFp32Act) {
+        Fmt::stage_act(smem, p.a, np, p.ncols, src_row);
+    } else {   // block g = (pair, block)
+        stage_q8k<Fmt::kBs>(
+            p.a, KTB200_TYPE_F32, np * nb, lane, warp, W,
+            [&](int g) {
+                const int pi = g / nb, b = g - pi * nb;
+                return src_row(pi) + (long)b * QK_K;
+            },
+            [&](int g) { return StagedBlock{q8 + (size_t)g * kActBlkStride, bs + g * Fmt::kBs, dx + g}; });
     }
     __syncthreads();
 
     for (int n = 0; n < ni; n++) {
-        mbar_wait(bar_u32 + 8 * slot_u, (phase >> slot_u) & 1u);
-        phase ^= 1u << slot_u;
-        const uint8_t* sl = ring + slot_u * item_bytes;
+        const uint8_t* sl = ring.wait();
         float res;
         {
             float acc[RW] = {0.f, 0.f, 0.f, 0.f};
             for (int f = lane; f < nrb; f += 32) {   // (row, block) pairs of the tile; 4 x 8 = one per lane for I = 2048
                 const int rw = f / nb, blk = f - rw * nb;
-                const int ab = cpi * nb + blk;
-                const float val = Fmt::dot(sl, f, nrb, q8 + (size_t)ab * kActBlkStride, bs + ab * Fmt::kBs, dx[ab]);
+                const int ab = cc.pi * nb + blk;
+                float val;
+                if constexpr (Fmt::kFp32Act)
+                    val = Fmt::dot(sl, f, reinterpret_cast<const float*>(smem) + (size_t)ab * (Fmt::kActBytes / 4));
+                else
+                    val = Fmt::dot(sl, f, nrb, q8 + (size_t)ab * kActBlkStride, bs + ab * Fmt::kBs, dx[ab]);
                 acc[0] += rw == 0 ? val : 0.f; acc[1] += rw == 1 ? val : 0.f; acc[2] += rw == 2 ? val : 0.f; acc[3] += rw == 3 ? val : 0.f;
             }
             res = warp_reduce4(acc[0], acc[1], acc[2], acc[3], lane);
         }
-        __syncwarp();
-        slot_u = (slot_u + 1 == SLOTS) ? 0 : slot_u + 1;
+        ring.release();
         issue_one();
-        if ((lane & 7) == 0) partial[(cq * RW + (lane >> 3)) * pcap + cpi] = res;
-        cq += W;
-        while (cq >= nquads) { cq -= nquads; cpi++; }
+        if ((lane & 7) == 0) partial[(cc.r * RW + (lane >> 3)) * pcap + cc.pi] = res;
+        cc.step(W, nquads);
     }
     __syncthreads();
     // weighted accumulation over a token's experts IN expert_ids ORDER (moe.cpp:222-236), one FMA per expert
@@ -586,14 +471,16 @@ __global__ void __launch_bounds__(kBulkMaxWarpsDown * 32, 1) reduce_bulk_kernel(
         for (int pi = s_first[tl]; pi < s_first[tl + 1]; pi++) {
             const int j = pairs[pi] & 0xff;
             const float dv = partial[hl * pcap + pi];
-            if (j == k) shared = dv;
+            if (Fmt::kSharedSlot && j == k) shared = dv;
             else acc = p.weights ? __fmaf_rn(dv, p.weights[t * k + j], acc) : acc + dv;
         }
         const long o = t * p.rows + r0 + hl;
-        bool has_sh = false;
-        for (int pi = s_first[tl]; pi < s_first[tl + 1]; pi++) has_sh |= (pairs[pi] & 0xff) == k;
-        if (p.xw_out) { if (has_sh) store_hidden(p.xw_out, o, p.xw_out_type, shared); }
-        else if (p.xw) acc = round_hidden(acc, p.hidden_type) + round_hidden(shared, p.hidden_type);
+        if constexpr (Fmt::kSharedSlot) {
+            bool has_sh = false;
+            for (int pi = s_first[tl]; pi < s_first[tl + 1]; pi++) has_sh |= (pairs[pi] & 0xff) == k;
+            if (p.xw_out) { if (has_sh) store_hidden(p.xw_out, o, p.xw_out_type, shared); }
+            else if (p.xw) acc = round_hidden(acc, p.hidden_type) + round_hidden(shared, p.hidden_type);
+        }
         if (p.accumulate) acc = load_hidden(p.out, o, p.hidden_type) + round_hidden(acc, p.hidden_type);
         store_hidden(p.out, o, p.hidden_type, acc);
     }

@@ -31,7 +31,7 @@ __device__ __forceinline__ uint32_t lds_u32_a2(const uint8_t* p) {
     return (uint32_t)h[0] | ((uint32_t)h[1] << 16);
 }
 
-struct BulkIQ1S {
+struct BulkIQ1S : BulkFmt {
     static constexpr int kType = KTB200_TYPE_IQ1_S;
     static constexpr int kBlockBytes = SZ_IQ1_S;
     static constexpr int kBs = 8;            // int16 activation sums per block (32-value groups)
@@ -79,7 +79,7 @@ struct BulkIQ1S {
 // IQ1_S's codebook with the scale per 16 values and the delta per 8.  The Q8_K sums cover 16 or 32 values, so the delta term is
 // summed per 8-value group: dp4a of the group's activations against 0x01010101 (+1) or 0xffffffff (-1).  56-byte blocks are
 // 8-byte aligned: words and the 8-byte scale field load whole.
-struct BulkIQ1M {
+struct BulkIQ1M : BulkFmt {
     static constexpr int kType = KTB200_TYPE_IQ1_M;
     static constexpr int kBlockBytes = SZ_IQ1_M;
     static constexpr int kBs = 8;            // staged, not read
@@ -121,7 +121,7 @@ struct BulkIQ1M {
     }
 };
 
-struct BulkIQ2XXS {
+struct BulkIQ2XXS : BulkFmt {
     static constexpr int kType = KTB200_TYPE_IQ2_XXS;
     static constexpr int kBlockBytes = SZ_IQ2_XXS;
     static constexpr int kBs = 8;
@@ -178,98 +178,48 @@ __global__ void __launch_bounds__(kIqMaxWarps * 32, 1) rows_bulk_iq_kernel(const
     const int nblk = p.ncols / QK_K;
     const int row_bytes = nblk * Fmt::kBlockBytes;
     const int unit_bytes = 2 * row_bytes;             // rows 2r, 2r+1 of one matrix
-    const int slot_bytes = 2 * unit_bytes;            // gate unit | up unit
     const int nru = p.rows / 2;                       // row pairs per matrix
     const int nslots = p.slots + (Fmt::kSharedSlot && p.x0 ? 1 : 0);
     const int total_out = nslots * p.rows;
-    // [tc activation rows: q8 [nblk][272] | bs [nblk][kBs] int16 | dx [nblk]] [pair list] [mbarriers] [rings]
+    // [tc activation rows: q8 [nblk][272] | bs [nblk][kBs] int16 | dx [nblk]] [pair list] [ring: slot = gate unit | up unit]
     int* pairs = reinterpret_cast<int*>(smem + (size_t)tc * act_tok);
-    // (p.slots spelled out, and the staging offsets below written per kBs, keep the i-quant instantiations' code as it was)
-    const size_t off = ((size_t)tc * act_tok + (size_t)tc * (Fmt::kSharedSlot ? nslots : p.slots) * 4 + 15) & ~(size_t)15;
-    const int bar_bytes = (W * SLOTS * 8 + 15) & ~15;
-    const uint32_t bar_u32 = (uint32_t)__cvta_generic_to_shared(smem + off) + warp * SLOTS * 8;
-    uint8_t* ring = smem + off + bar_bytes + (size_t)warp * SLOTS * slot_bytes;
-    const uint32_t ring_u32 = (uint32_t)__cvta_generic_to_shared(ring);
-    if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < SLOTS; s++) mbar_init(bar_u32 + 8 * s, 1);
-        mbar_fence_init();
-        fence_proxy_async_smem();
-    }
-    int slot_i = 0, slot_u = 0;
-    uint32_t phase = 0;
+    BulkRing<SLOTS> ring(smem, (size_t)tc * act_tok + (size_t)tc * nslots * 4, 2 * unit_bytes, lane, warp, W);
 
   for (int t0 = 0; t0 < Teff; t0 += tc) {
     const int nt = min(tc, Teff - t0);
     __syncthreads();
-    if (threadIdx.x == 0) {
-        int np = 0;
-        for (int tl = 0; tl < nt; tl++) {
-            for (int s = 0; s < p.slots; s++) {
-                const long e = (long)p.ids[(long)(t0 + tl) * p.slots + s] - p.id_offset;
-                if (e >= 0 && e < p.n_experts) pairs[np++] = (tl << 8) | s;
-            }
-            if (Fmt::kSharedSlot && p.x0) pairs[np++] = (tl << 8) | p.slots;
-        }
-        s_np = np;
-    }
+    if (threadIdx.x == 0) s_np = gateup_pairs(p, t0, nt, Fmt::kSharedSlot && p.x0, pairs);
     __syncthreads();
     const int total = s_np * nru;
     const int u0 = (int)((long)total * blockIdx.x / gridDim.x), u1 = (int)((long)total * (blockIdx.x + 1) / gridDim.x);
-    int nu = u1 - u0 - warp;
-    nu = nu > 0 ? (nu + W - 1) / W : 0;
-    int ipi = 0, iru = 0, iss = 0;
-    if (nu > 0) { ipi = (u0 + warp) / nru; iru = (u0 + warp) - ipi * nru; }
-    int cpi = ipi, cru = iru;
+    const int nu = warp_units(u0, u1, warp, W);
+    UnitCursor ic;
+    if (nu > 0) ic.start(u0 + warp, nru);
+    UnitCursor cc = ic;
+    int iss = 0;
 
     auto issue_one = [&]() {
         if (iss < nu) {
-            if (lane == 0) {
-                const int pr = pairs[ipi];
+            ring.issue(lane, 2, (uint32_t)unit_bytes, [&](int c) {
+                const int pr = pairs[ic.pi];
                 const bool sh = Fmt::kSharedSlot && (pr & 0xff) == p.slots;
-                const long e = sh ? 0L : (long)p.ids[(long)(t0 + (pr >> 8)) * p.slots + (pr & 0xff)] - p.id_offset;
-                const long first = (e * p.rows + 2L * iru) * row_bytes;
-                const uint32_t bar = bar_u32 + 8 * slot_i, dst = ring_u32 + slot_i * slot_bytes;
-                mbar_expect_tx(bar, (uint32_t)slot_bytes);
-                bulk_g2s(dst, reinterpret_cast<const uint8_t*>(sh ? p.x0 : p.w0) + first, (uint32_t)unit_bytes, bar);
-                bulk_g2s(dst + unit_bytes, reinterpret_cast<const uint8_t*>(sh ? p.x1 : p.w1) + first, (uint32_t)unit_bytes, bar);
-            }
+                const long e = sh ? 0L : pair_expert(p, t0 + (pr >> 8), pr & 0xff);
+                const void* w = sh ? (c ? p.x1 : p.x0) : (c ? p.w1 : p.w0);
+                return reinterpret_cast<const uint8_t*>(w) + (e * p.rows + 2L * ic.r) * row_bytes;
+            });
             iss++;
-            iru += W;
-            while (iru >= nru) { iru -= nru; ipi++; }
-            slot_i = (slot_i + 1 == SLOTS) ? 0 : slot_i + 1;
+            ic.step(W, nru);
         }
     };
 #pragma unroll
     for (int s = 0; s < SLOTS; s++) issue_one();
 
-    {   // quantise the chunk's activation rows into the padded layout (as rows_bulk_q4k_kernel)
-        float cur[8], nxt[8];
-        const int totalb = nt * nblk;
-        int g = warp;
-        if (g < totalb) load_block8(p.x, (long)(t0 + g / nblk) * p.ncols + (long)(g % nblk) * QK_K + lane * 8, p.hidden_type, cur);
-#pragma unroll 1
-        while (g < totalb) {
-            const int gn = g + W;
-            if (gn < totalb) load_block8(p.x, (long)(t0 + gn / nblk) * p.ncols + (long)(gn % nblk) * QK_K + lane * 8, p.hidden_type, nxt);
-            const int tl = g / nblk, b = g - tl * nblk;
-            uint8_t* at = smem + (size_t)tl * act_tok;
-            warp_quantize_q8k_block(cur, lane, reinterpret_cast<uint32_t*>(at + (size_t)b * kActBlkStride),
-                                    reinterpret_cast<float*>(at + (size_t)nblk * (kActBlkStride + 2 * Fmt::kBs)) + b,
-                                    Fmt::kBs == 16 ? reinterpret_cast<int16_t*>(at + (size_t)nblk * kActBlkStride) + b * 16 : nullptr,
-                                    Fmt::kBs == 8 ? reinterpret_cast<int16_t*>(at + (size_t)nblk * kActBlkStride) + b * 8 : nullptr);
-#pragma unroll
-            for (int i = 0; i < 8; i++) cur[i] = nxt[i];
-            g = gn;
-        }
-    }
+    stage_q8k_rows<Fmt::kBs>(p.x, p.hidden_type, t0, nt, p.ncols, smem, act_tok, lane, warp, W);
     __syncthreads();
 
     for (int n = 0; n < nu; n++) {
-        mbar_wait(bar_u32 + 8 * slot_u, (phase >> slot_u) & 1u);
-        phase ^= 1u << slot_u;
-        const uint8_t* sl = ring + slot_u * slot_bytes;
-        const int pr = pairs[cpi];
+        const uint8_t* sl = ring.wait();
+        const int pr = pairs[cc.pi];
         const uint8_t* at = smem + (size_t)(pr >> 8) * act_tok;
         const int16_t* bs = reinterpret_cast<const int16_t*>(at + (size_t)nblk * kActBlkStride);
         const float* dx = reinterpret_cast<const float*>(at + (size_t)nblk * (kActBlkStride + 2 * Fmt::kBs));
@@ -282,16 +232,14 @@ __global__ void __launch_bounds__(kIqMaxWarps * 32, 1) rows_bulk_iq_kernel(const
             if (rw) { g1 += g; v1 += u; } else { g0 += g; v0 += u; }
         }
         const float r = warp_reduce4(g0, g1, v0, v1, lane);   // lane 0: g0, 8: g1, 16: u0, 24: u1
-        __syncwarp();
-        slot_u = (slot_u + 1 == SLOTS) ? 0 : slot_u + 1;
+        ring.release();
         issue_one();
         const float gs = __shfl_sync(0xffffffffu, r, 8 * (lane & 1)), us = __shfl_sync(0xffffffffu, r, 16 + 8 * (lane & 1));
         if (lane < 2) {
-            const long o = (long)(t0 + (pr >> 8)) * total_out + (long)(pr & 0xff) * p.rows + 2L * cru + lane;
+            const long o = (long)(t0 + (pr >> 8)) * total_out + (long)(pr & 0xff) * p.rows + 2L * cc.r + lane;
             p.out_f32[o] = (p.use_silu ? act_silu(gs) : act_relu(gs)) * us;
         }
-        cru += W;
-        while (cru >= nru) { cru -= nru; cpi++; }
+        cc.step(W, nru);
     }
   }  // token chunks
 }

@@ -145,9 +145,10 @@ static int grid_x(long units, int device) {
 
 // Shared-memory plan of a bulk-copy ring kernel (gemv_bulk.cuh, dense_bulk.cuh, iq.cuh, rawint4.cuh): a head of `chunk`
 // staged units (tokens for gate/up, (token, slot) pairs for down) of `unit_bytes` each, padded to 16 bytes, then W warps of
-// `slots` ring slots of `slot_bytes` with an 8-byte mbarrier per slot, within the opt-in limit less the format's static
-// tables (`table_bytes`).  The chunk is the largest in [lo, hi] whose head leaves room for `room_warps` warps plus `spare`
-// bytes (lo when none does); W is as many warps as fit next to it, at most max_warps.  W = 0: fewer than min_warps fit.
+// `slots` ring slots of `slot_bytes` with an 8-byte mbarrier per slot — the layout BulkRing (bulk_ring.cuh) places; a change
+// there is a change here — within the opt-in limit less the format's static tables (`table_bytes`).  The chunk is the
+// largest in [lo, hi] whose head leaves room for `room_warps` warps plus `spare` bytes (lo when none does); W is as many
+// warps as fit next to it, at most max_warps.  W = 0: fewer than min_warps fit.
 struct RingPlan { int chunk, W; size_t smem; };
 static RingPlan plan_ring(size_t unit_bytes, int lo, int hi, int room_warps, size_t spare, size_t slot_bytes, int slots,
                           int min_warps, int max_warps, int table_bytes) {
@@ -409,7 +410,7 @@ static int launch_reduce_pipe_q6k8(const ReduceParams& p, int T, int device, cud
     return KTB200_OK;
 }
 
-// Plan of the bulk-copy down kernels (reduce_bulk_kernel, reduce_bulk_i4_kernel): one CTA per SM over 4-row items of
+// Plan of the bulk-copy down kernel (reduce_bulk_kernel): one CTA per SM over 4-row items of
 // `item` bytes; a token chunk stages `pcap` (token, slot) pairs of `act_pair` activation bytes and a partial sum per row.
 // pcap: one token's worth (ns) at least; up to 2 tokens' worth (<= 18) when several tokens share the launch and >= 10
 // warps still fit.  W = 0: does not fit.
@@ -438,9 +439,10 @@ static DownPlan plan_down(int rows, int nb, int ns, int T, size_t act_pair, size
 template <class Fmt>
 static int launch_reduce_bulk(const ReduceParams& p, int T, int device, cudaStream_t stream) {
     constexpr int S = 2;
+    if (p.xw && !Fmt::kSharedSlot) return 1;   // the instantiation has no shared-expert slot code
     const int nb = p.ncols / QK_K;
-    const DownPlan d = plan_down(p.rows, nb, p.slots + (p.xw ? 1 : 0), T, (size_t)nb * (kActBlkStride + 2 * Fmt::kBs + 4),
-                                 (size_t)4 * nb * Fmt::kBlockBytes, S, 2, Fmt::kTableBytes, device);
+    const DownPlan d = plan_down(p.rows, nb, p.slots + (p.xw ? 1 : 0), T, (size_t)nb * act_block_bytes<Fmt>(),
+                                 (size_t)4 * nb * Fmt::kBlockBytes, S, Fmt::kMinWarps, Fmt::kTableBytes, device);
     if (!d.W) return 1;
     KTB_CUDA_CHECK(cudaFuncSetAttribute(reduce_bulk_kernel<Fmt, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d.smem));
     reduce_bulk_kernel<Fmt, S><<<d.gx, d.W * 32, d.smem, stream>>>(p, d.nrows_max, d.pcap);
@@ -455,27 +457,19 @@ static bool q6k4t_eligible(int rows, int ncols, int ns_max, int device) {
     const int nb = ncols / QK_K;
     if (nb % 2 || rows % 4) return false;
     using F = BulkQ6K4T;
-    return plan_down(rows, nb, ns_max, 1, (size_t)nb * (kActBlkStride + 2 * F::kBs + 4), (size_t)4 * nb * F::kBlockBytes,
+    return plan_down(rows, nb, ns_max, 1, (size_t)nb * act_block_bytes<F>(), (size_t)4 * nb * F::kBlockBytes,
                      kQ6K4TPlanSlots, 4, F::kTableBytes, device).W > 0;
-}
-
-// RAWINT4 down projection (reduce_bulk_i4_kernel): the only kernel for the format, so a shape it cannot take is an error.
-static int launch_reduce_i4(const ReduceParams& p, int T, int device, cudaStream_t stream) {
-    constexpr int S = 2;
-    if (p.xw) { set_error("RAWINT4 down: the shared expert cannot ride in the routed launch"); return KTB200_EINVAL; }
-    const int nb = p.ncols / QK_K;
-    const DownPlan d = plan_down(p.rows, nb, p.slots, T, (size_t)nb * kI4ActStride, (size_t)4 * nb * SZ_RAWINT4, S, 1, 0, device);
-    if (!d.W) { set_error("RAWINT4 down: k=%d x intermediate_size=%d does not fit shared memory", p.slots, p.ncols); return KTB200_EINVAL; }
-    KTB_CUDA_CHECK(cudaFuncSetAttribute(reduce_bulk_i4_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d.smem));
-    reduce_bulk_i4_kernel<S><<<d.gx, d.W * 32, d.smem, stream>>>(p, d.nrows_max, d.pcap);
-    KTB_LAUNCH_CHECK();
-    return KTB200_OK;
 }
 
 static int launch_reduce(FmtId f, const ReduceParams& p_in, int T, int device, cudaStream_t stream) {
     ReduceParams p = p_in;
     p.ntokens = T;
-    if (f == FMT_RAWINT4) return launch_reduce_i4(p, T, device, stream);
+    if (f == FMT_RAWINT4) {   // the only kernel for the format, so a launch it cannot take is an error
+        if (p.xw) { set_error("RAWINT4 down: the shared expert cannot ride in the routed launch"); return KTB200_EINVAL; }
+        const int rc = launch_reduce_bulk<BulkI4>(p, T, device, stream);
+        if (rc == 1) { set_error("RAWINT4 down: k=%d x intermediate_size=%d does not fit shared memory", p.slots, p.ncols); return KTB200_EINVAL; }
+        return rc;
+    }
     if (f == FMT_Q6K4T) {
         const int rc = launch_reduce_bulk<BulkQ6K4T>(p, T, device, stream);
         if (rc == 1) { set_error("Q6_K tile layout: k=%d x ncols=%d does not fit the bulk kernel", p.slots, p.ncols); return KTB200_EINVAL; }

@@ -115,6 +115,28 @@ __device__ __forceinline__ void i4_stage(float* dst, const void* x, int hidden_t
     }
 }
 
+// Down item format of reduce_bulk_kernel: 4 rows x nb raw super-blocks, block f at f * 144.  The fp32 intermediate rows `a`
+// of a chunk's pairs are staged unchanged (not requantised), and a RAWINT4 down projection never carries the shared expert.
+struct BulkI4 : BulkFmt {
+    static constexpr int kBlockBytes = SZ_RAWINT4;
+    static constexpr int kBs = 0;
+    static constexpr bool kFp32Act = true;
+    static constexpr int kActBytes = kI4ActStride;
+    static constexpr bool kSharedSlot = false;
+    static constexpr int kMinWarps = 1;
+    // rows 0 .. n-1 of `a` (fp32), src(r) = element offset of row r, as [n][nb] padded blocks
+    template <class SrcFn>
+    __device__ static __forceinline__ void stage_act(uint8_t* dst, const void* a, int n, int ncols, SrcFn&& src) {
+        i4_stage(reinterpret_cast<float*>(dst), a, KTB200_TYPE_F32, n, ncols, src);
+    }
+    __device__ static __forceinline__ float dot(const uint8_t* sl, int f, const float* xb) {
+        const uint8_t* const wb[1] = {sl + f * SZ_RAWINT4};
+        float v[1] = {0.f};
+        i4_block_dot<1>(wb, xb, v);
+        return v[0];
+    }
+};
+
 // ---------------------------------------------------------------------------------------------------------------
 // Gate/up rows + silu(g) * u.  One ring slot = the gate row AND the up row of one (pair, row) unit (two bulk copies on
 // one mbarrier), so a lane reads its 256 activations once for both matrices.  Otherwise the work split of
@@ -131,58 +153,32 @@ __global__ void __launch_bounds__(kBulkMaxWarps * 32, 1) rows_bulk_i4_kernel(con
     const int row_bytes = nblk * SZ_RAWINT4;
     const int act_tok = nblk * kI4ActStride;
     const int total_out = p.slots * p.rows;
-    // [tc activation rows, fp32 padded] [pair list: tc*slots ints] [mbarriers] [rings: W x SLOTS x (gate row | up row)]
+    // [tc activation rows, fp32 padded] [pair list: tc*slots ints] [ring: slot = gate row | up row]
     int* pairs = reinterpret_cast<int*>(smem + (size_t)tc * act_tok);   // (token in chunk) << 8 | slot
-    const size_t off = ((size_t)tc * act_tok + (size_t)tc * p.slots * 4 + 15) & ~(size_t)15;
-    const int bar_bytes = (W * SLOTS * 8 + 15) & ~15;
-    const uint32_t bar_u32 = (uint32_t)__cvta_generic_to_shared(smem + off) + warp * SLOTS * 8;
-    uint8_t* ring = smem + off + bar_bytes + (size_t)warp * SLOTS * 2 * row_bytes;
-    const uint32_t ring_u32 = (uint32_t)__cvta_generic_to_shared(ring);
-    if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < SLOTS; s++) mbar_init(bar_u32 + 8 * s, 1);
-        mbar_fence_init();
-        fence_proxy_async_smem();
-    }
-    int slot_i = 0, slot_u = 0;
-    uint32_t phase = 0;
+    BulkRing<SLOTS> ring(smem, (size_t)tc * act_tok + (size_t)tc * p.slots * 4, 2 * row_bytes, lane, warp, W);
 
   for (int t0 = 0; t0 < Teff; t0 += tc) {
     const int nt = min(tc, Teff - t0);
     __syncthreads();
-    if (threadIdx.x == 0) {
-        int np = 0;
-        for (int tl = 0; tl < nt; tl++)
-            for (int s = 0; s < p.slots; s++) {
-                const long e = p.ids ? (long)p.ids[(long)(t0 + tl) * p.slots + s] - p.id_offset : 0;
-                if (e >= 0 && e < p.n_experts) pairs[np++] = (tl << 8) | s;
-            }
-        s_np = np;
-    }
+    if (threadIdx.x == 0) s_np = gateup_pairs(p, t0, nt, false, pairs);
     __syncthreads();
     const int total = s_np * p.rows;
     const int u0 = (int)((long)total * blockIdx.x / gridDim.x), u1 = (int)((long)total * (blockIdx.x + 1) / gridDim.x);
-    int nu = u1 - u0 - warp;
-    nu = nu > 0 ? (nu + W - 1) / W : 0;
-    int ipi = 0, irr = 0, iu = 0;
-    if (nu > 0) { ipi = (u0 + warp) / p.rows; irr = (u0 + warp) - ipi * p.rows; }
-    int cpi = ipi, crr = irr;
+    const int nu = warp_units(u0, u1, warp, W);
+    UnitCursor ic;
+    if (nu > 0) ic.start(u0 + warp, p.rows);
+    UnitCursor cc = ic;
+    int iu = 0;
 
     auto issue_one = [&]() {
         if (iu < nu) {
-            if (lane == 0) {
-                const int pr = pairs[ipi], s = pr & 0xff, tl = pr >> 8;
-                const long e = p.ids ? (long)p.ids[(long)(t0 + tl) * p.slots + s] - p.id_offset : 0;
-                const long ro = (e * p.rows + irr) * row_bytes;
-                const uint32_t bar = bar_u32 + 8 * slot_i, dst = ring_u32 + slot_i * 2 * row_bytes;
-                mbar_expect_tx(bar, (uint32_t)(2 * row_bytes));
-                bulk_g2s(dst, reinterpret_cast<const uint8_t*>(p.w0) + ro, (uint32_t)row_bytes, bar);
-                bulk_g2s(dst + row_bytes, reinterpret_cast<const uint8_t*>(p.w1) + ro, (uint32_t)row_bytes, bar);
-            }
+            ring.issue(lane, 2, (uint32_t)row_bytes, [&](int c) {
+                const int pr = pairs[ic.pi];
+                const long e = pair_expert(p, t0 + (pr >> 8), pr & 0xff);
+                return reinterpret_cast<const uint8_t*>(c ? p.w1 : p.w0) + (e * p.rows + ic.r) * row_bytes;
+            });
             iu++;
-            irr += W;
-            while (irr >= p.rows) { irr -= p.rows; ipi++; }
-            slot_i = (slot_i + 1 == SLOTS) ? 0 : slot_i + 1;
+            ic.step(W, p.rows);
         }
     };
 #pragma unroll
@@ -192,18 +188,15 @@ __global__ void __launch_bounds__(kBulkMaxWarps * 32, 1) rows_bulk_i4_kernel(con
     __syncthreads();
 
     for (int n = 0; n < nu; n++) {
-        mbar_wait(bar_u32 + 8 * slot_u, (phase >> slot_u) & 1u);
-        phase ^= 1u << slot_u;
-        const uint8_t* row0 = ring + slot_u * 2 * row_bytes;
-        const int pr = pairs[cpi];
+        const uint8_t* row0 = ring.wait();
+        const int pr = pairs[cc.pi];
         const float* xt = reinterpret_cast<const float*>(smem + (size_t)(pr >> 8) * act_tok);
         float acc[2] = {0.f, 0.f};
         for (int blk = lane; blk < nblk; blk += 32) {
             const uint8_t* const wb[2] = {row0 + blk * SZ_RAWINT4, row0 + row_bytes + blk * SZ_RAWINT4};
             i4_block_dot<2>(wb, xt + blk * (kI4ActStride / 4), acc);
         }
-        __syncwarp();                       // every lane is done reading the slot: hand it back to the copy engine
-        slot_u = (slot_u + 1 == SLOTS) ? 0 : slot_u + 1;
+        ring.release();
         issue_one();
         float g = acc[0], uu = acc[1];
 #pragma unroll
@@ -212,150 +205,11 @@ __global__ void __launch_bounds__(kBulkMaxWarps * 32, 1) rows_bulk_i4_kernel(con
             uu += __shfl_xor_sync(0xffffffffu, uu, o);
         }
         if (lane == 0) {
-            const long o = (long)(t0 + (pr >> 8)) * total_out + (pr & 0xff) * p.rows + crr;
+            const long o = (long)(t0 + (pr >> 8)) * total_out + (pr & 0xff) * p.rows + cc.r;
             p.out_f32[o] = (p.use_silu ? act_silu(g) : act_relu(g)) * uu;
         }
-        crr += W;
-        while (crr >= p.rows) { crr -= p.rows; cpi++; }
+        cc.step(W, p.rows);
     }
-  }  // token chunks
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Down projection + weighted combine over experts.  Work item of a warp = (pair, 4 consecutive output rows) = one bulk
-// copy of 4 * nb raw super-blocks; lane f = rw * nb + blk.  The fp32 intermediate rows `a` of a chunk's pairs are
-// staged unchanged (not requantised).  Work split, chunking and the combine in expert_ids order are those of
-// reduce_bulk_kernel.
-template <int SLOTS>
-__global__ void __launch_bounds__(kBulkMaxWarpsDown * 32, 1) reduce_bulk_i4_kernel(const ReduceParams p, int nrows_max, int pcap) {
-    constexpr int RW = 4;
-    extern __shared__ __align__(16) uint8_t smem[];
-    __shared__ int s_np, s_nt;
-    __shared__ int s_first[kBulkMaxChunkTokens + 1];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, W = blockDim.x >> 5;
-    int Teff = p.ntokens;
-    if (p.bsz) Teff = min(Teff, *p.bsz);
-    const int nb = p.ncols / QK_K;
-    const int k = p.slots;
-    const int nrb = RW * nb;
-    const int item_bytes = nrb * SZ_RAWINT4;
-    // staging: a [pcap][nb][1040 B] | partial [nrows_max][pcap] | pair list [pcap] | mbarriers | rings
-    float* act = reinterpret_cast<float*>(smem);
-    float* partial = reinterpret_cast<float*>(smem + (size_t)pcap * nb * kI4ActStride);
-    int* pairs = reinterpret_cast<int*>(partial + (size_t)nrows_max * pcap);
-    size_t off = (size_t)pcap * nb * kI4ActStride + (size_t)nrows_max * pcap * 4 + (size_t)pcap * 4;
-    off = (off + 15) & ~(size_t)15;
-    const int bar_bytes = (W * SLOTS * 8 + 15) & ~15;
-    const uint32_t bar_u32 = (uint32_t)__cvta_generic_to_shared(smem + off) + warp * SLOTS * 8;
-    uint8_t* ring = smem + off + bar_bytes + (size_t)warp * SLOTS * item_bytes;
-    const uint32_t ring_u32 = (uint32_t)__cvta_generic_to_shared(ring);
-    if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < SLOTS; s++) mbar_init(bar_u32 + 8 * s, 1);
-        mbar_fence_init();
-        fence_proxy_async_smem();
-    }
-    int slot_i = 0, slot_u = 0;
-    uint32_t phase = 0;
-    const int quads = p.rows / RW;
-    const int q0 = (int)((long)quads * blockIdx.x / gridDim.x), q1 = (int)((long)quads * (blockIdx.x + 1) / gridDim.x);
-    const int r0 = q0 * RW, nquads = q1 - q0, nrows = nquads * RW;
-
-  for (int t0 = 0; t0 < Teff;) {
-    __syncthreads();
-    if (threadIdx.x == 0) {   // greedy chunk: tokens t0.. while their owned pairs fit
-        int np = 0, nt = 0;
-        while (t0 + nt < Teff && nt < kBulkMaxChunkTokens) {
-            int cnt = 0;
-            for (int j = 0; j < k; j++) {
-                const long e = p.ids ? (long)p.ids[(long)(t0 + nt) * k + j] - p.id_offset : 0;
-                cnt += (e >= 0 && e < p.n_experts) ? 1 : 0;
-            }
-            if (nt > 0 && np + cnt > pcap) break;
-            s_first[nt] = np;
-            for (int j = 0; j < k; j++) {
-                const long e = p.ids ? (long)p.ids[(long)(t0 + nt) * k + j] - p.id_offset : 0;
-                if (e >= 0 && e < p.n_experts) pairs[np++] = (nt << 8) | j;
-            }
-            nt++;
-        }
-        s_first[nt] = np;
-        s_np = np;
-        s_nt = nt;
-    }
-    __syncthreads();
-    const int np = s_np, nt = s_nt;
-    const int total = nquads * np;
-    int ni = total - warp;
-    ni = ni > 0 ? (ni + W - 1) / W : 0;
-    int ipi = 0, iq = 0, iss = 0;
-    if (ni > 0) { ipi = warp / nquads; iq = warp - ipi * nquads; }
-    int cpi = ipi, cq = iq;
-
-    auto issue_one = [&]() {
-        if (iss < ni) {
-            if (lane == 0) {
-                const int pr = pairs[ipi], j = pr & 0xff;
-                const long e = p.ids ? (long)p.ids[(long)(t0 + (pr >> 8)) * k + j] - p.id_offset : 0L;
-                const long row = e * p.rows + r0 + iq * RW;
-                const uint8_t* src = reinterpret_cast<const uint8_t*>(p.w) + (row >> 2) * item_bytes;
-                const uint32_t bar = bar_u32 + 8 * slot_i;
-                mbar_expect_tx(bar, (uint32_t)item_bytes);
-                bulk_g2s(ring_u32 + slot_i * item_bytes, src, (uint32_t)item_bytes, bar);
-            }
-            iss++;
-            iq += W;
-            while (iq >= nquads) { iq -= nquads; ipi++; }
-            slot_i = (slot_i + 1 == SLOTS) ? 0 : slot_i + 1;
-        }
-    };
-#pragma unroll
-    for (int s = 0; s < SLOTS; s++) issue_one();
-
-    i4_stage(act, p.a, KTB200_TYPE_F32, np, p.ncols, [&](int pi) {
-        const int pr = pairs[pi];
-        return ((long)(t0 + (pr >> 8)) * k + (pr & 0xff)) * p.ncols;
-    });
-    __syncthreads();
-
-    for (int n = 0; n < ni; n++) {
-        mbar_wait(bar_u32 + 8 * slot_u, (phase >> slot_u) & 1u);
-        phase ^= 1u << slot_u;
-        const uint8_t* sl = ring + slot_u * item_bytes;
-        float res;
-        {
-            float acc[RW] = {0.f, 0.f, 0.f, 0.f};
-            for (int f = lane; f < nrb; f += 32) {
-                const int rw = f / nb, blk = f - rw * nb;
-                const uint8_t* const wb[1] = {sl + f * SZ_RAWINT4};
-                float v[1] = {0.f};
-                i4_block_dot<1>(wb, act + ((size_t)cpi * nb + blk) * (kI4ActStride / 4), v);
-                acc[0] += rw == 0 ? v[0] : 0.f; acc[1] += rw == 1 ? v[0] : 0.f; acc[2] += rw == 2 ? v[0] : 0.f; acc[3] += rw == 3 ? v[0] : 0.f;
-            }
-            res = warp_reduce4(acc[0], acc[1], acc[2], acc[3], lane);
-        }
-        __syncwarp();
-        slot_u = (slot_u + 1 == SLOTS) ? 0 : slot_u + 1;
-        issue_one();
-        if ((lane & 7) == 0) partial[(cq * RW + (lane >> 3)) * pcap + cpi] = res;
-        cq += W;
-        while (cq >= nquads) { cq -= nquads; cpi++; }
-    }
-    __syncthreads();
-    // weighted accumulation over a token's experts IN expert_ids ORDER, one FMA per expert
-    for (int idx = threadIdx.x; idx < nrows * nt; idx += W * 32) {
-        const int tl = idx / nrows, hl = idx - tl * nrows;
-        const long t = t0 + tl;
-        float acc = 0.f;
-        for (int pi = s_first[tl]; pi < s_first[tl + 1]; pi++) {
-            const float dv = partial[hl * pcap + pi];
-            acc = p.weights ? __fmaf_rn(dv, p.weights[t * k + (pairs[pi] & 0xff)], acc) : acc + dv;
-        }
-        const long o = t * p.rows + r0 + hl;
-        if (p.accumulate) acc = load_hidden(p.out, o, p.hidden_type) + round_hidden(acc, p.hidden_type);
-        store_hidden(p.out, o, p.hidden_type, acc);
-    }
-    t0 += nt;
   }  // token chunks
 }
 

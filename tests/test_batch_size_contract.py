@@ -221,7 +221,7 @@ def moe_case(qlen, H, I, dt, hid=BF16, E=8, k=4, shared=None, launches=2, m=None
 
 
 def rawint4_case(qlen, H=512, I=256, E=8, k=4):
-    """RAWINT4_G32 routed experts (rows_bulk_i4_kernel + reduce_bulk_i4_kernel)"""
+    """RAWINT4_G32 routed experts (rows_bulk_i4_kernel + reduce_bulk_kernel<BulkI4>)"""
     lib = _lib()
     gen = torch.Generator(device="cuda").manual_seed(5)
     blocks = []

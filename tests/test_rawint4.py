@@ -3,6 +3,8 @@ and the sm_90a kernels against the float64 oracle in tests/int4_oracle.py."""
 import ctypes as C
 import json
 import os
+import subprocess
+import sys
 
 import numpy as np
 import pytest
@@ -256,6 +258,48 @@ def test_moe_forward_small(hidden_type, E, k, H, I, qlen):
     x, x64 = _x(qlen, H, qlen, hidden_type)
     got = m.forward(ids, w, x)
     _check(got, o4.moe_forward(x64, ids, w, ex.expert, E), hidden_type)
+
+
+# torch.profiler in an interpreter of its own, as test_rawint4_grouped's census at the grouped threshold
+_CENSUS = r"""
+import json, sys
+import numpy as np, torch
+sys.path[:0] = sys.argv[1:]
+from torch.profiler import ProfilerActivity, profile
+from test_rawint4 import F32, _Experts, _x
+res = {}
+m = _Experts(8, 1024, 512, 5).moe(4, F32)
+for T in (1, 8):
+    rng = np.random.default_rng(T)
+    ids = np.stack([rng.permutation(8)[:4] for _ in range(T)]).astype(np.int64)
+    w = rng.random((T, 4)).astype(np.float32)
+    x = _x(T, 1024, T, F32)[0]
+    m.forward(ids, w, x)
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        m.forward(ids, w, x)
+        torch.cuda.synchronize()
+    res[T] = [e.key for e in prof.key_averages() if "ktb::" in e.key for _ in range(e.count)]
+m.close()
+print("CENSUS " + json.dumps(res))
+"""
+
+
+@pytest.mark.gpu
+def test_kernels_that_ran_below_the_grouped_threshold():
+    """1 and 8 tokens: gate/up on rows_bulk_i4_kernel, down on reduce_bulk_kernel<BulkI4>, and nothing else"""
+    here = os.path.dirname(os.path.abspath(__file__))
+    root = os.path.dirname(here)
+    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", _CENSUS, here, root]
+    r = subprocess.run(cmd, capture_output=True, text=True, timeout=600, cwd=root)
+    assert r.returncode == 0, r.stderr[-3000:]
+    res = json.loads(next(l for l in r.stdout.splitlines() if l.startswith("CENSUS "))[7:])
+    for T, names in res.items():
+        assert len(names) == 2, (T, names)
+        gate_up = [n for n in names if "rows_" in n]
+        down = [n for n in names if "reduce_" in n]
+        assert len(gate_up) == 1 and len(down) == 1, (T, names)
+        assert "rows_bulk_i4_kernel<" in gate_up[0], (T, names)
+        assert "reduce_bulk_kernel<ktb::BulkI4," in down[0], (T, names)
 
 
 @pytest.mark.gpu

@@ -103,7 +103,7 @@ def test_kernels_that_ran_at_the_threshold():
         names = res[ht]
         ran = sorted(n.split("grouped_i4_kernel<")[1][0] for n in names if "grouped_i4_kernel<" in n)
         assert ran == sorted(want), (ht, names)
-        assert not any(s in n for n in names for s in ("rows_bulk_i4", "reduce_bulk_i4", "grouped_gemm_kernel")), (ht, names)
+        assert not any(s in n for n in names for s in ("rows_bulk_i4", "reduce_bulk_kernel<ktb::BulkI4", "grouped_gemm_kernel")), (ht, names)
 
 
 @pytest.mark.gpu
