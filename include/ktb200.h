@@ -325,7 +325,14 @@ int ktb200_ep_reduce_own_token(const ktb200_ep_comm* comm, void* y_out_dev, cons
  * call sequence.  Every rank must issue the same sequence of calls.  moe->group_max_len >= world.  idx_dev / w_dev
  * receive the own token's routing.  phase_mask: 7 = the whole layer (production); 1 / 2 / 4 run the route+send, the
  * experts+deliver and the combine phase as separate launches (tests emulate N ranks on one GPU with them).
- * KTB200_EINVAL when the configuration is not the persistent kernel's (see ktb200_moe_block_forward).
+ * Accepted expert types (gate / up / down, gate and up of one type): Q4_K / Q4_K / {Q4_K, Q6_K}, with a shared expert of the
+ * same types and shapes; and {Q2_K, Q3_K} gate / up with {Q2_K, Q3_K, Q4_K, Q6_K} down (llama.cpp's Q2_K, Q3_K_S and Q3_K_M
+ * files; hidden_size a multiple of 1024 up to 16384, an even number of blocks per down row for Q3_K).  With Q2_K / Q3_K the
+ * shared expert may be of any types ktb200_mlp_forward takes: with the combine phase (phase_mask bit 4) its rounded output is
+ * written into y_out on `stream` first, and the kernel adds the cross-rank sum to it; so y_out must not alias x_own (the
+ * router still reads x_own after that write).
+ * KTB200_EINVAL when the configuration is not the persistent kernel's (see ktb200_moe_block_forward): other type sets (mixed
+ * Q2_K / Q3_K gate / up, Q5_K, the i-quants, RAWINT4), or a shape that does not fit shared memory.
  * ------------------------------------------------------------------------------------------ */
 long ktb200_ep_msg_bytes(int hidden_size, int hidden_type);
 int ktb200_moe_ep_block_forward(const ktb200_gate_config* gate, ktb200_moe* moe, ktb200_mlp* shared, const ktb200_ep_comm* comm,

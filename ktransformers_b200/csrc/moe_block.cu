@@ -695,6 +695,8 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
 //   C (4)  wait until all CTAs of all ranks have delivered; y = round(sum over ranks, rank order) + round(shared).
 // Buffers are reused every layer without extra barriers: a rank can only send its next token after it finished
 // phase C, which needs every rank's phase-X stores, which come after that rank's reads of the messages.
+// moe_ep_block_kernel<GU, DownFmt> below (Q2_K / Q3_K gate/up) repeats this exchange (the message push, the pair list, the
+// deliver stores, the flag and epoch protocol, phase C and the exit): a change to the protocol is a change to both.
 constexpr int kEpWorldMax = 8;
 constexpr int kEpPairsMax = 64;
 
@@ -727,12 +729,13 @@ __device__ __forceinline__ void red_release_sys_add(unsigned* p, unsigned v) {
     asm volatile("red.release.sys.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-// one token row (hidden type, read at L2: it was written by a peer) -> Q8_K in staging slot `slot`
+// one token row (hidden type, read at L2: it was written by a peer) -> Q8_K in staging slot `slot`, KBS int16 sums per block
+template <int KBS>
 __device__ __forceinline__ void ep_quantize_row(const BlockParams& p, const uint8_t* row, uint8_t* slot_base) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, W = blockDim.x >> 5, nblk = p.H / QK_K;
     uint8_t* xq = slot_base;
     int16_t* xbs = reinterpret_cast<int16_t*>(slot_base + (size_t)nblk * kActBlkStride);
-    float* xdx = reinterpret_cast<float*>(slot_base + (size_t)nblk * (kActBlkStride + 16));
+    float* xdx = reinterpret_cast<float*>(slot_base + (size_t)nblk * (kActBlkStride + 2 * KBS));
     for (int b = warp; b < nblk; b += W) {
         float x[8];
         const long e0 = (long)b * QK_K + lane * 8;
@@ -753,7 +756,8 @@ __device__ __forceinline__ void ep_quantize_row(const BlockParams& p, const uint
                 }
             }
         }
-        warp_quantize_q8k_block(x, lane, reinterpret_cast<uint32_t*>(xq + (size_t)b * kActBlkStride), xdx + b, nullptr, xbs + b * 8);
+        warp_quantize_q8k_block(x, lane, reinterpret_cast<uint32_t*>(xq + (size_t)b * kActBlkStride), xdx + b,
+                                KBS == 16 ? xbs + b * 16 : nullptr, KBS == 8 ? xbs + b * 8 : nullptr);
     }
 }
 
@@ -947,8 +951,8 @@ __global__ void __launch_bounds__(kBlockWarpsLo * 32, 1) moe_ep_block_kernel(con
             const int pe0 = u0 / p.I, pe1 = (u1 - 1) / p.I;       // at most two pairs: total / grid < I
             if (threadIdx.x == 0) { es.tok_slot[0] = es.pair_src[pe0]; es.tok_slot[1] = es.pair_src[pe1]; }
             const BlockLay L = block_layout<DownFmt::kBs>(p, smem);
-            ep_quantize_row(p, mymsg + (size_t)es.pair_src[pe0] * pp.x.msg_bytes, L.xq);
-            if (es.pair_src[pe1] != es.pair_src[pe0]) ep_quantize_row(p, mymsg + (size_t)es.pair_src[pe1] * pp.x.msg_bytes, L.xq + x_slot_bytes);
+            ep_quantize_row<8>(p, mymsg + (size_t)es.pair_src[pe0] * pp.x.msg_bytes, L.xq);
+            if (es.pair_src[pe1] != es.pair_src[pe0]) ep_quantize_row<8>(p, mymsg + (size_t)es.pair_src[pe1] * pp.x.msg_bytes, L.xq + x_slot_bytes);
         }
         __syncthreads();
         list_shared = false;
@@ -1084,6 +1088,318 @@ __global__ void __launch_bounds__(kBlockWarpsLo * 32, 1) moe_ep_block_kernel(con
             for (int r = 0; r < world; r++) acc += __ldcg(mine + (size_t)r * p.H + row);   // rank order: deterministic
             float v = round_hidden(acc, p.hidden_type);
             if (has_shared) v += round_hidden(__ldcg(pp.x.shared_out + row), p.hidden_type);
+            store_hidden(p.out, row, p.hidden_type, v);
+        }
+        block_stamp(p, 10);
+    }
+
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const unsigned prev = atomicAdd(p.sync + 1, 1u);
+        if (prev == gridDim.x - 1) {
+            p.sync[0] = 0;
+            p.sync[1] = 0;
+            if (mask & 4) my_flags[2 * world] = epoch;
+            __threadfence();
+        }
+    }
+}
+
+// The same layer for Q2_K / Q3_K routed gate/up (GU = BulkQ2K | BulkQ3K, gate and up of one type) and any bulk down item
+// (BulkQ2K | BulkQ3K | BulkQ4K | BulkQ6K4T): llama.cpp's Q2_K, Q3_K_S and Q3_K_M files.  Phases, messages, flags, epochs and
+// the reuse argument are those of the kernel above, and the code that implements them repeats that kernel's (kept apart so
+// that the Q4_K instantiations compile to the same instructions as before): a change to the protocol is a change to both.
+// What differs:
+//   * a gate/up unit is rows 2r, 2r+1 of gate and of up (the unit of rows_bulk_iq_kernel, iq.cuh: single Q2_K / Q3_K rows are
+//     not 16-byte sized), two bulk copies on one mbarrier; the per-lane loop and the reduction are that kernel's, so `inter`
+//     equals the per-pair kernels' output bit for bit;
+//   * the shared expert is not in the launch (its types need not be the routed ones): the launcher runs ktb200_mlp_forward
+//     into y first, with the combine phase, and p.s_gate != null says y holds that rounded term.  Phase C computes
+//     y = round(sum over ranks, rank order) + y, as ep_tok_combine_kernel does; phase R streams nothing beside the router;
+//   * warps per CTA and the down chunk `pa` come from the shared-memory plan (ep_kq_plan).
+// Dynamic shared memory: [BlockShared][region A][EpShared | tokacc [nrows_max][kEpWorldMax] | partial [nrows_max][pa]]
+// [mbarriers W x 2][rings W x ring_bytes].  Region A holds in turn the router's selection scratch (blk_select's layout), the
+// Q8_K rows of up to two tokens (GU's sums) and the Q8_K `a` of pa entries (DownFmt's sums).
+constexpr int kEpKqSlots = 2;   // ring slots per warp, gate/up units and down items alike
+template <int KBS>
+__host__ __device__ constexpr int ep_x_slot_bytes(int nblk) { return (nblk * (kActBlkStride + 2 * KBS + 4) + 15) & ~15; }
+
+template <class GU, class DownFmt>
+__global__ void __launch_bounds__(kBlockWarpsLo * 32, 1) moe_ep_block_kernel(const EpParams pp) {
+    constexpr int RW = 4, S = kEpKqSlots;
+    extern __shared__ __align__(16) uint8_t smem[];
+    BlockShared& sh = *reinterpret_cast<BlockShared*>(smem);
+    EpShared& es = *reinterpret_cast<EpShared*>(smem + pp.x.ep_off);
+    const BlockParams& p = pp.b;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, W = blockDim.x >> 5;
+    griddep_launch_dependents();
+    bool waited = false;
+    const int k = p.k, world = pp.x.world, rank = pp.x.rank, mask = pp.x.phase_mask;
+    const bool has_shared = p.s_gate != nullptr;
+    const int nblk = p.H / QK_K, nb = p.I / QK_K;
+    const int pa = pp.x.pa;
+    float* tokacc = reinterpret_cast<float*>(smem + pp.x.ep_off + ((sizeof(EpShared) + 15) & ~(size_t)15));   // [nrows_max][world]
+    float* partial = tokacc + (size_t)p.nrows_max * kEpWorldMax;                                            // [nrows_max][pa]
+    uint32_t bar_u32, ring_u32;
+    {
+        const size_t off = (reinterpret_cast<uint8_t*>(partial + (size_t)p.nrows_max * pa) - smem + 15) & ~(size_t)15;
+        bar_u32 = (uint32_t)__cvta_generic_to_shared(smem + off) + warp * S * 8;
+        ring_u32 = (uint32_t)__cvta_generic_to_shared(smem + off + ((W * S * 8 + 15) & ~15)) + warp * p.ring_bytes;
+    }
+    if (lane == 0) {
+#pragma unroll
+        for (int s = 0; s < S; s++) mbar_init(bar_u32 + 8 * s, 1);
+        mbar_fence_init();
+        fence_proxy_async_smem();
+    }
+    {
+        const uint32_t* src = reinterpret_cast<const uint32_t*>(&pp.b);
+        uint32_t* dst = reinterpret_cast<uint32_t*>(&sh.prm);
+        for (int i = threadIdx.x; i < (int)(sizeof(BlockParams) / 4); i += blockDim.x) dst[i] = src[i];
+        const uint32_t* src2 = reinterpret_cast<const uint32_t*>(&pp.x);
+        uint32_t* dst2 = reinterpret_cast<uint32_t*>(&es.x);
+        for (int i = threadIdx.x; i < (int)(sizeof(EpExtra) / 4); i += blockDim.x) dst2[i] = src2[i];
+    }
+    __syncthreads();   // the parameter copies in shared memory (read by blk_router & co through sh.prm) and the mbarriers are ready
+    uint32_t phase = 0;   // bit s = parity the next use of barrier s waits for
+    unsigned gen = 0;
+    const uint8_t* ring = smem + (ring_u32 - (uint32_t)__cvta_generic_to_shared(smem));
+    unsigned* my_flags = pp.x.flags[rank];
+    unsigned* status = my_flags + 2 * world + 1;
+    // row slice of this CTA (phases X and C)
+    const int quads = p.H / RW;
+    const int q0 = (int)((long)quads * blockIdx.x / gridDim.x), nquads = (int)((long)quads * (blockIdx.x + 1) / gridDim.x) - q0;
+    const int nrows = nquads * RW;
+    uint8_t* region_a = smem + kBlockSharedBytes;
+    block_stamp(p, 0);
+
+    // =============================================================================================== phase R
+    if (mask & 1) {
+        blk_router(0, waited);
+        block_stamp(p, 2);
+        grid_arrive(p.sync, gen);
+        grid_wait(p.sync, gen);
+        block_stamp(p, 3);
+        blk_select(0);
+        block_stamp(p, 4);
+        // push {x, ids, w} to peer `blockIdx.x`
+        if ((int)blockIdx.x < world) {
+            const int peer = blockIdx.x;
+            uint8_t* dst = pp.x.msg[peer] + (size_t)rank * pp.x.msg_bytes;
+            const int xb = p.H * (int)type_size(p.hidden_type);
+            const uint4* src = reinterpret_cast<const uint4*>(p.g.x);
+            for (int i = threadIdx.x; i < xb / 16; i += blockDim.x) reinterpret_cast<uint4*>(dst)[i] = src[i];
+            if ((int)threadIdx.x < k) {
+                reinterpret_cast<int*>(dst + xb)[threadIdx.x] = (int)sh.ids[threadIdx.x];
+                reinterpret_cast<float*>(dst + xb + 64)[threadIdx.x] = sh.w[threadIdx.x];
+            }
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                unsigned ep = *reinterpret_cast<volatile unsigned*>(my_flags + 2 * world) + 1;
+                __threadfence_system();
+                st_release_sys_u32(pp.x.flags[peer] + rank, ep);
+            }
+        }
+    }
+    if (!waited) { griddep_wait(); waited = true; }
+    if (threadIdx.x == 0) es.epoch = *reinterpret_cast<volatile unsigned*>(my_flags + 2 * world) + 1;
+    __syncthreads();
+    const unsigned epoch = es.epoch;
+
+    // =============================================================================================== phase X
+    if (mask & 2) {
+        if ((int)threadIdx.x < world) wait_ge<true>(my_flags + threadIdx.x, epoch, status);
+        __syncthreads();
+        block_stamp(p, 5);
+        const uint8_t* mymsg = pp.x.msg[rank];
+        const int xb = p.H * (int)type_size(p.hidden_type);
+        if (threadIdx.x == 0) {   // the pairs this shard owns, by (token, slot): identical in every CTA
+            int np = 0;
+            for (int t = 0; t < world; t++) {
+                const uint8_t* m = mymsg + (size_t)t * pp.x.msg_bytes + xb;
+                for (int j = 0; j < k; j++) {
+                    const int e = __ldcg(reinterpret_cast<const int*>(m) + j) - p.id_offset;
+                    if (e >= 0 && e < p.n_local && np < kEpPairsMax) {
+                        es.pair_src[np] = t; es.pair_e[np] = e; es.pair_w[np] = __ldcg(reinterpret_cast<const float*>(m + 64) + j);
+                        np++;
+                    }
+                }
+            }
+            es.np = np;
+        }
+        __syncthreads();
+        const int np = es.np;
+        // ------------------------------------------------------------ gate/up over (pair, row pair) units
+        const int nru = p.I / 2, row_bytes = nblk * GU::kBlockBytes, unit_bytes = 2 * row_bytes;
+        const int x_slot = ep_x_slot_bytes<GU::kBs>(nblk);
+        const long total = (long)np * nru;
+        const int u0 = (int)(total * blockIdx.x / gridDim.x), u1 = (int)(total * (blockIdx.x + 1) / gridDim.x);
+        if (u1 > u0) {
+            const int pe0 = u0 / nru, pe1 = (u1 - 1) / nru;       // at most two pairs: total / grid < I / 2
+            if (threadIdx.x == 0) { es.tok_slot[0] = es.pair_src[pe0]; es.tok_slot[1] = es.pair_src[pe1]; }
+            ep_quantize_row<GU::kBs>(p, mymsg + (size_t)es.pair_src[pe0] * pp.x.msg_bytes, region_a);
+            if (es.pair_src[pe1] != es.pair_src[pe0]) ep_quantize_row<GU::kBs>(p, mymsg + (size_t)es.pair_src[pe1] * pp.x.msg_bytes, region_a + x_slot);
+        }
+        __syncthreads();
+        const int nu = warp_units(u0, u1, warp, W);
+        UnitCursor ic;
+        if (nu > 0) ic.start(u0 + warp, nru);
+        UnitCursor cc = ic;
+        int iss = 0, slot_i = 0, slot_u = 0;
+        auto issue_u = [&]() {
+            if (iss < nu) {
+                if (lane == 0) {
+                    const long off = ((long)es.pair_e[ic.pi] * p.I + 2L * ic.r) * row_bytes;
+                    const uint32_t bar = bar_u32 + 8 * slot_i, dst = ring_u32 + slot_i * 2 * unit_bytes;
+                    mbar_expect_tx(bar, 2u * unit_bytes);
+                    bulk_g2s(dst, reinterpret_cast<const uint8_t*>(p.w_gate) + off, (uint32_t)unit_bytes, bar);
+                    bulk_g2s(dst + unit_bytes, reinterpret_cast<const uint8_t*>(p.w_up) + off, (uint32_t)unit_bytes, bar);
+                }
+                iss++;
+                ic.step(W, nru);
+                slot_i = (slot_i + 1 == S) ? 0 : slot_i + 1;
+            }
+        };
+#pragma unroll
+        for (int s = 0; s < S; s++) issue_u();
+        for (int n = 0; n < nu; n++) {
+            mbar_wait(bar_u32 + 8 * slot_u, (phase >> slot_u) & 1u);
+            phase ^= 1u << slot_u;
+            const uint8_t* sl = ring + slot_u * 2 * unit_bytes;
+            const uint8_t* at = region_a + (es.pair_src[cc.pi] == es.tok_slot[0] ? 0 : x_slot);
+            const int16_t* bs = reinterpret_cast<const int16_t*>(at + (size_t)nblk * kActBlkStride);
+            const float* dx = reinterpret_cast<const float*>(at + (size_t)nblk * (kActBlkStride + 2 * GU::kBs));
+            float g0 = 0.f, g1 = 0.f, v0 = 0.f, v1 = 0.f;
+            for (int f = lane; f < 2 * nblk; f += 32) {   // (row, block) of the unit: f = rw * nblk + blk
+                const int rw = f >= nblk, blk = f - rw * nblk;
+                const uint8_t* aq = at + (size_t)blk * kActBlkStride;
+                const float g = GU::block_dot(sl + f * GU::kBlockBytes, aq, bs + blk * GU::kBs, dx[blk]);
+                const float u = GU::block_dot(sl + unit_bytes + f * GU::kBlockBytes, aq, bs + blk * GU::kBs, dx[blk]);
+                if (rw) { g1 += g; v1 += u; } else { g0 += g; v0 += u; }
+            }
+            const float r = warp_reduce4(g0, g1, v0, v1, lane);   // lane 0: g0, 8: g1, 16: u0, 24: u1
+            __syncwarp();
+            slot_u = (slot_u + 1 == S) ? 0 : slot_u + 1;
+            issue_u();
+            const float gs = __shfl_sync(0xffffffffu, r, 8 * (lane & 1)), us = __shfl_sync(0xffffffffu, r, 16 + 8 * (lane & 1));
+            if (lane < 2) p.inter[(long)cc.pi * p.I + 2L * cc.r + lane] = (p.use_silu ? act_silu(gs) : act_relu(gs)) * us;
+            cc.step(W, nru);
+        }
+        block_stamp(p, 6);
+
+        // ------------------------------------------------------------ down (entries = the pairs, in chunks of pa)
+        const int nrb = RW * nb, item_bytes = nrb * DownFmt::kBlockBytes;
+        for (int i = threadIdx.x; i < nrows * world; i += blockDim.x) tokacc[i] = 0.f;
+        grid_arrive(p.sync, gen);
+        int dvi = 0, dq = 0, dss = 0, dcons = 0, ni = 0, evi = 0, eq = 0, dslot_i = 0, dslot_u = 0, c0 = 0;
+        auto issue_d = [&]() {
+            if (dss < ni && dss - dcons < S) {
+                if (lane == 0) {
+                    const long row = (long)(q0 + dq) * RW + (long)es.pair_e[c0 + dvi] * p.H;
+                    const uint32_t bar = bar_u32 + 8 * dslot_i;
+                    mbar_expect_tx(bar, (uint32_t)item_bytes);
+                    bulk_g2s(ring_u32 + dslot_i * item_bytes, reinterpret_cast<const uint8_t*>(p.w_down) + (row >> 2) * item_bytes,
+                             (uint32_t)item_bytes, bar);
+                }
+                dss++;
+                dq += W;
+                while (dq >= nquads) { dq -= nquads; dvi++; }
+                dslot_i = (dslot_i + 1 == S) ? 0 : dslot_i + 1;
+            }
+        };
+        auto start_chunk = [&](int c0_, int cn) {
+            c0 = c0_;
+            ni = nquads * cn - warp;
+            ni = ni > 0 ? (ni + W - 1) / W : 0;
+            dss = dcons = 0;
+            dvi = ni > 0 ? warp / nquads : 0; dq = ni > 0 ? warp - dvi * nquads : 0;
+            evi = dvi; eq = dq;
+        };
+        start_chunk(0, min(pa, np));
+#pragma unroll
+        for (int s = 0; s < S; s++)
+            if (s < p.prime_d) issue_d();
+        grid_wait(p.sync, gen);
+        block_stamp(p, 7);
+        uint8_t* aq = region_a;
+        int16_t* abs_ = reinterpret_cast<int16_t*>(aq + (size_t)pa * nb * kActBlkStride);
+        float* adx = reinterpret_cast<float*>(aq + (size_t)pa * nb * (kActBlkStride + 2 * DownFmt::kBs));
+        for (int cbase = 0; cbase < np; cbase += pa) {
+            const int cn = min(pa, np - cbase);
+            if (cbase) start_chunk(cbase, cn);
+            // activations of the chunk's pairs -> Q8_K (region A is free: gate/up is done everywhere after the barrier)
+            for (int gb = warp; gb < cn * nb; gb += W) {
+                const int r = gb / nb, b = gb - r * nb;
+                const float4* src = reinterpret_cast<const float4*>(p.inter + (long)(cbase + r) * p.I + (long)b * QK_K + lane * 8);
+                const float4 v0 = __ldcg(src), v1 = __ldcg(src + 1);
+                float x[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+                warp_quantize_q8k_block(x, lane, reinterpret_cast<uint32_t*>(aq + (size_t)gb * kActBlkStride), adx + gb,
+                                        DownFmt::kBs == 16 ? abs_ + gb * 16 : nullptr, DownFmt::kBs == 8 ? abs_ + gb * 8 : nullptr);
+            }
+#pragma unroll
+            for (int s = 0; s < S; s++) issue_d();
+            __syncthreads();
+            for (int n = 0; n < ni; n++) {
+                mbar_wait(bar_u32 + 8 * dslot_u, (phase >> dslot_u) & 1u);
+                phase ^= 1u << dslot_u;
+                const uint8_t* sl = ring + dslot_u * item_bytes;
+                float res;
+                {
+                    float acc[RW] = {0.f, 0.f, 0.f, 0.f};
+                    for (int f = lane; f < nrb; f += 32) {
+                        const int rw = f / nb, blk = f - rw * nb;
+                        const int ab = evi * nb + blk;
+                        const float val = DownFmt::dot(sl, f, nrb, aq + (size_t)ab * kActBlkStride, abs_ + ab * DownFmt::kBs, adx[ab]);
+                        acc[0] += rw == 0 ? val : 0.f; acc[1] += rw == 1 ? val : 0.f; acc[2] += rw == 2 ? val : 0.f; acc[3] += rw == 3 ? val : 0.f;
+                    }
+                    res = warp_reduce4(acc[0], acc[1], acc[2], acc[3], lane);
+                }
+                __syncwarp();
+                dslot_u = (dslot_u + 1 == S) ? 0 : dslot_u + 1;
+                dcons++;
+                issue_d();
+                if ((lane & 7) == 0) partial[(eq * RW + (lane >> 3)) * pa + evi] = res;
+                eq += W;
+                while (eq >= nquads) { eq -= nquads; evi++; }
+            }
+            __syncthreads();
+            // weighted accumulation per token in (token, slot) order with one FMA per pair (moe.cpp:222-236)
+            for (int hl = threadIdx.x; hl < nrows; hl += blockDim.x) {
+                for (int r = 0; r < cn; r++) {
+                    const int pi = cbase + r;
+                    float* a = tokacc + hl * world + es.pair_src[pi];
+                    *a = __fmaf_rn(partial[hl * pa + r], es.pair_w[pi], *a);
+                }
+            }
+            __syncthreads();
+        }
+        block_stamp(p, 8);
+        // ------------------------------------------------------------ deliver: my rows of every token's partial sum
+        for (int i = threadIdx.x; i < nquads * world; i += blockDim.x) {
+            const int t = i / nquads, qd = i - t * nquads;
+            const float4 v = make_float4(tokacc[(qd * 4 + 0) * world + t], tokacc[(qd * 4 + 1) * world + t], tokacc[(qd * 4 + 2) * world + t],
+                                         tokacc[(qd * 4 + 3) * world + t]);
+            *reinterpret_cast<float4*>(pp.x.part[t] + (size_t)rank * p.H + (size_t)(q0 + qd) * 4) = v;
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            __threadfence_system();
+            for (int t = 0; t < world; t++) red_release_sys_add(pp.x.flags[t] + world + rank, 1u);
+        }
+    }
+
+    // =============================================================================================== phase C
+    if (mask & 4) {
+        if ((int)threadIdx.x < world) wait_ge<true>(my_flags + world + threadIdx.x, epoch * gridDim.x, status);
+        __syncthreads();
+        block_stamp(p, 9);
+        const float* mine = pp.x.part[rank];
+        for (int hl = threadIdx.x; hl < nrows; hl += blockDim.x) {
+            const int row = q0 * 4 + hl;
+            float acc = 0.f;
+            for (int r = 0; r < world; r++) acc += __ldcg(mine + (size_t)r * p.H + row);   // rank order: deterministic
+            float v = round_hidden(acc, p.hidden_type);
+            if (has_shared) v += load_hidden(p.out, row, p.hidden_type);   // the rounded shared term ktb200_mlp_forward stored
             store_hidden(p.out, row, p.hidden_type, v);
         }
         block_stamp(p, 10);
@@ -1247,6 +1563,168 @@ extern "C" int ktb200_moe_block_forward(const ktb200_gate_config* gc, ktb200_moe
 
 extern "C" long ktb200_ep_msg_bytes(int hidden_size, int hidden_type) { return (long)hidden_size * type_size(hidden_type) + 128; }
 
+namespace ktb {
+// the router configurations the persistent kernels' grouped top-k (gate_select_token) takes
+static bool ep_gate_ok(const ktb200_gate_config* gc, int k) {
+    return gc->n_experts <= kGateThreads * kGateEPT && gc->n_experts > 0 && gc->n_group >= 1 && gc->n_group <= 32 &&
+           gc->n_experts % gc->n_group == 0 && gc->topk_group >= 1 && gc->topk_group <= gc->n_group && gc->weight && gc->scoring >= 0 &&
+           gc->scoring <= 1 && gc->topk_method >= 0 && gc->topk_method <= 2 && k <= gc->n_experts;
+}
+
+// Fills everything of an expert-parallel launch but the plan (nrows_max, region_a, ring_bytes, pa, ep_off).
+static int ep_block_params(EpParams& pp, const ktb200_gate_config* gc, ktb200_moe* m, ktb200_mlp* sh, const ktb200_ep_comm* comm,
+                           const void* x_own, void* y_out, int64_t* idx, float* w, int phase_mask) {
+    const ktb200_moe_config& c = m->cfg;
+    const int k = gc->top_k, world = comm->world;
+    BlockParams& p = pp.b;
+    const int S = gate_splits(gc->n_experts, gc->hidden_size, num_sms(m->device));
+    p.g = GateParams{gc->weight, x_own, gc->hidden_type, gc->n_experts, gc->hidden_size, 1, S, k, gc->n_group, gc->topk_group,
+                     gc->scoring, gc->topk_method, gc->norm_topk_prob, gc->routed_scaling_factor, gc->bias, m->blk_partial, nullptr,
+                     idx, w, nullptr, nullptr};
+    p.w_gate = c.gate_proj; p.w_up = c.up_proj; p.w_down = c.down_proj;
+    p.s_gate = sh ? sh->gate : nullptr; p.s_up = sh ? sh->up : nullptr; p.s_down = sh ? sh->down : nullptr;
+    p.n_local = c.expert_num; p.id_offset = c.expert_id_offset;
+    p.H = c.hidden_size; p.I = c.intermediate_size; p.k = k; p.hidden_type = c.hidden_type; p.use_silu = c.use_silu;
+    p.inter = m->inter; p.out = y_out; p.sync = m->blk_sync + 2 * (m->blk_flip++ & 1u); p.trace = g_btrace;
+    p.prime_u = 3; p.prime_d = 2;
+    pp.x.rank = comm->rank; pp.x.world = world; pp.x.phase_mask = phase_mask;
+    pp.x.msg_bytes = (int)ktb200_ep_msg_bytes(c.hidden_size, c.hidden_type);
+    pp.x.inter_shared_row = world * k;
+    pp.x.shared_out = m->blk_partial + 16384;
+    for (int r = 0; r < world; r++) {
+        if (!comm->token_bufs[r] || !comm->partial_bufs[r] || !comm->flag_bufs[r]) { set_error("ep_block: null peer pointer for rank %d", r); return KTB200_EINVAL; }
+        pp.x.msg[r] = (uint8_t*)comm->token_bufs[r]; pp.x.part[r] = comm->partial_bufs[r]; pp.x.flags[r] = comm->flag_bufs[r];
+    }
+    return KTB200_OK;
+}
+
+// Once per (variant, device): raise the kernel's dynamic shared-memory limit and check that the G CTAs can be co-resident
+// (the grid barriers spin on all of them).  Variants: 0 / 1 the Q4_K kernels (Q4_K / Q6_K down), 2 .. 9 the Q2_K / Q3_K ones.
+static int ep_block_resident(const void* fn, int variant, int G, int W, size_t smem, int dev) {
+    static size_t limit[10][64] = {};
+    static int resident[10][64] = {};
+    if (limit[variant][dev & 63] < smem) {
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int per_sm = 0;
+        KTB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, W * 32, smem));
+        resident[variant][dev & 63] = per_sm * num_sms(dev);
+        limit[variant][dev & 63] = smem;
+    }
+    if (resident[variant][dev & 63] < G) { set_error("ep_block: %d CTAs cannot be co-resident on this device", G); return KTB200_EINVAL; }
+    return KTB200_OK;
+}
+
+// Cooperative launch with programmatic stream serialization (the cooperative attribute alone where a driver refuses both).
+static int ep_block_launch(const void* fn, int G, int W, size_t smem, EpParams& pp, cudaStream_t s) {
+    static const int coop = [] { const char* e = getenv("KTB200_BLK_COOP"); return e ? atoi(e) : 1; }();
+    static const int pdl = [] { const char* e = getenv("KTB200_BLK_PDL"); return e ? atoi(e) : 1; }();
+    void* args[] = {&pp};
+    cudaLaunchConfig_t lc{};
+    lc.gridDim = dim3(G); lc.blockDim = dim3(W * 32); lc.dynamicSmemBytes = smem; lc.stream = s;
+    cudaLaunchAttribute at[2];
+    int na = 0;
+    if (coop) { at[na].id = cudaLaunchAttributeCooperative; at[na].val.cooperative = 1; na++; }
+    if (pdl) { at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[na].val.programmaticStreamSerializationAllowed = 1; na++; }
+    lc.attrs = at; lc.numAttrs = na;
+    cudaError_t le = cudaLaunchKernelExC(&lc, fn, args);
+    if (le != cudaSuccess && coop && pdl && (le == cudaErrorNotSupported || le == cudaErrorInvalidValue)) {
+        (void)cudaGetLastError();
+        lc.numAttrs = 1;
+        le = cudaLaunchKernelExC(&lc, fn, args);
+    }
+    if (le != cudaSuccess) { set_error("ep_block launch failed: %s", cudaGetErrorString(le)); return KTB200_ECUDA; }
+    count_launch(1);
+    return KTB200_OK;
+}
+
+// Shared-memory plan of moe_ep_block_kernel<GU, D> (layout at the kernel): the most warps (12 down to 4), then for them the
+// largest down chunk pa (16 down to 2), within the opt-in limit.  False when no such pair fits.
+struct EpKqPlan { int W, pa; size_t region_a, ep_off, smem; };
+static bool ep_kq_plan(int nblk, int nb, int n_experts, int gu_kbs, int gu_block, int d_kbs, int d_block, int nrows_max, EpKqPlan& pl) {
+    const size_t cap = 232448 - 1024;
+    const size_t unit = (size_t)2 * nblk * gu_block, item = (size_t)4 * nb * d_block;
+    const size_t ring = kEpKqSlots * (2 * unit > item ? 2 * unit : item);
+    // blk_select's scratch sits behind one Q8_K row of 8 sums per block; two rows of GU's layout; pa entries of D's
+    const size_t sel = ep_x_slot_bytes<8>(nblk) + ((size_t)2 * n_experts + 32 + 4 * kGateWarps) * 4;
+    const size_t x2 = (size_t)2 * (((size_t)nblk * (kActBlkStride + 2 * gu_kbs + 4) + 15) & ~(size_t)15);
+    for (int W = kBlockWarpsLo; W >= 4; W--) {
+        for (int pa = 16; pa >= 2; pa--) {
+            size_t ra = sel > x2 ? sel : x2;
+            const size_t aqb = (size_t)pa * nb * (kActBlkStride + 2 * d_kbs + 4);
+            if (aqb > ra) ra = aqb;
+            ra = (ra + 15) & ~(size_t)15;
+            const size_t ep_off = ((size_t)kBlockSharedBytes + ra + 15) & ~(size_t)15;
+            size_t off = ep_off + ((sizeof(EpShared) + 15) & ~(size_t)15) + (size_t)nrows_max * (kEpWorldMax + pa) * 4;
+            off = (off + 15) & ~(size_t)15;
+            const size_t smem = off + (((size_t)W * kEpKqSlots * 8 + 15) & ~(size_t)15) + (size_t)W * ring;
+            if (smem <= cap) { pl = EpKqPlan{W, pa, ra, ep_off, smem}; return true; }
+        }
+    }
+    return false;
+}
+
+static const char* kq_name(int t) {
+    return t == KTB200_TYPE_Q2_K ? "Q2_K" : t == KTB200_TYPE_Q3_K ? "Q3_K" : t == KTB200_TYPE_Q4_K ? "Q4_K" : "Q6_K";
+}
+
+template <class GU>
+static const void* ep_kq_kernel(int down_fmt, int down_type) {
+    if (down_fmt == FMT_Q4K) return (const void*)moe_ep_block_kernel<GU, BulkQ4K>;
+    if (down_fmt == FMT_Q6K4T) return (const void*)moe_ep_block_kernel<GU, BulkQ6K4T>;
+    return down_type == KTB200_TYPE_Q2_K ? (const void*)moe_ep_block_kernel<GU, BulkQ2K> : (const void*)moe_ep_block_kernel<GU, BulkQ3K>;
+}
+
+// Q2_K / Q3_K routed gate/up (ktb200_moe_ep_block_forward has checked the arguments every configuration shares)
+static int ep_block_kq_forward(const ktb200_gate_config* gc, ktb200_moe* m, ktb200_mlp* sh, const ktb200_ep_comm* comm, const void* x_own,
+                               void* y_out, int64_t* idx, float* w, int phase_mask, void* stream, FmtId fd) {
+    const ktb200_moe_config& c = m->cfg;
+    const int k = gc->top_k, world = comm->world;
+    const int nblk = c.hidden_size / QK_K, nb = c.intermediate_size / QK_K;
+    const bool q2 = c.gate_type == KTB200_TYPE_Q2_K;
+    if (sh && (sh->H != c.hidden_size || sh->hidden_type != c.hidden_type)) {
+        set_error("ep_block: the shared expert's hidden size / type differ from the routed experts'"); return KTB200_EINVAL;
+    }
+    if (!ep_gate_ok(gc, k) || nblk % BulkQ2K::kNblkMultiple || nblk < 4 || c.hidden_size > 16384 || c.hidden_size % 16) {
+        set_error("ep_block: unsupported configuration (Q2_K / Q3_K gate/up rows need a multiple of 1024 columns, at most 16384)");
+        return KTB200_EINVAL;
+    }
+    const int d_kbs = fd == FMT_Q6K4T ? BulkQ6K4T::kBs : fd == FMT_Q4K ? BulkQ4K::kBs : c.down_type == KTB200_TYPE_Q2_K ? BulkQ2K::kBs : BulkQ3K::kBs;
+    const int d_block = fd == FMT_Q6K4T ? SZ_Q6_K : fd == FMT_Q4K ? SZ_Q4_K : c.down_type == KTB200_TYPE_Q2_K ? SZ_Q2_K : SZ_Q3_K;
+    if ((size_t)4 * nb * d_block % 16) { set_error("ep_block: %s down rows of %d blocks: a 4-row item is not 16-byte sized", kq_name(c.down_type), nb); return KTB200_EINVAL; }
+    const int dev = m->device;
+    int G = num_sms(dev);
+    if (G > c.intermediate_size / 2) G = c.intermediate_size / 2;
+    if (G > c.hidden_size / 4) G = c.hidden_size / 4;
+    if (world * k >= G) { set_error("ep_block: grid too small for %d pairs", world * k); return KTB200_EINVAL; }
+    EpParams pp{};
+    BlockParams& p = pp.b;
+    p.nrows_max = ((c.hidden_size / 4 + G - 1) / G) * 4;
+    EpKqPlan pl;
+    if (!ep_kq_plan(nblk, nb, gc->n_experts, q2 ? BulkQ2K::kBs : BulkQ3K::kBs, q2 ? SZ_Q2_K : SZ_Q3_K, d_kbs, d_block, p.nrows_max, pl)) {
+        set_error("ep_block: %s gate/up rows of %d columns and %s down rows of %d columns leave no room for 4 warps and 2 down "
+                  "entries in shared memory", kq_name(c.gate_type), c.hidden_size, kq_name(c.down_type), c.intermediate_size);
+        return KTB200_EINVAL;
+    }
+    int rc = ep_block_params(pp, gc, m, sh, comm, x_own, y_out, idx, w, phase_mask);
+    if (rc) return rc;
+    const size_t unit = (size_t)2 * nblk * (q2 ? SZ_Q2_K : SZ_Q3_K), item = (size_t)4 * nb * d_block;
+    p.ring_bytes = (int)(kEpKqSlots * (2 * unit > item ? 2 * unit : item));
+    p.region_a = (int)pl.region_a;
+    pp.x.pa = pl.pa;
+    pp.x.ep_off = (int)pl.ep_off;
+    const void* fn = q2 ? ep_kq_kernel<BulkQ2K>(fd, c.down_type) : ep_kq_kernel<BulkQ3K>(fd, c.down_type);
+    const int variant = 2 + (q2 ? 0 : 4) + (fd == FMT_Q4K ? 0 : fd == FMT_Q6K4T ? 1 : c.down_type == KTB200_TYPE_Q2_K ? 2 : 3);
+    rc = ep_block_resident(fn, variant, G, pl.W, pl.smem, dev);
+    if (rc) return rc;
+    // the shared expert's rounded output goes into y first, with the combine phase (whose sum adds to it)
+    if (sh && (phase_mask & 4)) {
+        rc = ktb200_mlp_forward(sh, 1, x_own, y_out, 0, nullptr, stream);
+        if (rc) return rc;
+    }
+    return ep_block_launch(fn, G, pl.W, pl.smem, pp, (cudaStream_t)stream);
+}
+}  // namespace ktb
+
 extern "C" int ktb200_moe_ep_block_forward(const ktb200_gate_config* gc, ktb200_moe* m, ktb200_mlp* sh, const ktb200_ep_comm* comm,
                                            const void* x_own, void* y_out, int64_t* idx, float* w, int phase_mask, void* stream) {
     if (!gc || !m || !comm || !x_own || !y_out || !idx || !w) { set_error("ep_block: null pointer"); return KTB200_EINVAL; }
@@ -1264,18 +1742,18 @@ extern "C" int ktb200_moe_ep_block_forward(const ktb200_gate_config* gc, ktb200_
     for (int t : {c.gate_type, c.up_type, c.down_type})
         if (is_iquant(t)) { set_error("ep_block: %s experts are not supported by the expert-parallel kernel", iquant_name(t)); return KTB200_EINVAL; }
     const FmtId fd = pick_fmt(c.down_type, m->down_layout);
+    DeviceGuard guard(m->device);
+    if ((c.gate_type == KTB200_TYPE_Q2_K || c.gate_type == KTB200_TYPE_Q3_K) && c.up_type == c.gate_type &&
+        (fd == FMT_Q4K || fd == FMT_Q6K4T || c.down_type == KTB200_TYPE_Q2_K || c.down_type == KTB200_TYPE_Q3_K))
+        return ep_block_kq_forward(gc, m, sh, comm, x_own, y_out, idx, w, phase_mask, stream, fd);
     const bool sh_ok = !sh || (sh->H == c.hidden_size && sh->I == c.intermediate_size && sh->hidden_type == c.hidden_type &&
                                sh->gate_type == c.gate_type && sh->up_type == c.up_type && sh->down_type == c.down_type &&
                                sh->gu_soa == m->gu_soa && sh->down_layout == m->down_layout && c.use_silu);
     const int nblk = c.hidden_size / QK_K, nb = c.intermediate_size / QK_K;
     const bool ok = sh_ok && c.gate_type == KTB200_TYPE_Q4_K && c.up_type == KTB200_TYPE_Q4_K && (fd == FMT_Q6K4T || fd == FMT_Q4K) && nblk >= 16 &&
-                    nblk <= 32 && c.hidden_size % 16 == 0 && gc->n_experts <= kGateThreads * kGateEPT && gc->n_experts > 0 && gc->n_group >= 1 &&
-                    gc->n_group <= 32 && gc->n_experts % gc->n_group == 0 && gc->topk_group >= 1 && gc->topk_group <= gc->n_group && gc->weight &&
-                    gc->scoring >= 0 && gc->scoring <= 1 && gc->topk_method >= 0 && gc->topk_method <= 2 && k <= gc->n_experts && c.hidden_size <= 16384;
+                    nblk <= 32 && c.hidden_size % 16 == 0 && ep_gate_ok(gc, k) && c.hidden_size <= 16384;
     if (!ok) { set_error("ep_block: unsupported configuration (needs Q4_K gate/up rows of 4096..8192 columns, Q6_K/Q4_K down, shared expert of the same shapes)"); return KTB200_EINVAL; }
-    DeviceGuard guard(m->device);
     const int dev = m->device;
-    cudaStream_t s = (cudaStream_t)stream;
     EpParams pp{};
     BlockParams& p = pp.b;
     const int ns = k + (sh ? 1 : 0);
@@ -1306,58 +1784,13 @@ extern "C" int ktb200_moe_ep_block_forward(const ktb200_gate_config* gc, ktb200_
         if (off + tail <= 232448 - 1024) { pa = cand; p.region_a = (int)ra; pp.x.ep_off = (int)off; smem = off + tail; break; }
     }
     if (pa < 2) { set_error("ep_block: shared memory budget"); return KTB200_EINVAL; }
-
-    const int S = gate_splits(gc->n_experts, gc->hidden_size, num_sms(dev));
-    p.g = GateParams{gc->weight, x_own, gc->hidden_type, gc->n_experts, gc->hidden_size, 1, S, k, gc->n_group, gc->topk_group,
-                     gc->scoring, gc->topk_method, gc->norm_topk_prob, gc->routed_scaling_factor, gc->bias, m->blk_partial, nullptr,
-                     idx, w, nullptr, nullptr};
-    p.w_gate = c.gate_proj; p.w_up = c.up_proj; p.w_down = c.down_proj;
-    p.s_gate = sh ? sh->gate : nullptr; p.s_up = sh ? sh->up : nullptr; p.s_down = sh ? sh->down : nullptr;
-    p.n_local = c.expert_num; p.id_offset = c.expert_id_offset;
-    p.H = c.hidden_size; p.I = c.intermediate_size; p.k = k; p.hidden_type = c.hidden_type; p.use_silu = c.use_silu;
-    p.inter = m->inter; p.out = y_out; p.sync = m->blk_sync + 2 * (m->blk_flip++ & 1u); p.trace = g_btrace;
-    p.prime_u = 3; p.prime_d = 2;
-    pp.x.rank = rank; pp.x.world = world; pp.x.phase_mask = phase_mask; pp.x.pa = pa;
-    pp.x.msg_bytes = (int)ktb200_ep_msg_bytes(c.hidden_size, c.hidden_type);
-    pp.x.inter_shared_row = world * k;
-    pp.x.shared_out = m->blk_partial + 16384;
-    for (int r = 0; r < world; r++) {
-        if (!comm->token_bufs[r] || !comm->partial_bufs[r] || !comm->flag_bufs[r]) { set_error("ep_block: null peer pointer for rank %d", r); return KTB200_EINVAL; }
-        pp.x.msg[r] = (uint8_t*)comm->token_bufs[r]; pp.x.part[r] = comm->partial_bufs[r]; pp.x.flags[r] = comm->flag_bufs[r];
-    }
-    void* args[] = {&pp};
+    const int rc = ep_block_params(pp, gc, m, sh, comm, x_own, y_out, idx, w, phase_mask);
+    if (rc) return rc;
+    pp.x.pa = pa;
     const void* fn = fd == FMT_Q6K4T ? (const void*)moe_ep_block_kernel<BulkQ6K4T> : (const void*)moe_ep_block_kernel<BulkQ4K>;
-    {
-        static size_t limit[2][64] = {};
-        static int resident[2][64] = {};
-        const int v = fd == FMT_Q6K4T ? 1 : 0;
-        if (limit[v][dev & 63] < smem) {
-            KTB_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            int per_sm = 0;
-            KTB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, W * 32, smem));
-            resident[v][dev & 63] = per_sm * num_sms(dev);
-            limit[v][dev & 63] = smem;
-        }
-        if (resident[v][dev & 63] < G) { set_error("ep_block: %d CTAs cannot be co-resident on this device", G); return KTB200_EINVAL; }
-    }
-    static const int coop = [] { const char* e = getenv("KTB200_BLK_COOP"); return e ? atoi(e) : 1; }();
-    static const int pdl = [] { const char* e = getenv("KTB200_BLK_PDL"); return e ? atoi(e) : 1; }();
-    cudaLaunchConfig_t lc{};
-    lc.gridDim = dim3(G); lc.blockDim = dim3(W * 32); lc.dynamicSmemBytes = smem; lc.stream = s;
-    cudaLaunchAttribute at[2];
-    int na = 0;
-    if (coop) { at[na].id = cudaLaunchAttributeCooperative; at[na].val.cooperative = 1; na++; }
-    if (pdl) { at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[na].val.programmaticStreamSerializationAllowed = 1; na++; }
-    lc.attrs = at; lc.numAttrs = na;
-    cudaError_t le = cudaLaunchKernelExC(&lc, fn, args);
-    if (le != cudaSuccess && coop && pdl && (le == cudaErrorNotSupported || le == cudaErrorInvalidValue)) {
-        (void)cudaGetLastError();
-        lc.numAttrs = 1;
-        le = cudaLaunchKernelExC(&lc, fn, args);
-    }
-    if (le != cudaSuccess) { set_error("ep_block launch failed: %s", cudaGetErrorString(le)); return KTB200_ECUDA; }
-    count_launch(1);
-    return KTB200_OK;
+    const int rr = ep_block_resident(fn, fd == FMT_Q6K4T ? 1 : 0, G, W, smem, dev);
+    if (rr) return rr;
+    return ep_block_launch(fn, G, W, smem, pp, (cudaStream_t)stream);
 }
 
 // Prefetch hint: while this handle's block kernel streams its down projection, pull up to three byte ranges into L2 — the

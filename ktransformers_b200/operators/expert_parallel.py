@@ -160,16 +160,16 @@ def attach_expert_parallel(model: torch.nn.Module, hidden_size: int, hidden_type
     """Give every injected MoE block of `model` whose experts are sharded the same PeerExchange; its step counts expire
     after one use by each of those blocks."""
     from ..native import RAWINT4_G32
-    from ..util.custom_gguf import GGML_NAMES, B200_EP_GATE_UP_TYPES, B200_EP_DOWN_TYPES
+    from ..util.custom_gguf import GGML_NAMES, B200_EP_TYPE_SETS
     for m in model.modules():
         gen = getattr(getattr(m, "experts", None), "generate_experts", None)
         if not hasattr(m, "_block_handles") or getattr(gen, "gate_type", None) is None:
             continue
         types = (gen.gate_type, gen.up_type, gen.down_type)
         names = ["RAWINT4_G32" if t == RAWINT4_G32 else GGML_NAMES.get(int(t), str(t)) for t in types]
-        if names[0] not in B200_EP_GATE_UP_TYPES or names[1] not in B200_EP_GATE_UP_TYPES or names[2] not in B200_EP_DOWN_TYPES:
-            # the single-launch NVLink kernel takes Q4_K gate/up and Q4_K/Q6_K down only, and without it a sharded block would
-            # return its shard's partial sums as the layer output
+        if names[0] != names[1] or (names[0], names[2]) not in B200_EP_TYPE_SETS:
+            # the single-launch NVLink kernel takes these sets only, and without it a sharded block would return its shard's
+            # partial sums as the layer output
             raise ValueError(f"attach_expert_parallel: {getattr(m, 'key', type(m).__name__)} has {'/'.join(names)} experts "
                              "(gate/up/down), which the expert-parallel kernel does not support")
     gens = [m.experts.generate_experts for m in model.modules() if hasattr(m, "_block_handles")

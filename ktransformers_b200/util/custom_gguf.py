@@ -70,9 +70,9 @@ B200_EXPERT_TYPES = B200_WEIGHT_TYPES | {"IQ1_S", "IQ2_XXS"}
 # what the routed-expert loaders accept: kept apart from B200_EXPERT_TYPES, whose value callers and tests rely on
 B200_ROUTED_EXPERT_TYPES = B200_EXPERT_TYPES | {"IQ1_M"}
 B200_DEQUANT_TYPES = B200_ROUTED_EXPERT_TYPES | {"Q8_0", "F32", "F16", "BF16"}
-# what the single-launch expert-parallel kernel takes: Q4_K gate/up, Q4_K or Q6_K down
-B200_EP_GATE_UP_TYPES = {"Q4_K"}
-B200_EP_DOWN_TYPES = {"Q4_K", "Q6_K"}
+# the (gate/up, down) type sets the single-launch expert-parallel kernel takes (gate and up of one type): Q4_K gate/up with
+# Q4_K or Q6_K down, and Q2_K or Q3_K gate/up with Q2_K, Q3_K, Q4_K or Q6_K down (llama.cpp's Q2_K, Q3_K_S and Q3_K_M files)
+B200_EP_TYPE_SETS = {("Q4_K", "Q4_K"), ("Q4_K", "Q6_K")} | {(gu, d) for gu in ("Q2_K", "Q3_K") for d in ("Q2_K", "Q3_K", "Q4_K", "Q6_K")}
 
 TORCH_TO_GGML_HIDDEN = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 30}
 
