@@ -13,8 +13,9 @@
 //   * the barrier is split into arrive / wait; the shared expert's first rows are requested in between, never before
 //     the arrive: a fence issued with bulk copies in flight waits for them (measured again on H100: one gpu-scope fence
 //     per CTA and Q8_K block inside the gate/up stream cost ~10 us per layer);
-//   * x is quantised under the barrier (the router reads x itself); the shared expert's gate/up rows are consumed by
-//     warps 4.. while warps 0..3 run the top-k;
+//   * the router's weights are bulk-copied into the warps' rings and x is quantised while they land, before the barrier
+//     (the router reads x itself); the shared expert's gate/up rows are consumed by warps 4.. while warps 0..3 run the
+//     top-k;
 //   * gate/up is entry-major: every CTA computes a slice of every entry, in work-list order, so the entries complete
 //     one after another across the grid.  The producers only store (`inter` starts out as kInterEmpty: a consumer sees
 //     each value arrive, no fence or count is needed).  Each Q8_K block is quantised once, by the first CTA to claim
@@ -23,7 +24,7 @@
 //     down tiles;
 //   * the selection runs redundantly in every CTA (128 threads, from the same partial sums in the same order): no
 //     second barrier and no global round trip for the ids;
-//   * programmatic dependent launch: the router's weight loads are issued before griddepcontrol.wait, so the next
+//   * programmatic dependent launch: the router's weight copies are issued before griddepcontrol.wait, so the next
 //     layer's launch latency and first DRAM round trip hide under this layer's tail.
 //
 // Arithmetic, summation orders and rounding are exactly those of the separate kernels (gate.cuh, gemv_bulk.cuh):
@@ -98,14 +99,16 @@ __device__ __forceinline__ void wait_ge(const unsigned* p, unsigned target, unsi
 
 // Grid-wide barrier over the (co-resident) CTAs, split in two so that work which does not depend on the other CTAs —
 // here: requesting the next phase's weights — can be issued in between.  `gen` counts the barriers passed.  The arrive
-// side fences BEFORE any of those requests exist (a fence issued with bulk copies in flight waits for them: measured).
+// is one release-ordered add after the CTA barrier (it publishes every thread's earlier stores at GPU scope, which
+// __syncthreads() ordered before it), issued BEFORE any of those requests exist (a fence issued with bulk copies in
+// flight waits for them: measured).
+__device__ __forceinline__ void red_release_gpu_add(unsigned* p, unsigned v) {
+    asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
 __device__ __forceinline__ void grid_arrive(unsigned* counter, unsigned& gen) {
     __syncthreads();
     gen++;
-    if (threadIdx.x == 0) {
-        __threadfence();
-        atomicAdd(counter, 1u);
-    }
+    if (threadIdx.x == 0) red_release_gpu_add(counter, 1u);
 }
 __device__ __forceinline__ void grid_wait(unsigned* counter, unsigned gen) {
     if (threadIdx.x == 0) {
@@ -200,7 +203,8 @@ __device__ __forceinline__ void blk_quantize_x(int t) {
     }
 }
 
-// router partial sums: unit = (expert row e, column split s); same loop and summation order as gate_dot<1> (gate.cuh)
+// router partial sums (moe_ep_block_kernel): unit = (expert row e, column split s); same loop and summation order as
+// gate_dot<1> (gate.cuh)
 // `waited`: whether this thread already passed griddep_wait() — the router's WEIGHT loads are issued before it (they do
 // not depend on the previous kernel), x is read after it.
 __device__ __forceinline__ void blk_router(int t, bool& waited) {
@@ -246,6 +250,68 @@ __device__ __forceinline__ void blk_router(int t, bool& waited) {
     if (!waited) { griddep_wait(); waited = true; }
 }
 
+// The same partial sums with the weights bulk-copied into the warp's ring (slot 0's mbarrier; `phase` bit 0 is its
+// parity) instead of held in registers: the first unit's weights are requested before griddep_wait(), and x is quantised
+// while they land (the quantisation is off the path to the grid barrier).  A unit longer than the ring is walked in
+// pieces of whole 32-float4 strides, so every lane still sums columns lane + 32 q in ascending order, then warp_sum:
+// bit-identical to blk_router and gate_dot<1>.  The ring is free again when this returns (no copy in flight).
+__device__ __forceinline__ void blk_router_ring(int t, bool& waited, uint32_t bar, uint32_t ring_u32, uint32_t& phase) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    const BlockParams& p = reinterpret_cast<const BlockShared*>(smem)->prm;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, W = blockDim.x >> 5;
+    const int E = p.g.E, S = p.g.S, n4 = p.H / 4, CH = p.ring_bytes / (16 * 32) * 32;
+    const int gw = blockIdx.x * W + warp, tw = gridDim.x * W;
+    const float4* ring = reinterpret_cast<const float4*>(smem + (ring_u32 - (uint32_t)__cvta_generic_to_shared(smem)));
+    auto request = [&](int u, int cs) {   // float4 [cs, cs + CH) of unit u's columns -> ring
+        const int s = u / E, e = u - s * E;
+        const int c0 = (int)((long)n4 * s / S), nc4 = (int)((long)n4 * (s + 1) / S) - c0;
+        if (lane == 0) {
+            const uint32_t bytes = (uint32_t)min(CH, nc4 - cs) * 16u;
+            mbar_expect_tx(bar, bytes);
+            bulk_g2s(ring_u32, reinterpret_cast<const float4*>(p.g.W + (long)e * p.H) + c0 + cs, bytes, bar);
+        }
+    };
+    if (gw < E * S) request(gw, 0);
+    if (!waited) { griddep_wait(); waited = true; }
+    blk_quantize_x(t);
+    block_stamp(p, 1);
+    for (int u = gw; u < E * S; u += tw) {
+        const int s = u / E;
+        const int c0 = (int)((long)n4 * s / S), nc4 = (int)((long)n4 * (s + 1) / S) - c0;
+        const long xbase = (long)t * n4 + c0;
+        float acc = 0.f;
+        for (int cs = 0; cs < nc4; cs += CH) {
+            if (u != gw || cs != 0) request(u, cs);
+            const int n = min(CH, nc4 - cs);
+            mbar_wait(bar, phase & 1u);
+            phase ^= 1u;
+            constexpr int NQ = 10;
+            for (int cb = lane; cb < n; cb += 32 * NQ) {
+                float4 xv[NQ];
+#pragma unroll
+                for (int q = 0; q < NQ; q++) {
+                    const int c = cb + 32 * q;
+                    if (c < n) xv[q] = load_x4(p.g.x, xbase + cs + c, p.hidden_type);
+                }
+#pragma unroll
+                for (int q = 0; q < NQ; q++) {
+                    const int c = cb + 32 * q;
+                    if (c < n) {
+                        const float4 w = ring[c];
+                        acc = fmaf(w.x, xv[q].x, acc);
+                        acc = fmaf(w.y, xv[q].y, acc);
+                        acc = fmaf(w.z, xv[q].z, acc);
+                        acc = fmaf(w.w, xv[q].w, acc);
+                    }
+                }
+            }
+            __syncwarp();   // every lane is done with the ring before the next copy into it
+        }
+        const float v = warp_sum(acc);
+        if (lane == 0) p.g.partial[((long)t * S + s) * E + (u - s * E)] = v;
+    }
+}
+
 // top-k selection (first 4 warps of EVERY CTA, identical results), work-list compaction, routing outputs (CTA 0)
 __device__ __forceinline__ void blk_select(int t) {
     extern __shared__ __align__(16) uint8_t smem[];
@@ -258,15 +324,16 @@ __device__ __forceinline__ void blk_select(int t) {
     }
     __syncthreads();
     block_stamp(p, 10);
-    if (threadIdx.x == 0) {
-        unsigned sk = 0;
-        int nv = p.s_gate ? 1 : 0;
-        for (int j = 0; j < k; j++) {
-            const long e = (long)sh.ids[j] - p.id_offset;
-            if (e < 0 || e >= p.n_local) sk |= 1u << j; else sh.vs[nv++] = j;
+    if (threadIdx.x < 32) {   // warp 0, lane j = slot j: the owned slots in slot order, after the shared expert (k <= 31)
+        const int j = threadIdx.x, e0 = p.s_gate ? 1 : 0;
+        const long e = j < k ? (long)sh.ids[j] - p.id_offset : -1;
+        const bool own = e >= 0 && e < p.n_local;
+        const unsigned m = __ballot_sync(0xffffffffu, own);
+        if (own) sh.vs[e0 + __popc(m & ((1u << j) - 1u))] = j;
+        if (j == 0) {
+            sh.nv = e0 + __popc(m);
+            sh.skip = ~m & ((1u << k) - 1u);
         }
-        sh.nv = nv;
-        sh.skip = sk;
     }
     if (blockIdx.x == 0 && threadIdx.x < k) {
         p.g.idx[(long)t * k + threadIdx.x] = sh.ids[threadIdx.x];
@@ -507,10 +574,10 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
             }
         };
         if (threadIdx.x < 36) sh.ent_state[threadIdx.x] = 0;
-        blk_router(t, waited);
+        blk_router_ring(t, waited, bar_u32, ring_u32, phase);   // quantises x too
         block_stamp(p, 2);
         grid_arrive(p.sync, gen);
-        // while the barrier completes: request the shared expert's first rows, then quantise x (the router read x itself)
+        // while the barrier completes: request the shared expert's first rows
         if (has_shared && warp >= kGateWarps) {
             int r0, nr;
             entry_slice(p.I, 0, r0, nr);
@@ -520,8 +587,6 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
 #pragma unroll
         for (int s = 0; s < SU; s++)
             if (s < p.prime_u) issue_u();
-        blk_quantize_x(t);
-        block_stamp(p, 1);
         grid_wait(p.sync, gen);
         block_stamp(p, 3);
         const BlockLay L = block_layout<DownFmt::kBs>(p, smem);
@@ -533,20 +598,23 @@ __global__ void __launch_bounds__(MAXW * 32, 1) moe_block_kernel(const BlockPara
                 blk_select(t);
                 block_stamp(p, 4);
                 const int e0 = has_shared ? 1 : 0, nv = sh.nv;
-                int total = 0;
-                for (int e = e0; e < nv; e++) {
-                    int r0, len;
-                    entry_slice(p.I, e, r0, len);
-                    total += len;
-                }
+                // entries e0 .. nv - 1 are slices s0, s0 + 1, ... (mod G) of I (entry_slice): their rows telescope
+                const unsigned G = gridDim.x, s0 = (blockIdx.x + (unsigned)e0) % G;
+                auto rows_before = [&](unsigned sl) { return (int)(sl / G) * p.I + (int)((unsigned long long)p.I * (sl % G) / G); };
+                const int total = rows_before(s0 + (unsigned)(nv - e0)) - rows_before(s0);
                 start_list(e0, nv, warp, (total - warp + W - 1) / W, W);
 #pragma unroll
                 for (int s = 0; s < SU; s++) issue_u();
             }
             float acc_first = 0.f;
+            bool stamp_first = list == 1 && warp == 0;   // trace: warp 0's first routed gate/up row landed
             while (cleft > 0) {
                 mbar_wait(bar_u32 + 8 * slot_u, (phase >> slot_u) & 1u);
                 phase ^= 1u << slot_u;
+                if (stamp_first) {
+                    if (lane == 0) trace_stamp(p, 11);
+                    stamp_first = false;
+                }
                 const uint8_t* row0 = ring + slot_u * row_bytes;
                 float acc = 0.f;
                 if (lane < nblk)
