@@ -36,7 +36,7 @@ enum ktb200_ggml_type {
     KTB200_TYPE_F32 = 0, KTB200_TYPE_F16 = 1, KTB200_TYPE_Q8_0 = 8, KTB200_TYPE_Q2_K = 10,
     KTB200_TYPE_Q3_K = 11, KTB200_TYPE_Q4_K = 12, KTB200_TYPE_Q5_K = 13, KTB200_TYPE_Q6_K = 14,
     KTB200_TYPE_Q8_K = 15, KTB200_TYPE_IQ4_XS = 23, KTB200_TYPE_BF16 = 30,
-    /* ggml's codebook i-quants (DeepSeek-R1's 1.5-2-bit GGUF experts), raw ggml blocks of 256 values:
+    /* ggml's codebook i-quants (DeepSeek-V3's and R1's 1.5-3-bit GGUF experts), raw ggml blocks of 256 values:
      *   IQ2_XXS  66 B: fp16 d, then per 32-value sub-block two 32-bit words: four 8-bit indices into iq2xxs_grid, then
      *            four 7-bit indices into ksigns_iq2xs and the 4-bit scale s in bits 28..31; value = d*(2s+1)/8 * grid * sign
      *   IQ1_S    50 B: fp16 d, qs[32], qh uint16[8]; sub-block ib has ls = 2*((qh>>12)&7)+1, delta = qh bit 15 ? -1/8 : +1/8,
@@ -45,11 +45,17 @@ enum ktb200_ggml_type {
      *            l): bits 0-2 the high bits of its iq1s_grid index qs[l] | (nibble & 7) << 8, bit 3 the sign of its
      *            delta (+-1/8); 16-value half h (0..15) has ls = 2*((scales[h/4] >> 3(h%4)) & 7)+1; the fp16 d is the
      *            four top nibbles, scales[0] >> 12 lowest; value = d*ls*(grid + delta)
+     *   IQ3_XXS  98 B: fp16 d, qs[64], then per 32-value sub-block ib one 32-bit word: four 7-bit indices into ksigns_iq2xs
+     *            (bits 7l..7l+6 for values 8l..8l+7) and the 4-bit scale s in bits 28..31; 4-value group g (0..7) of ib is
+     *            iq3xxs_grid[qs[8ib+g]]; value = d*(2s+1)/4 * grid * sign
+     *   IQ3_S   110 B: fp16 d, qs[64], qh[8], signs[32], scales[4]; 4-value group j (0..63) is iq3s_grid[qs[j] | (bit j%8
+     *            of qh[j/8]) << 8], bit i of signs[k] negates value 8k+i, sub-block ib has s = nibble ib%2 (low for
+     *            even ib) of scales[ib/2]; value = d*(2s+1) * grid * sign
      * vec_dot_type Q8_K.  Routed experts only (ktb200_moe_create, any mix with the K-quants); linears, MLP handles and the
      * one-token expert-parallel entry points reject them.  ktb200_moe_forward runs them per (token, expert) pair below 80
      * tokens and on the grouped tensor-core GEMM from 80 (gate, up and down each in its own format).  The codebooks are
      * ktransformers_b200/csrc/iq_tables.h. */
-    KTB200_TYPE_IQ2_XXS = 16, KTB200_TYPE_IQ1_S = 19, KTB200_TYPE_IQ1_M = 29,
+    KTB200_TYPE_IQ2_XXS = 16, KTB200_TYPE_IQ3_XXS = 18, KTB200_TYPE_IQ1_S = 19, KTB200_TYPE_IQ3_S = 21, KTB200_TYPE_IQ1_M = 29,
     /* Not a ggml type: ggml's ids stay below 64, so 256 cannot collide with one.
      * Symmetric INT4 in groups of 32 with bf16 scales (compressed-tensors "pack-quantized", kt-kernel's RAWINT4; Kimi-K2's
      * routed experts), in the device layout ktb200_rawint4_pack writes: 144 B per 256 values of a row,

@@ -19,6 +19,8 @@
 #define SZ_IQ2_XXS 66    // fp16 d + 8 x (4 grid indices | signs + scale) words
 #define SZ_IQ1_S 50      // fp16 d + qs[32] + qh[8] (uint16)
 #define SZ_IQ1_M 56      // qs[32] + qh[16] + scales[4] (uint16, fp16 d in the top nibbles)
+#define SZ_IQ3_XXS 98    // fp16 d + qs[64] + 8 x (signs + scale) words
+#define SZ_IQ3_S 110     // fp16 d + qs[64] + qh[8] + signs[32] + scales[4]
 #define SZ_RAWINT4 144   // 8 bf16 scales + 256 nibbles (rawint4.cuh)
 
 namespace ktb {
@@ -93,15 +95,18 @@ __host__ __device__ inline bool is_kquant(int t) {
 // codebook i-quants: routed experts only (iq.cuh bulk kernels, generic per-pair fallback), no linear /
 // MLP / grouped / block / expert-parallel path
 __host__ __device__ inline bool is_iquant(int t) {
-    return t == KTB200_TYPE_IQ2_XXS || t == KTB200_TYPE_IQ1_S || t == KTB200_TYPE_IQ1_M;
+    return t == KTB200_TYPE_IQ2_XXS || t == KTB200_TYPE_IQ1_S || t == KTB200_TYPE_IQ1_M || t == KTB200_TYPE_IQ3_XXS ||
+           t == KTB200_TYPE_IQ3_S;
 }
 static inline const char* iquant_name(int t) {
-    return t == KTB200_TYPE_IQ1_S ? "IQ1_S" : t == KTB200_TYPE_IQ2_XXS ? "IQ2_XXS" : t == KTB200_TYPE_IQ1_M ? "IQ1_M" : "?";
+    return t == KTB200_TYPE_IQ1_S ? "IQ1_S" : t == KTB200_TYPE_IQ2_XXS ? "IQ2_XXS" : t == KTB200_TYPE_IQ1_M ? "IQ1_M"
+         : t == KTB200_TYPE_IQ3_XXS ? "IQ3_XXS" : t == KTB200_TYPE_IQ3_S ? "IQ3_S" : "?";
 }
 // block geometry including the i-quants.  Kept apart from type_size / blck_size, which every kernel inlines for its hidden
 // type: a longer switch there would change the code of kernels that never see an i-quant.
 __host__ __device__ inline long weight_block_bytes(int t) {
-    return t == KTB200_TYPE_IQ2_XXS ? SZ_IQ2_XXS : t == KTB200_TYPE_IQ1_S ? SZ_IQ1_S : t == KTB200_TYPE_IQ1_M ? SZ_IQ1_M : type_size(t);
+    return t == KTB200_TYPE_IQ2_XXS ? SZ_IQ2_XXS : t == KTB200_TYPE_IQ1_S ? SZ_IQ1_S : t == KTB200_TYPE_IQ1_M ? SZ_IQ1_M
+         : t == KTB200_TYPE_IQ3_XXS ? SZ_IQ3_XXS : t == KTB200_TYPE_IQ3_S ? SZ_IQ3_S : type_size(t);
 }
 __host__ __device__ inline long weight_block_elems(int t) { return is_iquant(t) ? QK_K : blck_size(t); }
 // not a K-quant: it has its own kernels (rawint4.cuh) and no path through the generic K-quant ones
@@ -157,10 +162,12 @@ __device__ __forceinline__ float warp_sum(float v) {
 // ------------------------------------------------------------------ hidden-type conversions
 __device__ __forceinline__ float fp16_bits_to_f32(uint16_t h) { return __half2float(__ushort_as_half(h)); }
 
-// ------------------------------------------------------------------ IQ1_S / IQ1_M / IQ2_XXS arithmetic shared by iq.cuh and grouped.cu
+// ------------------------------------------------------------------ IQ1_S / IQ1_M / IQ2_XXS / IQ3 arithmetic shared by iq.cuh and grouped.cu
 // a super-block's fp32 term (DESIGN.md §2): ((d / 8) * dx) * S with the exact integer S of the super-block; also the term
 // (d * dx) * isum of Q3_K and Q6_K (gemv_bulk.cuh BulkQ3K, grouped.cu)
 __device__ __forceinline__ float iq_d8(uint16_t d_bits) { return fp16_bits_to_f32(d_bits) * 0.125f; }
+// IQ3_XXS's d / 4: the reference's final 0.25 folded into the scale (exact, a power of two)
+__device__ __forceinline__ float iq_d4(uint16_t d_bits) { return fp16_bits_to_f32(d_bits) * 0.25f; }
 __device__ __forceinline__ float iq_term(float d8, float dx, int isum) { return (d8 * dx) * (float)isum; }
 // IQ1_M's fp16 d: the top nibbles of its four scale words (s01 = scales[0] | scales[1] << 16, s23 likewise), scales[0]'s lowest
 __device__ __forceinline__ uint16_t iq1m_d_bits(uint32_t s01, uint32_t s23) {
@@ -171,7 +178,7 @@ __device__ __forceinline__ uint16_t iq1m_d_bits(uint32_t s01, uint32_t s23) {
 __device__ __forceinline__ float kq_min_term(float d, float dmin, float dx, int isum, float msum) {
     return (d * dx) * (float)isum - (dmin * dx) * msum;
 }
-// an IQ2_XXS sign pattern (ksigns_iq2xs byte) as byte masks: value = (grid ^ m) - m per byte
+// an IQ2_XXS / IQ3_XXS sign pattern (ksigns_iq2xs byte), or an IQ3_S sign byte, as byte masks: value = (grid ^ m) - m per byte
 __device__ __forceinline__ uint2 iq2_sign_masks(uint32_t s) {
     uint32_t lo = 0, hi = 0;
 #pragma unroll

@@ -13,16 +13,17 @@
 //   FmtQ4K    raw GGUF block_q4_K (144 B, already 16-byte aligned)   unit = 16 B of qs = 32 weights, 4 blocks/step
 //   FmtQ5K    raw GGUF block_q5_K (176 B, 16-byte aligned)           unit = 16 B qs + qh   = 32 weights, 4 blocks/step
 //   FmtQ6K8   block_q6_K re-laid as "8-row SoA" (moe.cu repack)      unit = 48 B           = 64 weights, 8 blocks/step
-//   FmtGenK   any raw K-quant / IQ4_XS / IQ2_XXS / IQ1_S / IQ1_M through byte loads (fallback)
+//   FmtGenK   any raw K-quant / IQ4_XS / IQ2_XXS / IQ1_S / IQ1_M / IQ3_XXS / IQ3_S through byte loads (fallback)
 //                                                                    unit = 16 weights,              2 blocks/step
 #pragma once
 #include "common.cuh"
 
-// The IQ1_S / IQ2_XXS codebooks (device globals) only exist in the translation units that dispatch those types
+// The IQ codebooks (device globals) only exist in the translation units that dispatch those types
 // (moe.cu, dequant.cu define KTB_IQ_CODEBOOKS); elsewhere unpack_group16 has no IQ cases and no table is emitted.
 #ifdef KTB_IQ_CODEBOOKS
 #define KTB_IQ_TABLE static __device__ const
 #include "iq_tables.h"
+#include "iq3_tables.h"
 #endif
 
 namespace ktb {
@@ -450,6 +451,39 @@ __device__ inline void unpack_group16(int type, const uint8_t* b, int g, GroupK&
                 for (int j = 0; j < 8; j++) {
                     const int gv = ldg_u8(&ktb_iq2xxs_grid[idx][j]);
                     v[8 * l + j] = (int8_t)(((signs >> j) & 1) ? -gv : gv);
+                }
+            }
+            break;
+        }
+        case KTB200_TYPE_IQ3_XXS: {
+            // d/4 and ls = 2s+1: the reference's final 0.25 folded into the scale; values +-grid (4..62)
+            o.d = fp16_bits_to_f32(ldg_u16(b)) * 0.25f;
+            const int ib = g >> 1, l0 = 2 * (g & 1);
+            const uint8_t* q = b + 2 + 8 * ib;
+            const uint32_t aux = (uint32_t)ldg_u16(b + 66 + 4 * ib) | ((uint32_t)ldg_u16(b + 68 + 4 * ib) << 16);
+            o.isc = 2 * (int)(aux >> 28) + 1;
+            for (int l = 0; l < 2; l++) {
+                const uint32_t signs = ldg_u8(&ktb_ksigns_iq2xs[(aux >> (7 * (l0 + l))) & 127]);
+                for (int j = 0; j < 8; j++) {
+                    const int gv = ldg_u8(&ktb_iq3xxs_grid[ldg_u8(q + 2 * (l0 + l) + (j >> 2))][j & 3]);
+                    v[8 * l + j] = (int8_t)(((signs >> j) & 1) ? -gv : gv);
+                }
+            }
+            break;
+        }
+        case KTB200_TYPE_IQ3_S: {
+            // d and ls = 2s+1; values +-grid (1..15).  16-value group g: 4-value groups 4g..4g+3, sign bytes 2g, 2g+1
+            o.d = fp16_bits_to_f32(ldg_u16(b));
+            const int ib = g >> 1;
+            o.isc = 2 * (int)((ldg_u8(b + 106 + (ib >> 1)) >> (4 * (ib & 1))) & 15) + 1;
+            const uint32_t qh = ldg_u8(b + 66 + ib);
+            const uint32_t signs = (uint32_t)ldg_u8(b + 74 + 2 * g) | ((uint32_t)ldg_u8(b + 75 + 2 * g) << 8);
+            for (int k = 0; k < 4; k++) {
+                const int j = 4 * g + k;   // 4-value group of the block; j % 8 = 4 (g & 1) + k
+                const int idx = ldg_u8(b + 2 + j) | (int)(((qh >> (j & 7)) & 1) << 8);
+                for (int i = 0; i < 4; i++) {
+                    const int gv = ldg_u8(&ktb_iq3s_grid[idx][i]);
+                    v[4 * k + i] = (int8_t)(((signs >> (4 * k + i)) & 1) ? -gv : gv);
                 }
             }
             break;

@@ -46,6 +46,13 @@
 // MMAs (one K = 32 MMA per sub-block against the 64-row B, the two halves' ls as the header's signed bytes) and Q3_K's finish
 // with d / 8.  56-byte blocks are 8-byte aligned: a thread's 8 B of qs, 4 B of qh and the 8-byte scale field (which holds d) are
 // plain cp.async words in FMT 2's 48-byte raw slots; own plan constants (kGSmemM) for the 64-row B.
+// IQ3_XXS (FMT 9) and IQ3_S (FMT 10), the experts of llama.cpp's 3-bit i-quant files: FMT 3 with 4-value codebook groups.  The
+// producers expand +-grid (IQ3_XXS 256 x 4, values 4..62, signs through IQ2_XXS's masks; IQ3_S 512 x 4, values 1..15, its sign
+// bytes through a 256-entry mask table) into the s8 A tile; the consumers are FMT 3's (32-row B, one K = 32 MMA per sub-block,
+// ls = 2s + 1 from the header) and the finish is iq_term with d / 4 (IQ3_XXS) or d (IQ3_S).  A thread's share of a stage
+// (two sub-blocks) does not fit the 20 payload bytes of FMT 2's raw slots: the covering 4-byte words of the 98 / 110-byte
+// blocks (2-byte aligned, funnel-shifted as FMT 2) are at most 36 B (qs 20, sign / scale words 12, d 4) and 44 B (qs 20, qh 4,
+// signs 12, scales 4, d 4).  Own plan (kGSmem3): the IQ plan with Q4_K's 80-byte raw slots and a 4 KB codebook region.
 #include <cuda_fp16.h>
 
 #include "act_quant.cuh"
@@ -54,6 +61,7 @@
 #include "wgmma.cuh"
 #define KTB_IQ_TABLE static __device__ const
 #include "iq_tables.h"
+#include "iq3_tables.h"
 
 namespace ktb {
 
@@ -90,6 +98,12 @@ static_assert(kGSmemI <= 227 * 1024 && kOffBI % 1024 == 0 && kGBI % 1024 == 0, "
 constexpr int kOffBM = kGStages * kGA, kOffRawM = kOffBM + kGStages * kGB, kOffTabM = kOffRawM + kGRaw * kRawSlotI, kOffMiscM = kOffTabM + kTabI;
 constexpr int kGSmemM = kOffMiscM + (int)sizeof(GrpMisc) + 1024;
 static_assert(kGSmemM <= 227 * 1024 && kOffBM % 1024 == 0 && kGB % 1024 == 0, "IQ1_M shared-memory plan");
+// IQ3_XXS / IQ3_S plan: the IQ plan with the 80-byte raw slots of the Q4_K plan and the IQ3 codebooks (IQ3_XXS 256 x 4 B grid +
+// 128 x 8 B sign masks; IQ3_S 512 x 4 B grid + 256 x 8 B sign masks)
+constexpr int kTab3 = 512 * 4 + 256 * 8;
+constexpr int kOffB3 = kGStages * kGA, kOffRaw3 = kOffB3 + kGStages * kGBI, kOffTab3 = kOffRaw3 + kGRaw * kRawSlot, kOffMisc3 = kOffTab3 + kTab3;
+constexpr int kGSmem3 = kOffMisc3 + (int)sizeof(GrpMisc) + 1024;
+static_assert(kGSmem3 <= 227 * 1024 && kOffB3 % 1024 == 0 && kGBI % 1024 == 0 && kOffRaw3 % 16 == 0, "IQ3 shared-memory plan");
 
 struct GrpGemmParams {
     const uint8_t* w;          // expert weights
@@ -154,6 +168,10 @@ __global__ void grp_tiles_kernel(const int* nt_prefix, const int* offsets, int E
 //   Q2_K: 0 scales[16], 1 qs[32 hh + l], 2 d | dmin (bytes 32-35), 3 activation piece, 4 as Q4_K
 //   IQ1_M (the IQ slots, sub-blocks q = 2 hh + part times 2 + {0, 1}): bytes 0-7 qs[8 q .. + 8], 8-11 qh[4 q .. + 4], 16-23 the
 //         scale words (d and word q's ls), 24 token scale (threads 64-95), 2 activation piece
+//   IQ3 (five units, sub-blocks 2 q, 2 q + 1, q = 2 hh + part; "covering" = the aligned words over the field, a last one only when
+//         the block starts on a word): bytes 0-19 those covering qs[16 q .. + 16]; IQ3_XXS 20-31 those covering its two sign /
+//         scale words, 32 the word holding d; IQ3_S 20 the word holding qh[2 q .. + 2], 24-35 those covering signs[8 q .. + 8],
+//         36 the word holding scales[q], 40 the word holding d; 44 token scale (threads 64-95), 3 activation piece
 template <int FMT>
 __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGemmParams p) {
     constexpr bool IQ = FMT == 2 || FMT == 3;
@@ -162,23 +180,33 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
     constexpr bool SUB16 = FMT == 1 || FMT == 6 || FMT == 7 || FMT == 8;  // 16-value sub-blocks on the 64-row B (Q6_K, Q3_K, Q2_K, IQ1_M)
     constexpr bool IQM = FMT == 8;                            // IQ1_M: the IQ raw slots and codebook, the Q6_K MMAs
     constexpr bool IQS = IQ || IQM;                           // the IQ raw-slot layout
+    constexpr bool IQ3 = FMT == 9 || FMT == 10;               // IQ3_XXS, IQ3_S: FMT 3's consumers, own raw slots and codebooks
     constexpr int nRaw = FMT == 5 ? kGRaw5 : kGRaw;
-    constexpr int offB = IQ ? kOffBI : IQM ? kOffBM : kOffB, strideB = IQ ? kGBI : kGB, offRaw = IQ ? kOffRawI : IQM ? kOffRawM : kOffRaw,
+    constexpr int offB = IQ ? kOffBI : IQM ? kOffBM : IQ3 ? kOffB3 : kOffB, strideB = (IQ || IQ3) ? kGBI : kGB,
+                  offRaw = IQ ? kOffRawI : IQM ? kOffRawM : IQ3 ? kOffRaw3 : kOffRaw,
                   rawPitch = IQS ? kRawPitchI : FMT == 5 ? kRawPitch5 : kRawPitch, rawSlot = IQS ? kRawSlotI : FMT == 5 ? kRawSlot5 : kRawSlot,
-                  BS = FMT == 2 ? SZ_IQ1_S : FMT == 3 ? SZ_IQ2_XXS : FMT == 6 ? SZ_Q3_K : FMT == 8 ? SZ_IQ1_M : SZ_Q2_K;
+                  BS = FMT == 2 ? SZ_IQ1_S : FMT == 3 ? SZ_IQ2_XXS : FMT == 6 ? SZ_Q3_K : FMT == 8 ? SZ_IQ1_M : FMT == 9 ? SZ_IQ3_XXS
+                     : FMT == 10 ? SZ_IQ3_S : SZ_Q2_K;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base - raw);
-    GrpMisc& misc = *reinterpret_cast<GrpMisc*>(smem + (IQ ? kOffMiscI : IQM ? kOffMiscM : kOffMiscG));
+    GrpMisc& misc = *reinterpret_cast<GrpMisc*>(smem + (IQ ? kOffMiscI : IQM ? kOffMiscM : IQ3 ? kOffMisc3 : kOffMiscG));
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nblk = p.Kc / QK_K, nst = 2 * nblk, MT = p.R / kGM;
-    uint2* tab = reinterpret_cast<uint2*>(smem + (IQM ? kOffTabM : kOffTabI));   // IQ codebooks (read after the __syncthreads below)
+    uint2* tab = reinterpret_cast<uint2*>(smem + (IQM ? kOffTabM : IQ3 ? kOffTab3 : kOffTabI));   // IQ codebooks (read after the __syncthreads below)
+    uint32_t* tab4 = reinterpret_cast<uint32_t*>(tab);   // IQ3 grids (4 bytes per entry); their sign masks follow them
     if (FMT == 2 || IQM) {
         for (int i = tid; i < 2048; i += kGThreads) tab[i] = *reinterpret_cast<const uint2*>(ktb_iq1s_grid[i]);
     } else if (FMT == 3) {
         for (int i = tid; i < 256; i += kGThreads) tab[i] = *reinterpret_cast<const uint2*>(ktb_iq2xxs_grid[i]);
         if (tid < 128) tab[256 + tid] = iq2_sign_masks(ktb_ksigns_iq2xs[tid]);
+    } else if (FMT == 9) {
+        for (int i = tid; i < 256; i += kGThreads) tab4[i] = *reinterpret_cast<const uint32_t*>(ktb_iq3xxs_grid[i]);
+        if (tid < 128) tab[128 + tid] = iq2_sign_masks(ktb_ksigns_iq2xs[tid]);
+    } else if (FMT == 10) {
+        for (int i = tid; i < 512; i += kGThreads) tab4[i] = *reinterpret_cast<const uint32_t*>(ktb_iq3s_grid[i]);
+        if (tid < 256) tab[256 + tid] = iq2_sign_masks(tid);
     }
     if (tid == 0) {
         for (int s = 0; s < kGStages; s++) { bar_init(smem_u32(&misc.ab_full[s]), kGProdWarps); bar_init(smem_u32(&misc.smem_free[s]), kGMmaWarps); }
@@ -263,6 +291,26 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                     cp_async8(dst, fw + 8 * q);
                     cp_async4(dst + 8, fw + 32 + 4 * q);
                     cp_async8(dst + 16, fw + 48);
+                } else if (IQ3) {
+                    // as FMT 2: every word fetched holds at least one byte this thread needs; the last word of a multi-word field
+                    // only when the block starts on a word (its fields then start mid-word)
+                    const int q = 2 * hh + part;
+                    const bool mid = (reinterpret_cast<uintptr_t>(fw) & 2) == 0;
+                    auto cover = [&](int off) { return reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(fw + off) & ~(uintptr_t)3); };
+                    const uint8_t* qs = cover(2 + 16 * q);
+#pragma unroll
+                    for (int i = 0; i < 4; i++) cp_async4(dst + 4 * i, qs + 4 * i);
+                    if (mid) cp_async4(dst + 16, qs + 16);
+                    const uint8_t* sg = cover(FMT == 9 ? 66 + 8 * q : 74 + 8 * q);
+                    const int o = FMT == 9 ? 20 : 24;
+                    cp_async4(dst + o, sg);
+                    cp_async4(dst + o + 4, sg + 4);
+                    if (mid) cp_async4(dst + o + 8, sg + 8);
+                    if (FMT == 10) {
+                        cp_async4(dst + 20, cover(66 + 2 * q));
+                        cp_async4(dst + 36, cover(106 + q));
+                    }
+                    cp_async4(dst + (FMT == 9 ? 32 : 40), cover(0));
                 } else if (IQ) {
                     // every word fetched holds at least one byte this thread needs (so it lies inside the tensor's pages);
                     // the last word of a field is only needed when the block starts on a word (the fields then start mid-word)
@@ -292,10 +340,10 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                         cp_async4(dst + 72, fitem + (long)13 * c16 + (ffi >> 1) * 4);
                     }
                 }
-                if (fxq) { cp_async16(dst + (IQS ? 32 : FMT == 6 ? 64 : 48), fxq); fxq += 128; }
+                if (fxq) { cp_async16(dst + (IQS ? 32 : FMT == 6 ? 64 : 48), fxq); fxq += 128; }   // IQ3: 48
                 if (hh == 1) {
                     if (MINS && fbs) { cp_async16(dst + 64, fbs); fbs += 16; }
-                    if (fdx) { cp_async4(dst + (MINS ? 64 : IQS ? 24 : FMT == 6 ? 56 : 76), fdx); fdx += 1; }
+                    if (fdx) { cp_async4(dst + (MINS ? 64 : IQS ? 24 : FMT == 6 ? 56 : IQ3 ? 44 : 76), fdx); fdx += 1; }
                     fw += FMT == 0 ? SZ_Q4_K : FMT == 5 ? SZ_Q5_K : (IQ || FMT >= 6) ? BS : 16;
                     ffi++;
                 }
@@ -311,8 +359,8 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
             const int n_valid = ti.w;
             int dsel = ((ti.y + r) & 3) * nblk;   // Q6_K: which half of the fetched word holds this block's d
             // IQ: 16 when the current block starts on a word (its fields then start mid-word), else 0; Q3_K (fields at word
-            // offsets of the block): 16 when it starts mid-word.  50, 66 and 110 are 2 mod 4, so it alternates block by block
-            uint32_t ish = IQ ? ((reinterpret_cast<uintptr_t>(p.w + (long)ti.x * p.expert_bytes + (long)(ti.y + r) * nblk * BS) & 2) ? 0u : 16u)
+            // offsets of the block): 16 when it starts mid-word.  50, 66, 98 and 110 are 2 mod 4, so it alternates block by block
+            uint32_t ish = (IQ || IQ3) ? ((reinterpret_cast<uintptr_t>(p.w + (long)ti.x * p.expert_bytes + (long)(ti.y + r) * nblk * BS) & 2) ? 0u : 16u)
                          : FMT == 6 ? ((reinterpret_cast<uintptr_t>(p.w + (long)ti.x * p.expert_bytes + (long)(ti.y + r) * nblk * BS) & 2) ? 16u : 0u) : 0u;
             for (int st = 0; st < nst; st++) {
                 const int hh = st & 1;
@@ -321,7 +369,7 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                 cp_async_wait<nRaw - 1>();
                 if (tr) p.trace[(0 * 96 + st) * 4 + 1] = clock64();
                 const uint4* rs = reinterpret_cast<const uint4*>(raw_src + slot * rawSlot);
-                const uint4 f0 = rs[0], f1 = rs[1], f2 = rs[2], f3 = rs[IQS ? 2 : FMT == 6 ? 4 : 3], f4 = rs[IQS ? 1 : FMT == 6 ? 3 : 4];
+                const uint4 f0 = rs[0], f1 = rs[1], f2 = rs[2], f3 = rs[IQS ? 2 : FMT == 6 ? 4 : 3], f4 = rs[IQS ? 1 : FMT == 6 ? 3 : IQ3 ? 2 : 4];
                 const uint4 f5 = rs[FMT == 5 ? 5 : 0], f6 = rs[FMT == 5 ? 6 : 0];   // Q5_K: qh
                 issue(raw_dst + slot * rawSlot);   // refill the slot just read (thread-private bytes: no barrier involved)
                 slot = slot == nRaw - 1 ? 0 : slot + 1;
@@ -394,6 +442,43 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                     uint32_t* hrow = reinterpret_cast<uint32_t*>(&misc.hdr[hs][r]);
                     hrow[part] = ls;
                     if (part == 0) hrow[2] = __float_as_uint(iq_d8(iq1m_d_bits(f1.x, f1.y)));
+                } else if (IQ3) {
+                    // sub-block 4 hh + 2 part + j -> A chunks 4 part + 2 j, + 1 as FMT 3 (value word g of 8 = 4-value group g, +-grid
+                    // through the sign masks); header word `part` = the two ls (16 bits each), word 2 = d / 4 (IQ3_XXS) or d as f32
+                    const int q = 2 * hh + part;
+                    const uint32_t w[5] = {f0.x, f0.y, f0.z, f0.w, f1.x};
+                    const uint32_t sgw[3] = {FMT == 9 ? f1.y : f1.z, FMT == 9 ? f1.z : f1.w, FMT == 9 ? f1.w : f2.x};
+                    const uint32_t dw = FMT == 9 ? f2.x : f2.z, dbits = ish ? (dw & 0xffffu) : (dw >> 16);
+                    // IQ3_S: qh[2 q], qh[2 q + 1] and scales[q] from the words holding them (2-byte / byte positions from ish)
+                    const uint32_t qh16 = f1.y >> ((q & 1) ? (ish ^ 16u) : ish), scb = f2.y >> (8 * ((q + (ish ? 2 : 0)) & 3));
+                    const uint2* sgn = tab + (FMT == 9 ? 128 : 256);
+                    uint32_t ls[2];
+#pragma unroll
+                    for (int j = 0; j < 2; j++) {
+                        const uint32_t sg = __funnelshift_r(sgw[j], sgw[j + 1], ish);   // IQ3_XXS: 4 x 7-bit sign index | s; IQ3_S: 4 sign bytes
+                        uint32_t v[8];
+#pragma unroll
+                        for (int l = 0; l < 4; l++) {   // 8 values: 4-value groups 2 l, 2 l + 1 = bytes 2 (l & 1), + 1 of qs word 2 j + l / 2
+                            const uint32_t qw = __funnelshift_r(w[2 * j + (l >> 1)], w[2 * j + (l >> 1) + 1], ish) >> (16 * (l & 1));
+                            uint32_t i0 = qw & 0xffu, i1 = (qw >> 8) & 0xffu;
+                            if (FMT == 10) {
+                                const uint32_t qh = qh16 >> (8 * j);
+                                i0 |= ((qh >> (2 * l)) & 1u) << 8;
+                                i1 |= ((qh >> (2 * l + 1)) & 1u) << 8;
+                            }
+                            const uint2 m = sgn[FMT == 9 ? (sg >> (7 * l)) & 127u : (sg >> (8 * l)) & 0xffu];
+                            v[2 * l] = __vsub4(tab4[i0] ^ m.x, m.x);
+                            v[2 * l + 1] = __vsub4(tab4[i1] ^ m.y, m.y);
+                        }
+                        ls[j] = FMT == 9 ? 2 * (sg >> 28) + 1 : 2 * ((scb >> (4 * j)) & 15u) + 1;
+                        const int c0 = 4 * part + 2 * j;
+                        *reinterpret_cast<uint4*>(arow + (((c0 + 0) ^ sw) << 4)) = make_uint4(v[0], v[1], v[2], v[3]);
+                        *reinterpret_cast<uint4*>(arow + (((c0 + 1) ^ sw) << 4)) = make_uint4(v[4], v[5], v[6], v[7]);
+                    }
+                    uint32_t* hrow = reinterpret_cast<uint32_t*>(&misc.hdr[hs][r]);
+                    hrow[part] = ls[0] | (ls[1] << 16);
+                    if (part == 0) hrow[2] = __float_as_uint(FMT == 9 ? iq_d4((uint16_t)dbits) : fp16_bits_to_f32((uint16_t)dbits));
+                    if (hh == 1) ish ^= 16u;
                 } else if (IQ) {
                     // sub-block 4 hh + 2 part + j -> A chunks 4 part + 2 j and 4 part + 2 j + 1; header word `part` = its two ls
                     // (16 bits each), word 2 = d / 8 as f32
@@ -515,7 +600,7 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                     *reinterpret_cast<uint4*>(Bs + (kGN + bn) * 128 + ((pc ^ (bn & 7)) << 4)) = (pc & 1) ? bv : z;
                 }
                 if (hh == 1 && pt < 96) {   // token scales, and (formats with mins) the sixteen 16-value sums of the super-block as fp16
-                    if (pt >= 64) misc.dxs[hs][pt - 64] = pt - 64 < n_valid ? __uint_as_float(MINS ? f4.x : (IQS || FMT == 6) ? f4.z : f4.w) : 0.f;
+                    if (pt >= 64) misc.dxs[hs][pt - 64] = pt - 64 < n_valid ? __uint_as_float(MINS ? f4.x : (IQS || FMT == 6) ? f4.z : f4.w) : 0.f;   // IQ3: f2.w
                     else if (MINS) {
                         const int n2 = pt >> 1, kg = pt & 1;
                         uint4 vv = z;
@@ -588,7 +673,7 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
 #pragma unroll
                         for (int i = 0; i < 16; i++) isum[i] += sc[(i >> 1) & 1][c] * (int)v0[i] + sc[(i >> 1) & 1][c + 1] * (int)v1[i];
                     }
-                } else if (IQ) {
+                } else if (IQ || IQ3) {
                     // sub-block c of the stage: one MMA into its own accumulator, times its ls (header word c / 2, half c % 2)
 #pragma unroll
                     for (int c = 0; c < 4; c += 2) {
@@ -1031,6 +1116,8 @@ static int grouped_fmt(int type, int layout) {
     if (type == KTB200_TYPE_Q3_K) return 6;
     if (type == KTB200_TYPE_Q2_K) return 7;
     if (type == KTB200_TYPE_IQ1_M) return 8;
+    if (type == KTB200_TYPE_IQ3_XXS) return 9;
+    if (type == KTB200_TYPE_IQ3_S) return 10;
     return -1;
 }
 static void grouped_i4(int np, const GrpI4Params& p, int grid, cudaStream_t s) {
@@ -1046,12 +1133,14 @@ static void grouped_gemm(int fmt, const GrpGemmParams& p, int grid, cudaStream_t
         case 5: grouped_gemm_kernel<5><<<grid, kGThreads, kGSmem, s>>>(p); break;
         case 6: grouped_gemm_kernel<6><<<grid, kGThreads, kGSmem, s>>>(p); break;
         case 7: grouped_gemm_kernel<7><<<grid, kGThreads, kGSmem, s>>>(p); break;
-        default: grouped_gemm_kernel<8><<<grid, kGThreads, kGSmemM, s>>>(p); break;
+        case 8: grouped_gemm_kernel<8><<<grid, kGThreads, kGSmemM, s>>>(p); break;
+        case 9: grouped_gemm_kernel<9><<<grid, kGThreads, kGSmem3, s>>>(p); break;
+        default: grouped_gemm_kernel<10><<<grid, kGThreads, kGSmem3, s>>>(p); break;
     }
 }
 
 // true when ktb200_moe_forward may take the grouped tensor-core path for this handle: gate and up Q4_K, Q5_K, Q3_K, Q2_K, IQ1_S,
-// IQ1_M or IQ2_XXS (each on its own), down any of those or Q6_K in the tile layout; or all three RAWINT4_G32
+// IQ1_M, IQ2_XXS, IQ3_XXS or IQ3_S (each on its own), down any of those or Q6_K in the tile layout; or all three RAWINT4_G32
 bool grouped_ok(const ktb200_moe* m, int k) {
     const ktb200_moe_config& c = m->cfg;
     const int fg = grouped_fmt(c.gate_type, LAYOUT_RAW), fu = grouped_fmt(c.up_type, LAYOUT_RAW), fd = grouped_fmt(c.down_type, m->down_layout);
@@ -1081,6 +1170,8 @@ int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, cons
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmemM));
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<9>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem3));
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<10>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem3));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_i4_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, I4Plan<1>::kSmem));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_i4_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, I4Plan<3>::kSmem));
         attr[dev & 63] = true;

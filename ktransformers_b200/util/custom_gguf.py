@@ -67,9 +67,12 @@ GGML_BLOCK_SIZES = {t.name: GGML_QUANT_SIZES[t][1] for t in GGML_QUANT_SIZES}
 B200_WEIGHT_TYPES = {"Q2_K", "Q3_K", "Q4_K", "Q5_K", "Q6_K", "IQ4_XS"}
 # routed experts also take ggml's codebook i-quants (DeepSeek-R1's 1.5-2-bit GGUF files); linears and MLPs do not
 B200_EXPERT_TYPES = B200_WEIGHT_TYPES | {"IQ1_S", "IQ2_XXS"}
-# what the routed-expert loaders accept: kept apart from B200_EXPERT_TYPES, whose value callers and tests rely on
+# routed experts with IQ1_M: kept apart from B200_EXPERT_TYPES, whose value callers and tests rely on
 B200_ROUTED_EXPERT_TYPES = B200_EXPERT_TYPES | {"IQ1_M"}
-B200_DEQUANT_TYPES = B200_ROUTED_EXPERT_TYPES | {"Q8_0", "F32", "F16", "BF16"}
+# what the routed-expert loaders accept: also ggml's 3-bit i-quants (llama.cpp's IQ3_XXS / IQ3_XS / IQ3_S / IQ3_M DeepSeek
+# files).  A set of its own, so that the sets above keep their values
+B200_EXPERT_LOAD_TYPES = B200_ROUTED_EXPERT_TYPES | {"IQ3_XXS", "IQ3_S"}
+B200_DEQUANT_TYPES = B200_EXPERT_LOAD_TYPES | {"Q8_0", "F32", "F16", "BF16"}
 # the (gate/up, down) type sets the single-launch expert-parallel kernel takes (gate and up of one type): Q4_K gate/up with
 # Q4_K or Q6_K down, and Q2_K or Q3_K gate/up with Q2_K, Q3_K, Q4_K or Q6_K down (llama.cpp's Q2_K, Q3_K_S and Q3_K_M files)
 B200_EP_TYPE_SETS = {("Q4_K", "Q4_K"), ("Q4_K", "Q6_K")} | {(gu, d) for gu in ("Q2_K", "Q3_K") for d in ("Q2_K", "Q3_K", "Q4_K", "Q6_K")}
