@@ -51,11 +51,18 @@ enum ktb200_ggml_type {
      *   IQ3_S   110 B: fp16 d, qs[64], qh[8], signs[32], scales[4]; 4-value group j (0..63) is iq3s_grid[qs[j] | (bit j%8
      *            of qh[j/8]) << 8], bit i of signs[k] negates value 8k+i, sub-block ib has s = nibble ib%2 (low for
      *            even ib) of scales[ib/2]; value = d*(2s+1) * grid * sign
+     *   IQ2_XS   74 B: fp16 d, qs uint16[32], scales[8]; 8-value group l (0..31) is iq2xs_grid[qs[l] & 511] with the signs
+     *            ksigns_iq2xs[qs[l] >> 9]; 16-value half h (0..15) has s = nibble h%2 (low for even h) of scales[h/2];
+     *            value = d*(2s+1)/8 * grid * sign
+     *   IQ2_S    82 B: fp16 d, qs[32], signs[32], qh[8], scales[8]; 8-value group l (0..31) is iq2s_grid[qs[l] | ((qh[l/4]
+     *            >> 2(l%4)) & 3) << 8], bit i of signs[l] negates its value i; s per 16 values as IQ2_XS;
+     *            value = d*(2s+1)/8 * grid * sign
      * vec_dot_type Q8_K.  Routed experts only (ktb200_moe_create, any mix with the K-quants); linears, MLP handles and the
      * one-token expert-parallel entry points reject them.  ktb200_moe_forward runs them per (token, expert) pair below 80
      * tokens and on the grouped tensor-core GEMM from 80 (gate, up and down each in its own format).  The codebooks are
-     * ktransformers_b200/csrc/iq_tables.h. */
-    KTB200_TYPE_IQ2_XXS = 16, KTB200_TYPE_IQ3_XXS = 18, KTB200_TYPE_IQ1_S = 19, KTB200_TYPE_IQ3_S = 21, KTB200_TYPE_IQ1_M = 29,
+     * ktransformers_b200/csrc/iq_tables.h, iq3_tables.h and iq2_tables.h. */
+    KTB200_TYPE_IQ2_XXS = 16, KTB200_TYPE_IQ2_XS = 17, KTB200_TYPE_IQ3_XXS = 18, KTB200_TYPE_IQ1_S = 19, KTB200_TYPE_IQ3_S = 21,
+    KTB200_TYPE_IQ2_S = 22, KTB200_TYPE_IQ1_M = 29,
     /* Not a ggml type: ggml's ids stay below 64, so 256 cannot collide with one.
      * Symmetric INT4 in groups of 32 with bf16 scales (compressed-tensors "pack-quantized", kt-kernel's RAWINT4; Kimi-K2's
      * routed experts), in the device layout ktb200_rawint4_pack writes: 144 B per 256 values of a row,

@@ -21,6 +21,8 @@
 #define SZ_IQ1_M 56      // qs[32] + qh[16] + scales[4] (uint16, fp16 d in the top nibbles)
 #define SZ_IQ3_XXS 98    // fp16 d + qs[64] + 8 x (signs + scale) words
 #define SZ_IQ3_S 110     // fp16 d + qs[64] + qh[8] + signs[32] + scales[4]
+#define SZ_IQ2_XS 74     // fp16 d + qs[32] (uint16: 9-bit grid index | 7-bit sign index) + scales[8]
+#define SZ_IQ2_S 82      // fp16 d + qs[32] + signs[32] + qh[8] + scales[8]
 #define SZ_RAWINT4 144   // 8 bf16 scales + 256 nibbles (rawint4.cuh)
 
 namespace ktb {
@@ -96,17 +98,19 @@ __host__ __device__ inline bool is_kquant(int t) {
 // MLP / grouped / block / expert-parallel path
 __host__ __device__ inline bool is_iquant(int t) {
     return t == KTB200_TYPE_IQ2_XXS || t == KTB200_TYPE_IQ1_S || t == KTB200_TYPE_IQ1_M || t == KTB200_TYPE_IQ3_XXS ||
-           t == KTB200_TYPE_IQ3_S;
+           t == KTB200_TYPE_IQ3_S || t == KTB200_TYPE_IQ2_XS || t == KTB200_TYPE_IQ2_S;
 }
 static inline const char* iquant_name(int t) {
     return t == KTB200_TYPE_IQ1_S ? "IQ1_S" : t == KTB200_TYPE_IQ2_XXS ? "IQ2_XXS" : t == KTB200_TYPE_IQ1_M ? "IQ1_M"
-         : t == KTB200_TYPE_IQ3_XXS ? "IQ3_XXS" : t == KTB200_TYPE_IQ3_S ? "IQ3_S" : "?";
+         : t == KTB200_TYPE_IQ3_XXS ? "IQ3_XXS" : t == KTB200_TYPE_IQ3_S ? "IQ3_S" : t == KTB200_TYPE_IQ2_XS ? "IQ2_XS"
+         : t == KTB200_TYPE_IQ2_S ? "IQ2_S" : "?";
 }
 // block geometry including the i-quants.  Kept apart from type_size / blck_size, which every kernel inlines for its hidden
 // type: a longer switch there would change the code of kernels that never see an i-quant.
 __host__ __device__ inline long weight_block_bytes(int t) {
     return t == KTB200_TYPE_IQ2_XXS ? SZ_IQ2_XXS : t == KTB200_TYPE_IQ1_S ? SZ_IQ1_S : t == KTB200_TYPE_IQ1_M ? SZ_IQ1_M
-         : t == KTB200_TYPE_IQ3_XXS ? SZ_IQ3_XXS : t == KTB200_TYPE_IQ3_S ? SZ_IQ3_S : type_size(t);
+         : t == KTB200_TYPE_IQ3_XXS ? SZ_IQ3_XXS : t == KTB200_TYPE_IQ3_S ? SZ_IQ3_S : t == KTB200_TYPE_IQ2_XS ? SZ_IQ2_XS
+         : t == KTB200_TYPE_IQ2_S ? SZ_IQ2_S : type_size(t);
 }
 __host__ __device__ inline long weight_block_elems(int t) { return is_iquant(t) ? QK_K : blck_size(t); }
 // not a K-quant: it has its own kernels (rawint4.cuh) and no path through the generic K-quant ones
@@ -162,7 +166,7 @@ __device__ __forceinline__ float warp_sum(float v) {
 // ------------------------------------------------------------------ hidden-type conversions
 __device__ __forceinline__ float fp16_bits_to_f32(uint16_t h) { return __half2float(__ushort_as_half(h)); }
 
-// ------------------------------------------------------------------ IQ1_S / IQ1_M / IQ2_XXS / IQ3 arithmetic shared by iq.cuh and grouped.cu
+// ------------------------------------------------------------------ IQ1_S / IQ1_M / IQ2 / IQ3 arithmetic shared by iq.cuh and grouped.cu
 // a super-block's fp32 term (DESIGN.md §2): ((d / 8) * dx) * S with the exact integer S of the super-block; also the term
 // (d * dx) * isum of Q3_K and Q6_K (gemv_bulk.cuh BulkQ3K, grouped.cu)
 __device__ __forceinline__ float iq_d8(uint16_t d_bits) { return fp16_bits_to_f32(d_bits) * 0.125f; }
@@ -178,7 +182,7 @@ __device__ __forceinline__ uint16_t iq1m_d_bits(uint32_t s01, uint32_t s23) {
 __device__ __forceinline__ float kq_min_term(float d, float dmin, float dx, int isum, float msum) {
     return (d * dx) * (float)isum - (dmin * dx) * msum;
 }
-// an IQ2_XXS / IQ3_XXS sign pattern (ksigns_iq2xs byte), or an IQ3_S sign byte, as byte masks: value = (grid ^ m) - m per byte
+// an IQ2_XXS / IQ2_XS / IQ3_XXS sign pattern (ksigns_iq2xs byte), or an IQ2_S / IQ3_S sign byte, as byte masks: value = (grid ^ m) - m per byte
 __device__ __forceinline__ uint2 iq2_sign_masks(uint32_t s) {
     uint32_t lo = 0, hi = 0;
 #pragma unroll

@@ -13,7 +13,7 @@
 //   FmtQ4K    raw GGUF block_q4_K (144 B, already 16-byte aligned)   unit = 16 B of qs = 32 weights, 4 blocks/step
 //   FmtQ5K    raw GGUF block_q5_K (176 B, 16-byte aligned)           unit = 16 B qs + qh   = 32 weights, 4 blocks/step
 //   FmtQ6K8   block_q6_K re-laid as "8-row SoA" (moe.cu repack)      unit = 48 B           = 64 weights, 8 blocks/step
-//   FmtGenK   any raw K-quant / IQ4_XS / IQ2_XXS / IQ1_S / IQ1_M / IQ3_XXS / IQ3_S through byte loads (fallback)
+//   FmtGenK   any raw K-quant / IQ4_XS / IQ2_XXS / IQ1_S / IQ1_M / IQ3_XXS / IQ3_S / IQ2_XS / IQ2_S through byte loads (fallback)
 //                                                                    unit = 16 weights,              2 blocks/step
 #pragma once
 #include "common.cuh"
@@ -24,6 +24,7 @@
 #define KTB_IQ_TABLE static __device__ const
 #include "iq_tables.h"
 #include "iq3_tables.h"
+#include "iq2_tables.h"
 #endif
 
 namespace ktb {
@@ -484,6 +485,37 @@ __device__ inline void unpack_group16(int type, const uint8_t* b, int g, GroupK&
                 for (int i = 0; i < 4; i++) {
                     const int gv = ldg_u8(&ktb_iq3s_grid[idx][i]);
                     v[4 * k + i] = (int8_t)(((signs >> (4 * k + i)) & 1) ? -gv : gv);
+                }
+            }
+            break;
+        }
+        case KTB200_TYPE_IQ2_XS: {
+            // d/8 and ls = 2s+1 per 16 values (nibble g % 2 of scales[g / 2]); 8-value group 2g + l: qs[2g + l] & 511 indexes
+            // iq2xs_grid, qs[2g + l] >> 9 ksigns_iq2xs
+            o.d = fp16_bits_to_f32(ldg_u16(b)) * 0.125f;
+            o.isc = 2 * (int)((ldg_u8(b + 66 + (g >> 1)) >> (4 * (g & 1))) & 15) + 1;
+            for (int l = 0; l < 2; l++) {
+                const uint32_t q = ldg_u16(b + 2 + 2 * (2 * g + l));
+                const uint32_t signs = ldg_u8(&ktb_ksigns_iq2xs[q >> 9]);
+                for (int j = 0; j < 8; j++) {
+                    const int gv = ldg_u8(&ktb_iq2xs_grid[q & 511][j]);
+                    v[8 * l + j] = (int8_t)(((signs >> j) & 1) ? -gv : gv);
+                }
+            }
+            break;
+        }
+        case KTB200_TYPE_IQ2_S: {
+            // d/8 and ls = 2s+1 per 16 values as IQ2_XS; 8-value group 2g + l: iq2s_grid[qs | 2 bits of qh << 8], sign byte
+            o.d = fp16_bits_to_f32(ldg_u16(b)) * 0.125f;
+            o.isc = 2 * (int)((ldg_u8(b + 74 + (g >> 1)) >> (4 * (g & 1))) & 15) + 1;
+            const uint32_t qh = ldg_u8(b + 66 + (g >> 1));
+            for (int l = 0; l < 2; l++) {
+                const int k = 2 * g + l;   // 8-value group of the block; k % 4 = 2 (g & 1) + l
+                const int idx = ldg_u8(b + 2 + k) | (int)(((qh >> (2 * (k & 3))) & 3) << 8);
+                const uint32_t signs = ldg_u8(b + 34 + k);
+                for (int j = 0; j < 8; j++) {
+                    const int gv = ldg_u8(&ktb_iq2s_grid[idx][j]);
+                    v[8 * l + j] = (int8_t)(((signs >> j) & 1) ? -gv : gv);
                 }
             }
             break;

@@ -53,6 +53,13 @@
 // (two sub-blocks) does not fit the 20 payload bytes of FMT 2's raw slots: the covering 4-byte words of the 98 / 110-byte
 // blocks (2-byte aligned, funnel-shifted as FMT 2) are at most 36 B (qs 20, sign / scale words 12, d 4) and 44 B (qs 20, qh 4,
 // signs 12, scales 4, d 4).  Own plan (kGSmem3): the IQ plan with Q4_K's 80-byte raw slots and a 4 KB codebook region.
+// IQ2_XS (FMT 11) and IQ2_S (FMT 12), the experts of llama.cpp's IQ2_XS / IQ2_S / IQ2_M files: IQ2_XXS's +-grid values with an
+// odd scale ls per 16 values, so IQ1_M's consumers (the Q6_K MMAs against the 64-row B, the two halves' ls as the header's
+// signed bytes, the d / 8 finish).  The producers expand +-grid (IQ2_XS 512 x 8 with 9-bit indices, signs through IQ2_XXS's
+// masks; IQ2_S 1024 x 8 with 10-bit indices, its sign bytes through IQ3_S's mask table) into the s8 A tile.  The covering
+// words of a thread's two sub-blocks in the 74 / 82-byte blocks (2-byte aligned, funnel-shifted as FMT 2) are at most 28 B (qs
+// 20, scales 4, d 4) and 36 B (qs 12, signs 12, qh 4, scales 4, d 4): IQ3's 80-byte raw slots.  Own plan (kGSmemI2): the IQ1_M
+// plan with those slots and a 10 KB codebook region.
 #include <cuda_fp16.h>
 
 #include "act_quant.cuh"
@@ -62,6 +69,7 @@
 #define KTB_IQ_TABLE static __device__ const
 #include "iq_tables.h"
 #include "iq3_tables.h"
+#include "iq2_tables.h"
 
 namespace ktb {
 
@@ -104,6 +112,12 @@ constexpr int kTab3 = 512 * 4 + 256 * 8;
 constexpr int kOffB3 = kGStages * kGA, kOffRaw3 = kOffB3 + kGStages * kGBI, kOffTab3 = kOffRaw3 + kGRaw * kRawSlot, kOffMisc3 = kOffTab3 + kTab3;
 constexpr int kGSmem3 = kOffMisc3 + (int)sizeof(GrpMisc) + 1024;
 static_assert(kGSmem3 <= 227 * 1024 && kOffB3 % 1024 == 0 && kGBI % 1024 == 0 && kOffRaw3 % 16 == 0, "IQ3 shared-memory plan");
+// IQ2_XS / IQ2_S plan: the IQ1_M plan (64-row B) with the 80-byte raw slots and the IQ2 codebooks (IQ2_XS 512 x 8 B grid +
+// 128 x 8 B sign masks; IQ2_S 1024 x 8 B grid + 256 x 8 B sign masks)
+constexpr int kTabI2 = 1024 * 8 + 256 * 8;
+constexpr int kOffBI2 = kGStages * kGA, kOffRawI2 = kOffBI2 + kGStages * kGB, kOffTabI2 = kOffRawI2 + kGRaw * kRawSlot, kOffMiscI2 = kOffTabI2 + kTabI2;
+constexpr int kGSmemI2 = kOffMiscI2 + (int)sizeof(GrpMisc) + 1024;
+static_assert(kGSmemI2 <= 227 * 1024 && kOffBI2 % 1024 == 0 && kGB % 1024 == 0 && kOffRawI2 % 16 == 0, "IQ2_XS / IQ2_S shared-memory plan");
 
 struct GrpGemmParams {
     const uint8_t* w;          // expert weights
@@ -172,29 +186,35 @@ __global__ void grp_tiles_kernel(const int* nt_prefix, const int* offsets, int E
 //         the block starts on a word): bytes 0-19 those covering qs[16 q .. + 16]; IQ3_XXS 20-31 those covering its two sign /
 //         scale words, 32 the word holding d; IQ3_S 20 the word holding qh[2 q .. + 2], 24-35 those covering signs[8 q .. + 8],
 //         36 the word holding scales[q], 40 the word holding d; 44 token scale (threads 64-95), 3 activation piece
+//   IQ2 (IQ3's five units and sub-blocks): IQ2_XS bytes 0-19 those covering qs[16 q .. + 16] (eight uint16), 20 the word holding
+//         scales[2 q .. + 2], 24 the word holding d; IQ2_S 0-11 those covering qs[8 q .. + 8], 12-23 those covering
+//         signs[8 q .. + 8], 24 the word holding qh[2 q .. + 2], 28 the word holding scales[2 q .. + 2], 32 the word holding d;
+//         44 token scale (threads 64-95), 3 activation piece
 template <int FMT>
 __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGemmParams p) {
     constexpr bool IQ = FMT == 2 || FMT == 3;
     constexpr bool K4 = FMT == 0 || FMT == 5;                 // 32-value sub-blocks with mins, u8 operands (Q4_K, Q5_K)
     constexpr bool MINS = K4 || FMT == 7;                     // the mins MMA and Q4_K's finish (Q4_K, Q5_K, Q2_K)
-    constexpr bool SUB16 = FMT == 1 || FMT == 6 || FMT == 7 || FMT == 8;  // 16-value sub-blocks on the 64-row B (Q6_K, Q3_K, Q2_K, IQ1_M)
+    // 16-value sub-blocks on the 64-row B (Q6_K, Q3_K, Q2_K, IQ1_M, IQ2_XS, IQ2_S)
+    constexpr bool SUB16 = FMT == 1 || FMT == 6 || FMT == 7 || FMT == 8 || FMT == 11 || FMT == 12;
     constexpr bool IQM = FMT == 8;                            // IQ1_M: the IQ raw slots and codebook, the Q6_K MMAs
     constexpr bool IQS = IQ || IQM;                           // the IQ raw-slot layout
     constexpr bool IQ3 = FMT == 9 || FMT == 10;               // IQ3_XXS, IQ3_S: FMT 3's consumers, own raw slots and codebooks
+    constexpr bool IQ2 = FMT == 11 || FMT == 12;              // IQ2_XS, IQ2_S: IQ1_M's consumers, IQ3's raw slots, own codebooks
     constexpr int nRaw = FMT == 5 ? kGRaw5 : kGRaw;
-    constexpr int offB = IQ ? kOffBI : IQM ? kOffBM : IQ3 ? kOffB3 : kOffB, strideB = (IQ || IQ3) ? kGBI : kGB,
-                  offRaw = IQ ? kOffRawI : IQM ? kOffRawM : IQ3 ? kOffRaw3 : kOffRaw,
+    constexpr int offB = IQ ? kOffBI : IQM ? kOffBM : IQ3 ? kOffB3 : IQ2 ? kOffBI2 : kOffB, strideB = (IQ || IQ3) ? kGBI : kGB,
+                  offRaw = IQ ? kOffRawI : IQM ? kOffRawM : IQ3 ? kOffRaw3 : IQ2 ? kOffRawI2 : kOffRaw,
                   rawPitch = IQS ? kRawPitchI : FMT == 5 ? kRawPitch5 : kRawPitch, rawSlot = IQS ? kRawSlotI : FMT == 5 ? kRawSlot5 : kRawSlot,
                   BS = FMT == 2 ? SZ_IQ1_S : FMT == 3 ? SZ_IQ2_XXS : FMT == 6 ? SZ_Q3_K : FMT == 8 ? SZ_IQ1_M : FMT == 9 ? SZ_IQ3_XXS
-                     : FMT == 10 ? SZ_IQ3_S : SZ_Q2_K;
+                     : FMT == 10 ? SZ_IQ3_S : FMT == 11 ? SZ_IQ2_XS : FMT == 12 ? SZ_IQ2_S : SZ_Q2_K;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base - raw);
-    GrpMisc& misc = *reinterpret_cast<GrpMisc*>(smem + (IQ ? kOffMiscI : IQM ? kOffMiscM : IQ3 ? kOffMisc3 : kOffMiscG));
+    GrpMisc& misc = *reinterpret_cast<GrpMisc*>(smem + (IQ ? kOffMiscI : IQM ? kOffMiscM : IQ3 ? kOffMisc3 : IQ2 ? kOffMiscI2 : kOffMiscG));
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nblk = p.Kc / QK_K, nst = 2 * nblk, MT = p.R / kGM;
-    uint2* tab = reinterpret_cast<uint2*>(smem + (IQM ? kOffTabM : IQ3 ? kOffTab3 : kOffTabI));   // IQ codebooks (read after the __syncthreads below)
+    uint2* tab = reinterpret_cast<uint2*>(smem + (IQM ? kOffTabM : IQ3 ? kOffTab3 : IQ2 ? kOffTabI2 : kOffTabI));   // IQ codebooks (read after the __syncthreads below)
     uint32_t* tab4 = reinterpret_cast<uint32_t*>(tab);   // IQ3 grids (4 bytes per entry); their sign masks follow them
     if (FMT == 2 || IQM) {
         for (int i = tid; i < 2048; i += kGThreads) tab[i] = *reinterpret_cast<const uint2*>(ktb_iq1s_grid[i]);
@@ -207,6 +227,12 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
     } else if (FMT == 10) {
         for (int i = tid; i < 512; i += kGThreads) tab4[i] = *reinterpret_cast<const uint32_t*>(ktb_iq3s_grid[i]);
         if (tid < 256) tab[256 + tid] = iq2_sign_masks(tid);
+    } else if (FMT == 11) {
+        for (int i = tid; i < 512; i += kGThreads) tab[i] = *reinterpret_cast<const uint2*>(ktb_iq2xs_grid[i]);
+        if (tid < 128) tab[512 + tid] = iq2_sign_masks(ktb_ksigns_iq2xs[tid]);
+    } else if (FMT == 12) {
+        for (int i = tid; i < 1024; i += kGThreads) tab[i] = *reinterpret_cast<const uint2*>(ktb_iq2s_grid[i]);
+        if (tid < 256) tab[1024 + tid] = iq2_sign_masks(tid);
     }
     if (tid == 0) {
         for (int s = 0; s < kGStages; s++) { bar_init(smem_u32(&misc.ab_full[s]), kGProdWarps); bar_init(smem_u32(&misc.smem_free[s]), kGMmaWarps); }
@@ -311,6 +337,31 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                         cp_async4(dst + 36, cover(106 + q));
                     }
                     cp_async4(dst + (FMT == 9 ? 32 : 40), cover(0));
+                } else if (IQ2) {
+                    // as IQ3: the covering words of each multi-word field (a last one only when the block starts on a word), the
+                    // words holding the 2-byte fields
+                    const int q = 2 * hh + part;
+                    const bool mid = (reinterpret_cast<uintptr_t>(fw) & 2) == 0;
+                    auto cover = [&](int off) { return reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(fw + off) & ~(uintptr_t)3); };
+                    if (FMT == 11) {
+                        const uint8_t* qs = cover(2 + 16 * q);
+#pragma unroll
+                        for (int i = 0; i < 4; i++) cp_async4(dst + 4 * i, qs + 4 * i);
+                        if (mid) cp_async4(dst + 16, qs + 16);
+                        cp_async4(dst + 20, cover(66 + 2 * q));
+                        cp_async4(dst + 24, cover(0));
+                    } else {
+                        const uint8_t *qs = cover(2 + 8 * q), *sg = cover(34 + 8 * q);
+                        cp_async4(dst, qs);
+                        cp_async4(dst + 4, qs + 4);
+                        if (mid) cp_async4(dst + 8, qs + 8);
+                        cp_async4(dst + 12, sg);
+                        cp_async4(dst + 16, sg + 4);
+                        if (mid) cp_async4(dst + 20, sg + 8);
+                        cp_async4(dst + 24, cover(66 + 2 * q));
+                        cp_async4(dst + 28, cover(74 + 2 * q));
+                        cp_async4(dst + 32, cover(0));
+                    }
                 } else if (IQ) {
                     // every word fetched holds at least one byte this thread needs (so it lies inside the tensor's pages);
                     // the last word of a field is only needed when the block starts on a word (the fields then start mid-word)
@@ -340,10 +391,10 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                         cp_async4(dst + 72, fitem + (long)13 * c16 + (ffi >> 1) * 4);
                     }
                 }
-                if (fxq) { cp_async16(dst + (IQS ? 32 : FMT == 6 ? 64 : 48), fxq); fxq += 128; }   // IQ3: 48
+                if (fxq) { cp_async16(dst + (IQS ? 32 : FMT == 6 ? 64 : 48), fxq); fxq += 128; }   // IQ3, IQ2: 48
                 if (hh == 1) {
                     if (MINS && fbs) { cp_async16(dst + 64, fbs); fbs += 16; }
-                    if (fdx) { cp_async4(dst + (MINS ? 64 : IQS ? 24 : FMT == 6 ? 56 : IQ3 ? 44 : 76), fdx); fdx += 1; }
+                    if (fdx) { cp_async4(dst + (MINS ? 64 : IQS ? 24 : FMT == 6 ? 56 : (IQ3 || IQ2) ? 44 : 76), fdx); fdx += 1; }
                     fw += FMT == 0 ? SZ_Q4_K : FMT == 5 ? SZ_Q5_K : (IQ || FMT >= 6) ? BS : 16;
                     ffi++;
                 }
@@ -359,8 +410,9 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
             const int n_valid = ti.w;
             int dsel = ((ti.y + r) & 3) * nblk;   // Q6_K: which half of the fetched word holds this block's d
             // IQ: 16 when the current block starts on a word (its fields then start mid-word), else 0; Q3_K (fields at word
-            // offsets of the block): 16 when it starts mid-word.  50, 66, 98 and 110 are 2 mod 4, so it alternates block by block
-            uint32_t ish = (IQ || IQ3) ? ((reinterpret_cast<uintptr_t>(p.w + (long)ti.x * p.expert_bytes + (long)(ti.y + r) * nblk * BS) & 2) ? 0u : 16u)
+            // offsets of the block): 16 when it starts mid-word.  50, 66, 74, 82, 98 and 110 are 2 mod 4, so it alternates block
+            // by block
+            uint32_t ish = (IQ || IQ3 || IQ2) ? ((reinterpret_cast<uintptr_t>(p.w + (long)ti.x * p.expert_bytes + (long)(ti.y + r) * nblk * BS) & 2) ? 0u : 16u)
                          : FMT == 6 ? ((reinterpret_cast<uintptr_t>(p.w + (long)ti.x * p.expert_bytes + (long)(ti.y + r) * nblk * BS) & 2) ? 16u : 0u) : 0u;
             for (int st = 0; st < nst; st++) {
                 const int hh = st & 1;
@@ -369,7 +421,7 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                 cp_async_wait<nRaw - 1>();
                 if (tr) p.trace[(0 * 96 + st) * 4 + 1] = clock64();
                 const uint4* rs = reinterpret_cast<const uint4*>(raw_src + slot * rawSlot);
-                const uint4 f0 = rs[0], f1 = rs[1], f2 = rs[2], f3 = rs[IQS ? 2 : FMT == 6 ? 4 : 3], f4 = rs[IQS ? 1 : FMT == 6 ? 3 : IQ3 ? 2 : 4];
+                const uint4 f0 = rs[0], f1 = rs[1], f2 = rs[2], f3 = rs[IQS ? 2 : FMT == 6 ? 4 : 3], f4 = rs[IQS ? 1 : FMT == 6 ? 3 : (IQ3 || IQ2) ? 2 : 4];
                 const uint4 f5 = rs[FMT == 5 ? 5 : 0], f6 = rs[FMT == 5 ? 6 : 0];   // Q5_K: qh
                 issue(raw_dst + slot * rawSlot);   // refill the slot just read (thread-private bytes: no barrier involved)
                 slot = slot == nRaw - 1 ? 0 : slot + 1;
@@ -478,6 +530,49 @@ __global__ void __launch_bounds__(kGThreads, 1) grouped_gemm_kernel(const GrpGem
                     uint32_t* hrow = reinterpret_cast<uint32_t*>(&misc.hdr[hs][r]);
                     hrow[part] = ls[0] | (ls[1] << 16);
                     if (part == 0) hrow[2] = __float_as_uint(FMT == 9 ? iq_d4((uint16_t)dbits) : fp16_bits_to_f32((uint16_t)dbits));
+                    if (hh == 1) ish ^= 16u;
+                } else if (IQ2) {
+                    // sub-block 4 hh + 2 part + j -> A chunks 4 part + 2 j (values 0-15), + 1 (16-31), value word 2 l + {0, 1} = 8-value
+                    // group l as +-grid through the sign masks; header as IQ1_M: the stage's eight ls as bytes 0-7 (byte 4 part + 2 j +
+                    // half), word 2 = d / 8 as f32.  The 2-byte fields of sub-blocks 2 q, 2 q + 1 sit at 16-bit position ish for even q
+                    const uint32_t fsh = part ? (ish ^ 16u) : ish;   // q = 2 hh + part
+                    const uint32_t sc16 = (FMT == 11 ? f1.y : f1.w) >> fsh, qh16 = f1.z >> fsh;
+                    const uint32_t dw = FMT == 11 ? f1.z : f2.x, dbits = ish ? (dw & 0xffffu) : (dw >> 16);
+                    const uint2* sgn = tab + (FMT == 11 ? 512 : 1024);
+#pragma unroll
+                    for (int j = 0; j < 2; j++) {
+                        uint32_t v[8];
+                        if (FMT == 11) {   // uint16 l: 9-bit grid index | 7-bit sign index << 9
+                            const uint32_t w[5] = {f0.x, f0.y, f0.z, f0.w, f1.x};
+                            const uint32_t u[2] = {__funnelshift_r(w[2 * j], w[2 * j + 1], ish), __funnelshift_r(w[2 * j + 1], w[2 * j + 2], ish)};
+#pragma unroll
+                            for (int l = 0; l < 4; l++) {
+                                const uint32_t ul = u[l >> 1] >> (16 * (l & 1));
+                                const uint2 g = tab[ul & 511u], m = sgn[(ul >> 9) & 127u];
+                                v[2 * l] = __vsub4(g.x ^ m.x, m.x);
+                                v[2 * l + 1] = __vsub4(g.y ^ m.y, m.y);
+                            }
+                        } else {           // qs byte l | bits 2 l, 2 l + 1 of qh << 8; sign byte l
+                            const uint32_t qw[3] = {f0.x, f0.y, f0.z}, sgw[3] = {f0.w, f1.x, f1.y};
+                            const uint32_t qs = __funnelshift_r(qw[j], qw[j + 1], ish), sg = __funnelshift_r(sgw[j], sgw[j + 1], ish);
+                            const uint32_t qh = qh16 >> (8 * j);
+#pragma unroll
+                            for (int l = 0; l < 4; l++) {
+                                const uint2 g = tab[((qs >> (8 * l)) & 0xffu) | ((qh << (8 - 2 * l)) & 0x300u)], m = sgn[(sg >> (8 * l)) & 0xffu];
+                                v[2 * l] = __vsub4(g.x ^ m.x, m.x);
+                                v[2 * l + 1] = __vsub4(g.y ^ m.y, m.y);
+                            }
+                        }
+                        const int c0 = 4 * part + 2 * j;
+                        *reinterpret_cast<uint4*>(arow + (((c0 + 0) ^ sw) << 4)) = make_uint4(v[0], v[1], v[2], v[3]);
+                        *reinterpret_cast<uint4*>(arow + (((c0 + 1) ^ sw) << 4)) = make_uint4(v[4], v[5], v[6], v[7]);
+                    }
+                    uint32_t ls = 0;   // nibble i of scales[2 q], scales[2 q + 1]: half i % 2 of sub-block 2 q + i / 2
+#pragma unroll
+                    for (int i = 0; i < 4; i++) ls |= (2 * ((sc16 >> (4 * i)) & 15u) + 1) << (8 * i);
+                    uint32_t* hrow = reinterpret_cast<uint32_t*>(&misc.hdr[hs][r]);
+                    hrow[part] = ls;
+                    if (part == 0) hrow[2] = __float_as_uint(iq_d8((uint16_t)dbits));
                     if (hh == 1) ish ^= 16u;
                 } else if (IQ) {
                     // sub-block 4 hh + 2 part + j -> A chunks 4 part + 2 j and 4 part + 2 j + 1; header word `part` = its two ls
@@ -1118,6 +1213,8 @@ static int grouped_fmt(int type, int layout) {
     if (type == KTB200_TYPE_IQ1_M) return 8;
     if (type == KTB200_TYPE_IQ3_XXS) return 9;
     if (type == KTB200_TYPE_IQ3_S) return 10;
+    if (type == KTB200_TYPE_IQ2_XS) return 11;
+    if (type == KTB200_TYPE_IQ2_S) return 12;
     return -1;
 }
 static void grouped_i4(int np, const GrpI4Params& p, int grid, cudaStream_t s) {
@@ -1135,12 +1232,15 @@ static void grouped_gemm(int fmt, const GrpGemmParams& p, int grid, cudaStream_t
         case 7: grouped_gemm_kernel<7><<<grid, kGThreads, kGSmem, s>>>(p); break;
         case 8: grouped_gemm_kernel<8><<<grid, kGThreads, kGSmemM, s>>>(p); break;
         case 9: grouped_gemm_kernel<9><<<grid, kGThreads, kGSmem3, s>>>(p); break;
-        default: grouped_gemm_kernel<10><<<grid, kGThreads, kGSmem3, s>>>(p); break;
+        case 10: grouped_gemm_kernel<10><<<grid, kGThreads, kGSmem3, s>>>(p); break;
+        case 11: grouped_gemm_kernel<11><<<grid, kGThreads, kGSmemI2, s>>>(p); break;
+        default: grouped_gemm_kernel<12><<<grid, kGThreads, kGSmemI2, s>>>(p); break;
     }
 }
 
 // true when ktb200_moe_forward may take the grouped tensor-core path for this handle: gate and up Q4_K, Q5_K, Q3_K, Q2_K, IQ1_S,
-// IQ1_M, IQ2_XXS, IQ3_XXS or IQ3_S (each on its own), down any of those or Q6_K in the tile layout; or all three RAWINT4_G32
+// IQ1_M, IQ2_XXS, IQ2_XS, IQ2_S, IQ3_XXS or IQ3_S (each on its own), down any of those or Q6_K in the tile layout; or all three
+// RAWINT4_G32
 bool grouped_ok(const ktb200_moe* m, int k) {
     const ktb200_moe_config& c = m->cfg;
     const int fg = grouped_fmt(c.gate_type, LAYOUT_RAW), fu = grouped_fmt(c.up_type, LAYOUT_RAW), fd = grouped_fmt(c.down_type, m->down_layout);
@@ -1172,6 +1272,8 @@ int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, cons
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmemM));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<9>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem3));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<10>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem3));
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<11>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmemI2));
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_gemm_kernel<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmemI2));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_i4_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, I4Plan<1>::kSmem));
         KTB_CUDA_CHECK(cudaFuncSetAttribute(grouped_i4_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, I4Plan<3>::kSmem));
         attr[dev & 63] = true;

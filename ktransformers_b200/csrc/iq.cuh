@@ -1,8 +1,9 @@
-// IQ1_S, IQ1_M, IQ2_XXS, IQ3_XXS and IQ3_S routed experts on the bulk-copy ring (gemv_bulk.cuh): one lane per super-block,
-// codebooks in shared memory.  IQ1_M (56-byte blocks, 8-byte aligned) takes every block count: its unit is 112 * nblk B and its
-// item 224 * nb B, so its launches skip the nblk % 4 (kNblkMultiple) condition of the 50 / 66 / 98 / 110-byte formats.  IQ3_S
-// blocks are Q3_K's size (110 B), so its units and items are Q3_K's; IQ3_XXS's 98-byte blocks give 196 * nblk B units (16-byte
-// sized when nblk % 4 == 0) and 392 * nb B items (when nb is even).
+// IQ1_S, IQ1_M, IQ2_XXS, IQ2_XS, IQ2_S, IQ3_XXS and IQ3_S routed experts on the bulk-copy ring (gemv_bulk.cuh): one lane per
+// super-block, codebooks in shared memory.  IQ1_M (56-byte blocks, 8-byte aligned) takes every block count: its unit is
+// 112 * nblk B and its item 224 * nb B, so its launches skip the nblk % 4 (kNblkMultiple) condition of the 50 / 66 / 74 / 82 /
+// 98 / 110-byte formats.  IQ3_S blocks are Q3_K's size (110 B), so its units and items are Q3_K's; IQ3_XXS's 98-byte blocks
+// give 196 * nblk B units (16-byte sized when nblk % 4 == 0) and 392 * nb B items (when nb is even); IQ2_XS / IQ2_S likewise
+// 148 / 164 * nblk B units and 296 / 328 * nb B items.
 //
 //   * down: item formats BulkIQ1S / BulkIQ2XXS of reduce_bulk_kernel — 4 rows x nb raw ggml blocks, one bulk copy
 //     (4 * nb * 50 B / 4 * nb * 66 B, a multiple of 16 when nb is even; 1600 B / 2112 B at I = 2048 = one block per lane);
@@ -13,13 +14,14 @@
 //     takes Q2_K and Q3_K gate/up (formats BulkQ2K / BulkQ3K, gemv_bulk.cuh): 168 B / 220 B per block pair of a unit.
 //
 // Codebooks: IQ1_S's (and IQ1_M's) 2048 x 8 int8 grid as 16 KB of uint2 (one LDS.64 per 8 values, no unpacking); IQ2_XXS's 256 x 8
-// grid (2 KB) and its 128 sign patterns expanded to byte masks (1 KB: value = (g ^ m) - m per byte); IQ3_XXS's 256 x 4 grid
-// (1 KB) with IQ2_XXS's sign masks; IQ3_S's 512 x 4 grid (2 KB) and its 256 sign bytes as byte masks (2 KB).  All are copied
-// from the device tables of iq_tables.h / iq3_tables.h once per CTA.
+// grid (2 KB) and its 128 sign patterns expanded to byte masks (1 KB: value = (g ^ m) - m per byte); IQ2_XS's 512 x 8 grid
+// (4 KB) with IQ2_XXS's sign masks; IQ2_S's 1024 x 8 grid (8 KB) with IQ3_S's sign-byte masks; IQ3_XXS's 256 x 4 grid (1 KB)
+// with IQ2_XXS's sign masks; IQ3_S's 512 x 4 grid (2 KB) and its 256 sign bytes as byte masks (2 KB).  All are copied from the
+// device tables of iq_tables.h / iq2_tables.h / iq3_tables.h once per CTA.
 //
 // Arithmetic (DESIGN.md §2): IQ1_S  S = sum_ib ls * (8 * sum grid * q8 + delta * bsum32) and term = ((d/8) * dx) * S;
-// IQ2_XXS  term = ((d/8) * dx) * sum_ib ls * sum (+-grid) * q8; IQ3_XXS the same with d/4, IQ3_S with d.  All equal the
-// reference's per-super-block fp32 terms.
+// IQ2_XXS  term = ((d/8) * dx) * sum_ib ls * sum (+-grid) * q8; IQ2_XS / IQ2_S the same with ls per 16 values; IQ3_XXS the
+// same as IQ2_XXS with d/4, IQ3_S with d.  All equal the reference's per-super-block fp32 terms.
 #pragma once
 #include "gemv_bulk.cuh"
 
@@ -31,6 +33,8 @@ __device__ __forceinline__ uint2* iq2xxs_signs_smem() { __shared__ uint2 t[128];
 __device__ __forceinline__ uint32_t* iq3xxs_grid_smem() { __shared__ uint32_t t[256]; return t; }
 __device__ __forceinline__ uint32_t* iq3s_grid_smem() { __shared__ uint32_t t[512]; return t; }
 __device__ __forceinline__ uint2* iq3s_signs_smem() { __shared__ uint2 t[256]; return t; }
+__device__ __forceinline__ uint2* iq2xs_grid_smem() { __shared__ uint2 t[512]; return t; }
+__device__ __forceinline__ uint2* iq2s_grid_smem() { __shared__ uint2 t[1024]; return t; }
 
 // 32 bits from a 2-byte aligned shared-memory address
 __device__ __forceinline__ uint32_t lds_u32_a2(const uint8_t* p) {
@@ -262,8 +266,103 @@ struct BulkIQ3S : BulkFmt {
     }
 };
 
+// IQ2_XXS's values with a 9-bit grid index per 8 values (one uint16: index | 7-bit sign index << 9) into the 512 x 8 grid and
+// one scale per 16 values (two nibbles per sub-block byte, low first).  The two 16-value halves of a sub-block are summed
+// apart and scaled by their own ls, as IQ1_M; term = ((d/8) * dx) * S.
+struct BulkIQ2XS : BulkFmt {
+    static constexpr int kType = KTB200_TYPE_IQ2_XS;
+    static constexpr int kBlockBytes = SZ_IQ2_XS;
+    static constexpr int kBs = 8;            // staged, not read
+    static constexpr int kTableBytes = 512 * 8 + 128 * 8;
+    static constexpr bool kSharedSlot = false;
+    static constexpr int kNblkMultiple = 4;  // a 2-row unit is 148 * nblk B
+    __device__ static __forceinline__ void stage_tables() {
+        uint2* g = iq2xs_grid_smem();
+        uint2* m = iq2xxs_signs_smem();
+        for (int i = threadIdx.x; i < 512; i += blockDim.x) g[i] = *reinterpret_cast<const uint2*>(ktb_iq2xs_grid[i]);
+        for (int i = threadIdx.x; i < 128; i += blockDim.x) m[i] = iq2_sign_masks(ktb_ksigns_iq2xs[i]);
+    }
+    __device__ static __forceinline__ float block_dot(const uint8_t* wb, const uint8_t* aq, const int16_t* /*bs*/, float dxb) {
+        const uint2* grid = iq2xs_grid_smem();
+        const uint2* sgn = iq2xxs_signs_smem();
+        const float d = iq_d8(*reinterpret_cast<const uint16_t*>(wb));
+        const uint32_t sc[2] = {lds_u32_a2(wb + 66), lds_u32_a2(wb + 70)};   // byte ib: the nibbles of sub-block ib's halves
+        int isum = 0;
+#pragma unroll
+        for (int ib = 0; ib < 8; ib++) {
+            const uint32_t q[2] = {lds_u32_a2(wb + 2 + 8 * ib), lds_u32_a2(wb + 6 + 8 * ib)};
+            const uint32_t s = sc[ib >> 2] >> (8 * (ib & 3));
+            const uint4 a0 = *reinterpret_cast<const uint4*>(aq + 32 * ib);
+            const uint4 a1 = *reinterpret_cast<const uint4*>(aq + 32 * ib + 16);
+            const uint32_t ax[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+            int v[2] = {0, 0};
+#pragma unroll
+            for (int l = 0; l < 4; l++) {   // 8-value group l: uint16 l of the sub-block
+                const uint32_t u = q[l >> 1] >> (16 * (l & 1));
+                const uint2 g = grid[u & 511];
+                const uint2 m = sgn[(u >> 9) & 127];
+                v[l >> 1] = dp4a_s8s8(__vsub4(g.x ^ m.x, m.x), ax[2 * l], v[l >> 1]);
+                v[l >> 1] = dp4a_s8s8(__vsub4(g.y ^ m.y, m.y), ax[2 * l + 1], v[l >> 1]);
+            }
+            isum += (2 * (int)(s & 15) + 1) * v[0] + (2 * (int)((s >> 4) & 15) + 1) * v[1];
+        }
+        return iq_term(d, dxb, isum);
+    }
+    __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int /*nrb*/, const uint8_t* aq, const int16_t* bs, float dxb) {
+        return block_dot(sl + f * SZ_IQ2_XS, aq, bs, dxb);
+    }
+};
+
+// 10-bit indices into the 1024 x 8 grid (qs byte | two bits of qh), one sign byte per 8 values (IQ3_S's byte-mask table) and
+// IQ2_XS's scale per 16 values; term = ((d/8) * dx) * S.
+struct BulkIQ2S : BulkFmt {
+    static constexpr int kType = KTB200_TYPE_IQ2_S;
+    static constexpr int kBlockBytes = SZ_IQ2_S;
+    static constexpr int kBs = 8;            // staged, not read
+    static constexpr int kTableBytes = 1024 * 8 + 256 * 8;
+    static constexpr bool kSharedSlot = false;
+    static constexpr int kNblkMultiple = 4;  // a 2-row unit is 164 * nblk B
+    __device__ static __forceinline__ void stage_tables() {
+        uint2* g = iq2s_grid_smem();
+        uint2* m = iq3s_signs_smem();
+        for (int i = threadIdx.x; i < 1024; i += blockDim.x) g[i] = *reinterpret_cast<const uint2*>(ktb_iq2s_grid[i]);
+        for (int i = threadIdx.x; i < 256; i += blockDim.x) m[i] = iq2_sign_masks(i);
+    }
+    __device__ static __forceinline__ float block_dot(const uint8_t* wb, const uint8_t* aq, const int16_t* /*bs*/, float dxb) {
+        const uint2* grid = iq2s_grid_smem();
+        const uint2* sgn = iq3s_signs_smem();
+        const float d = iq_d8(*reinterpret_cast<const uint16_t*>(wb));
+        const uint32_t qhw[2] = {lds_u32_a2(wb + 66), lds_u32_a2(wb + 70)};   // byte ib: 2 high index bits per 8-value group
+        const uint32_t sc[2] = {lds_u32_a2(wb + 74), lds_u32_a2(wb + 78)};
+        int isum = 0;
+#pragma unroll
+        for (int ib = 0; ib < 8; ib++) {
+            const uint32_t qs = lds_u32_a2(wb + 2 + 4 * ib);
+            const uint32_t sg = lds_u32_a2(wb + 34 + 4 * ib);   // byte l: the signs of values 8l..8l+7
+            const uint32_t qh = qhw[ib >> 2] >> (8 * (ib & 3)), s = sc[ib >> 2] >> (8 * (ib & 3));
+            const uint4 a0 = *reinterpret_cast<const uint4*>(aq + 32 * ib);
+            const uint4 a1 = *reinterpret_cast<const uint4*>(aq + 32 * ib + 16);
+            const uint32_t ax[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+            int v[2] = {0, 0};
+#pragma unroll
+            for (int l = 0; l < 4; l++) {
+                const uint2 g = grid[((qs >> (8 * l)) & 0xff) | ((qh << (8 - 2 * l)) & 0x300)];
+                const uint2 m = sgn[(sg >> (8 * l)) & 0xff];
+                v[l >> 1] = dp4a_s8s8(__vsub4(g.x ^ m.x, m.x), ax[2 * l], v[l >> 1]);
+                v[l >> 1] = dp4a_s8s8(__vsub4(g.y ^ m.y, m.y), ax[2 * l + 1], v[l >> 1]);
+            }
+            isum += (2 * (int)(s & 15) + 1) * v[0] + (2 * (int)((s >> 4) & 15) + 1) * v[1];
+        }
+        return iq_term(d, dxb, isum);
+    }
+    __device__ static __forceinline__ float dot(const uint8_t* sl, int f, int /*nrb*/, const uint8_t* aq, const int16_t* bs, float dxb) {
+        return block_dot(sl + f * SZ_IQ2_S, aq, bs, dxb);
+    }
+};
+
 // ---------------------------------------------------------------------------------------------------------------
-// Gate/up pairs of IQ1_S, IQ1_M, IQ2_XXS, IQ3_XXS, IQ3_S, Q2_K or Q3_K experts (gate and up of the same type).  Structure of rows_bulk_q4k_kernel
+// Gate/up pairs of IQ1_S, IQ1_M, IQ2_XXS, IQ2_XS, IQ2_S, IQ3_XXS, IQ3_S, Q2_K or Q3_K experts (gate and up of the same type).
+// Structure of rows_bulk_q4k_kernel
 // (token chunks, one (token, slot) work list per chunk, Q8_K activations staged side by side), with a 2-row unit per ring slot.
 // Fmt::kSharedSlot: a shared expert (p.x0 / p.x1, launcher: every token of the chunk) is slot p.slots of every token.
 constexpr int kIqMaxWarps = 16;

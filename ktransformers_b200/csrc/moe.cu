@@ -288,7 +288,7 @@ static int launch_rows_i4(const RowsParams& p, int T, int device, cudaStream_t s
     return KTB200_OK;
 }
 
-// IQ1_S / IQ1_M / IQ2_XXS / IQ3_XXS / IQ3_S / Q2_K / Q3_K gate/up pairs of routed experts through the bulk-copy ring (rows_bulk_iq_kernel, iq.cuh):
+// IQ1_S / IQ1_M / IQ2_XXS / IQ2_XS / IQ2_S / IQ3_XXS / IQ3_S / Q2_K / Q3_K gate/up pairs of routed experts through the bulk-copy ring (rows_bulk_iq_kernel, iq.cuh):
 // 2-row units, 2 slots per warp, tokens per chunk as many (<= 8) as leave room for >= 8 warps.  Returns 1 when the launch
 // does not suit it (no expert ids, gate and up of different types, rows not 16-byte aligned in pairs, a shared-expert slot
 // the format has no room for or of one token only): the generic kernels take it then.
@@ -325,6 +325,8 @@ static int launch_rows(FmtId f, const RowsParams& p_in, int T, int device, cudaS
             case KTB200_TYPE_IQ1_S: rci = launch_rows_bulk_iq<BulkIQ1S>(p, T, device, stream); break;
             case KTB200_TYPE_IQ1_M: rci = launch_rows_bulk_iq<BulkIQ1M>(p, T, device, stream); break;
             case KTB200_TYPE_IQ2_XXS: rci = launch_rows_bulk_iq<BulkIQ2XXS>(p, T, device, stream); break;
+            case KTB200_TYPE_IQ2_XS: rci = launch_rows_bulk_iq<BulkIQ2XS>(p, T, device, stream); break;
+            case KTB200_TYPE_IQ2_S: rci = launch_rows_bulk_iq<BulkIQ2S>(p, T, device, stream); break;
             case KTB200_TYPE_IQ3_XXS: rci = launch_rows_bulk_iq<BulkIQ3XXS>(p, T, device, stream); break;
             case KTB200_TYPE_IQ3_S: rci = launch_rows_bulk_iq<BulkIQ3S>(p, T, device, stream); break;
             case KTB200_TYPE_Q2_K: rci = launch_rows_bulk_iq<BulkQ2K>(p, T, device, stream); break;
@@ -487,6 +489,8 @@ static int launch_reduce(FmtId f, const ReduceParams& p_in, int T, int device, c
             case KTB200_TYPE_IQ1_S: rc = launch_reduce_bulk<BulkIQ1S>(p, T, device, stream); break;
             case KTB200_TYPE_IQ1_M: rc = launch_reduce_bulk<BulkIQ1M>(p, T, device, stream); break;
             case KTB200_TYPE_IQ2_XXS: rc = launch_reduce_bulk<BulkIQ2XXS>(p, T, device, stream); break;
+            case KTB200_TYPE_IQ2_XS: rc = launch_reduce_bulk<BulkIQ2XS>(p, T, device, stream); break;
+            case KTB200_TYPE_IQ2_S: rc = launch_reduce_bulk<BulkIQ2S>(p, T, device, stream); break;
             case KTB200_TYPE_IQ3_XXS: rc = launch_reduce_bulk<BulkIQ3XXS>(p, T, device, stream); break;
             case KTB200_TYPE_IQ3_S: rc = launch_reduce_bulk<BulkIQ3S>(p, T, device, stream); break;
         }
@@ -650,8 +654,8 @@ void grouped_set_trace(long long* t);
 // same split between MOE::forward_one and MOE::forward_many (moe.cpp:367-377, threshold group_min_len).  48 tokens for the
 // K-quants (Q5_K's per-pair kernels stay faster only below about 40 tokens at DeepSeek-V3's shapes; Q3_K's and Q2_K's bulk-copy
 // per-pair kernels up to about 100 / 150 tokens, a crossover this threshold does not follow yet: DESIGN.md §5, §8); 80 for a
-// handle with an IQ1_S, IQ1_M, IQ2_XXS, IQ3_XXS or IQ3_S tensor, whose per-pair kernels stay faster up to about 68 tokens at
-// DeepSeek-R1's shapes (IQ3: DESIGN.md §4.13);
+// handle with an IQ1_S, IQ1_M, IQ2_XXS, IQ2_XS, IQ2_S, IQ3_XXS or IQ3_S tensor, whose per-pair kernels stay faster up to about
+// 68 tokens at DeepSeek-R1's shapes (IQ3: DESIGN.md §4.13, IQ2_XS / IQ2_S: §4.14);
 // 96 for RAWINT4_G32, whose per-pair kernels stay faster up to 88 tokens at Kimi-K2's shapes (DESIGN.md §5).  KTB200_GROUPED_MIN, when set, is the threshold of every handle (0: never).
 void ktb200_debug_grouped(long long* trace_dev) { ktb::grouped_set_trace(trace_dev); }
 static int grouped_min_qlen(const ktb200_moe_config& c) {

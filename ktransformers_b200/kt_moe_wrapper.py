@@ -6,7 +6,7 @@ API mirror of kt-kernel's factory (kt-kernel/python/experts.py:72-262) and its i
 cuda_stream)`, the capture-batch-size helpers.  What changes underneath:
 
   * `method="B200_GGUF"`: the layer's GGUF expert tensors (`blk.L.ffn_{gate,up,down}_exps.weight`, any K-quant the
-    sm_90a kernels take, or IQ1_S / IQ1_M / IQ2_XXS / IQ3_XXS / IQ3_S) are uploaded as raw blocks and consumed on the GPU through the C-ABI (`ktb200_moe_*`);
+    sm_90a kernels take, or IQ1_S / IQ1_M / IQ2_XXS / IQ2_XS / IQ2_S / IQ3_XXS / IQ3_S) are uploaded as raw blocks and consumed on the GPU through the C-ABI (`ktb200_moe_*`);
     there is no CPU worker pool, so `cpuinfer_threads`, `threadpool_count`, `numa_nodes`, `cpu_save` are accepted and
     ignored, and `submit_forward` launches on `cuda_stream` while `sync_forward` only hands back the (stream-ordered)
     output buffer — the two names keep their meaning for callers such as SGLang's KTEPWrapperMethod.
@@ -30,7 +30,7 @@ import torch
 
 from .native import RAWINT4_G32
 from .operators.experts import KExpertsB200
-from .util.custom_gguf import GGML_NAMES, B200_EXPERT_LOAD_TYPES
+from .util.custom_gguf import GGML_NAMES, B200_ROUTED_LOAD_TYPES
 from .util.custom_loader import ModelLoaderFactory
 
 B200_METHODS = frozenset(["B200_GGUF", "B200_RAWINT4"])
@@ -132,7 +132,7 @@ class KTMoEWrapper:
 
     def _load(self, raw, types, p2l):
         for t in types.values():
-            if GGML_NAMES.get(t) not in B200_EXPERT_LOAD_TYPES:
+            if GGML_NAMES.get(t) not in B200_ROUTED_LOAD_TYPES:
                 raise ValueError(f"ggml type {GGML_NAMES.get(t, t)} is not supported by the sm_90a kernels")
         w = {n: self._permute(raw[n], self.num_experts, p2l) for n in ("gate", "up", "down")}
         w.update(gate_type=types["gate"], up_type=types["up"], down_type=types["down"])

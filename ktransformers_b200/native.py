@@ -22,6 +22,7 @@ GGML_F32, GGML_F16, GGML_Q8_0, GGML_Q2_K, GGML_Q3_K, GGML_Q4_K, GGML_Q5_K, GGML_
 GGML_IQ4_XS, GGML_BF16 = 23, 30
 GGML_IQ2_XXS, GGML_IQ1_S, GGML_IQ1_M = 16, 19, 29   # codebook i-quants: routed experts only
 GGML_IQ3_XXS, GGML_IQ3_S = 18, 21
+GGML_IQ2_XS, GGML_IQ2_S = 17, 22
 # not a ggml id (include/ktb200.h): symmetric INT4, group 32, bf16 scales, in the layout ktb200_rawint4_pack writes
 RAWINT4_G32 = 256
 

@@ -22,7 +22,7 @@ import torch
 from torch import nn
 
 from .. import native
-from ..util.custom_gguf import GGML_NAMES, TORCH_TO_GGML_HIDDEN, B200_WEIGHT_TYPES, B200_EXPERT_LOAD_TYPES
+from ..util.custom_gguf import GGML_NAMES, TORCH_TO_GGML_HIDDEN, B200_WEIGHT_TYPES, B200_ROUTED_LOAD_TYPES
 from ..util.utils import InferenceState
 from .base_operator import BaseInjectedModule
 
@@ -79,7 +79,7 @@ class KExpertsBase(ABC):
 class KExpertsB200(KExpertsBase):
     """GPU-resident GGUF experts on the hand-written sm_90a kernels: per-pair GEMV kernels for decode batches, and the grouped
     tensor-core GEMM from 48 tokens up for Q2_K / Q3_K / Q4_K / Q5_K / Q6_K experts (80 with an IQ1_S / IQ1_M / IQ2_XXS /
-    IQ3_XXS / IQ3_S tensor)."""
+    IQ2_XS / IQ2_S / IQ3_XXS / IQ3_S tensor)."""
 
     # graph-safe output buffers per device, like KExpertsCPU.output_gpu_map (experts.py:147)
     output_gpu_map: dict = {}
@@ -114,7 +114,7 @@ class KExpertsB200(KExpertsBase):
         if n_i4 not in (0, 3):
             raise ValueError("KExpertsB200: RAWINT4_G32 must be the type of all three expert tensors")
         for t in (self.gate_type, self.up_type, self.down_type) if not n_i4 else ():
-            if GGML_NAMES.get(t) not in B200_EXPERT_LOAD_TYPES:
+            if GGML_NAMES.get(t) not in B200_ROUTED_LOAD_TYPES:
                 raise ValueError(f"KExpertsB200: ggml type {GGML_NAMES.get(t, t)} is not supported by the sm_90a kernels")
         E = self.n_routed_experts
         per, lo = E // self.ep_size, (E // self.ep_size) * self.ep_rank
@@ -340,7 +340,7 @@ class KTransformersExpertsV2(KTransformersExperts):
     """experts.py:1273-1350: the balance-serve variant whose forward carries `bsz_tensor` (device-side live batch size) and a
     CUDA-graph slot.  With `prefill_op: None` the generate experts serve both phases (one GPU-resident KExpertsB200: per-pair
     GEMV kernels for decode batches, the grouped tensor-core path from 48 tokens up for Q2_K-Q6_K experts, 80 for IQ1_S /
-    IQ1_M / IQ2_XXS / IQ3_XXS / IQ3_S experts)."""
+    IQ1_M / IQ2_XXS / IQ2_XS / IQ2_S / IQ3_XXS / IQ3_S experts)."""
 
     def forward(self, input_tensor, expert_ids, weights, bsz_tensor=None, cuda_graph_idx=0):
         if self.mode == InferenceState.GENERATE or (self.mode == InferenceState.PREFILL and self.prefill_experts is None):

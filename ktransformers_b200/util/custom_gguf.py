@@ -69,10 +69,13 @@ B200_WEIGHT_TYPES = {"Q2_K", "Q3_K", "Q4_K", "Q5_K", "Q6_K", "IQ4_XS"}
 B200_EXPERT_TYPES = B200_WEIGHT_TYPES | {"IQ1_S", "IQ2_XXS"}
 # routed experts with IQ1_M: kept apart from B200_EXPERT_TYPES, whose value callers and tests rely on
 B200_ROUTED_EXPERT_TYPES = B200_EXPERT_TYPES | {"IQ1_M"}
-# what the routed-expert loaders accept: also ggml's 3-bit i-quants (llama.cpp's IQ3_XXS / IQ3_XS / IQ3_S / IQ3_M DeepSeek
-# files).  A set of its own, so that the sets above keep their values
+# routed experts with ggml's 3-bit i-quants (llama.cpp's IQ3_XXS / IQ3_XS / IQ3_S / IQ3_M DeepSeek files): kept apart from the
+# sets above for the same reason
 B200_EXPERT_LOAD_TYPES = B200_ROUTED_EXPERT_TYPES | {"IQ3_XXS", "IQ3_S"}
-B200_DEQUANT_TYPES = B200_EXPERT_LOAD_TYPES | {"Q8_0", "F32", "F16", "BF16"}
+# what the routed-expert loaders accept: also ggml's 2-bit i-quants with 9 / 10-bit grid indices (the experts of llama.cpp's
+# IQ2_XS / IQ2_S / IQ2_M DeepSeek files).  A set of its own, so that the sets above keep their values
+B200_ROUTED_LOAD_TYPES = B200_EXPERT_LOAD_TYPES | {"IQ2_XS", "IQ2_S"}
+B200_DEQUANT_TYPES = B200_ROUTED_LOAD_TYPES | {"Q8_0", "F32", "F16", "BF16"}
 # the (gate/up, down) type sets the single-launch expert-parallel kernel takes (gate and up of one type): Q4_K gate/up with
 # Q4_K or Q6_K down, and Q2_K or Q3_K gate/up with Q2_K, Q3_K, Q4_K or Q6_K down (llama.cpp's Q2_K, Q3_K_S and Q3_K_M files)
 B200_EP_TYPE_SETS = {("Q4_K", "Q4_K"), ("Q4_K", "Q6_K")} | {(gu, d) for gu in ("Q2_K", "Q3_K") for d in ("Q2_K", "Q3_K", "Q4_K", "Q6_K")}

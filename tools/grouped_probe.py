@@ -1,7 +1,8 @@
 """Times the grouped (prefill) MoE path at DeepSeek-V3 shapes (E 256, H 7168, I 2048, k 8, BF16) against the per-pair kernels,
 for the expert type sets Q4_K/Q4_K/Q6_K, DeepSeek-R1's IQ1_S x3, IQ1_S/IQ1_S/IQ2_XXS, IQ1_M x3 ("iq1mx3") and IQ1_M/IQ1_M/IQ2_XXS
 ("iq1m_iq1m_iq2"), the 3-bit i-quant sets IQ3_XXS x3 ("iq3xxsx3"), IQ3_XXS/IQ3_XXS/IQ3_S ("iq3xxs_iq3xxs_iq3s") and IQ3_S x3
-("iq3sx3"), and the K-quant mixes "q5k" (Q5_K/Q5_K/Q6_K,
+("iq3sx3"), the 2-bit i-quant sets IQ2_XS x3 ("iq2xsx3"), IQ2_XS/IQ2_XS/IQ2_S ("iq2xs_iq2xs_iq2s") and IQ2_S x3 ("iq2sx3"), and
+the K-quant mixes "q5k" (Q5_K/Q5_K/Q6_K,
 Q5_K_M), "q3k" (Q3_K/Q3_K/Q4_K, Q3_K_M), "q2k" (Q2_K/Q2_K/Q3_K, Q2_K) and "q2k_q6k" (Q2_K/Q2_K/Q6_K: the per-pair kernels refuse
 a Q3_K down projection at these shapes, so this set gives Q2_K gate / up a per-pair time); and set "i4" at Kimi-K2's shapes
 (RAWINT4_G32 x3, E 384, 60 MoE layers), packed with ktb200_rawint4_pack from seeded words and scales as tools/rawint4_probe.py.
@@ -25,15 +26,18 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 Q2_K, Q3_K, Q4_K, Q5_K, Q6_K, IQ2_XXS, IQ1_S, IQ1_M, BF16, I4 = 10, 11, 12, 13, 14, 16, 19, 29, 30, 256
 IQ3_XXS, IQ3_S = 18, 21
+IQ2_XS, IQ2_S = 17, 22
 TYPE_SETS = {"q4k": (Q4_K, Q4_K, Q6_K), "iq1x3": (IQ1_S,) * 3, "iq1_iq1_iq2": (IQ1_S, IQ1_S, IQ2_XXS), "i4": (I4,) * 3,
              "iq1mx3": (IQ1_M,) * 3, "iq1m_iq1m_iq2": (IQ1_M, IQ1_M, IQ2_XXS), "q5k": (Q5_K, Q5_K, Q6_K), "q3k": (Q3_K, Q3_K, Q4_K), "q2k": (Q2_K, Q2_K, Q3_K), "q2k_q6k": (Q2_K, Q2_K, Q6_K),
-             "iq3xxsx3": (IQ3_XXS,) * 3, "iq3xxs_iq3xxs_iq3s": (IQ3_XXS, IQ3_XXS, IQ3_S), "iq3sx3": (IQ3_S,) * 3}
+             "iq3xxsx3": (IQ3_XXS,) * 3, "iq3xxs_iq3xxs_iq3s": (IQ3_XXS, IQ3_XXS, IQ3_S), "iq3sx3": (IQ3_S,) * 3,
+             "iq2xsx3": (IQ2_XS,) * 3, "iq2xs_iq2xs_iq2s": (IQ2_XS, IQ2_XS, IQ2_S), "iq2sx3": (IQ2_S,) * 3}
 NAMES = {Q2_K: "Q2_K", Q3_K: "Q3_K", Q4_K: "Q4_K", Q5_K: "Q5_K", Q6_K: "Q6_K", IQ1_S: "IQ1_S", IQ1_M: "IQ1_M", IQ2_XXS: "IQ2_XXS",
-         I4: "RAWINT4_G32", IQ3_XXS: "IQ3_XXS", IQ3_S: "IQ3_S"}
-BLOCK = {Q2_K: 84, Q3_K: 110, Q4_K: 144, Q5_K: 176, Q6_K: 210, IQ1_S: 50, IQ1_M: 56, IQ2_XXS: 66, I4: 144, IQ3_XXS: 98, IQ3_S: 110}
+         I4: "RAWINT4_G32", IQ3_XXS: "IQ3_XXS", IQ3_S: "IQ3_S", IQ2_XS: "IQ2_XS", IQ2_S: "IQ2_S"}
+BLOCK = {Q2_K: 84, Q3_K: 110, Q4_K: 144, Q5_K: 176, Q6_K: 210, IQ1_S: 50, IQ1_M: 56, IQ2_XXS: 66, I4: 144, IQ3_XXS: 98, IQ3_S: 110, IQ2_XS: 74, IQ2_S: 82}
 KERNEL = {Q4_K: "grouped_gemm_kernel<0>", Q6_K: "grouped_gemm_kernel<1>", IQ1_S: "grouped_gemm_kernel<2>", IQ2_XXS: "grouped_gemm_kernel<3>",
           I4: "grouped_i4_kernel<1> (gate, BF16) / <3> (down)", Q5_K: "grouped_gemm_kernel<5>", Q3_K: "grouped_gemm_kernel<6>",
-          Q2_K: "grouped_gemm_kernel<7>", IQ1_M: "grouped_gemm_kernel<8>", IQ3_XXS: "grouped_gemm_kernel<9>", IQ3_S: "grouped_gemm_kernel<10>"}
+          Q2_K: "grouped_gemm_kernel<7>", IQ1_M: "grouped_gemm_kernel<8>", IQ3_XXS: "grouped_gemm_kernel<9>", IQ3_S: "grouped_gemm_kernel<10>",
+          IQ2_XS: "grouped_gemm_kernel<11>", IQ2_S: "grouped_gemm_kernel<12>"}
 k, H, I, HBM = 8, 7168, 2048, 3.35e12
 # (experts, MoE layers) per type set: DeepSeek-V3/R1 256 and 58, Kimi-K2 384 and 60; E in the environment overrides the experts
 SHAPE = {"i4": (384, 60)}
@@ -43,7 +47,7 @@ set_layers = lambda tset: SHAPE.get(tset, (256, 58))[1]
 
 def weights(t, n, seed, cols=H):
     """seeded raw blocks on the device: synth_blocks for the K-quants; random bytes with d in [0.75, 1.25) / 64 (IQ1_S, IQ1_M), / 512
-    (IQ2_XXS) or / 1024 (IQ3_XXS, IQ3_S) for the i-quants (every bit pattern is a valid i-quant block); RAWINT4 packed from random words and bf16 scales
+    (IQ2_XXS, IQ2_XS, IQ2_S) or / 1024 (IQ3_XXS, IQ3_S) for the i-quants (every bit pattern is a valid i-quant block); RAWINT4 packed from random words and bf16 scales
     in [0.005, 0.025) (tools/rawint4_probe.py)"""
     if t == I4:
         from ktransformers_b200 import native
@@ -59,7 +63,7 @@ def weights(t, n, seed, cols=H):
         return synth_blocks(t, n, "cuda", seed)
     g = torch.Generator(device="cuda").manual_seed(seed)
     b = torch.randint(0, 256, (n // 256, BLOCK[t]), dtype=torch.uint8, device="cuda", generator=g)
-    d = ((torch.rand(n // 256, device="cuda", generator=g) * 0.5 + 0.75) / (512 if t == IQ2_XXS else 1024 if t in (IQ3_XXS, IQ3_S) else 64)).half()
+    d = ((torch.rand(n // 256, device="cuda", generator=g) * 0.5 + 0.75) / (512 if t in (IQ2_XXS, IQ2_XS, IQ2_S) else 1024 if t in (IQ3_XXS, IQ3_S) else 64)).half()
     if t == IQ1_M:   # d in the top nibbles of the four scale words (bytes 49, 51, 53, 55), lowest nibble first
         bits = d.view(torch.int16).to(torch.int32) & 0xFFFF
         for w in range(4):

@@ -3,7 +3,8 @@
 E=256, H=7168, I=2048, k=8.  Formats (gate/up/down), chosen with FORMATS (comma-separated names, default the first three):
 IQ1_S x3 (8,601,600 B per expert), IQ1_S/IQ1_S/IQ2_XXS (9,519,104 B), Q4_K/Q4_K/Q6_K (28,557,312 B, bench.py's mix),
 IQ1_M/IQ1_M/IQ2_XXS (10,207,232 B, the 1.73-bit R1 files' experts), IQ1_M x3 (9,633,792 B), llama.cpp's 3-bit i-quant
-mixes IQ3_XXS x3 (16,859,136 B), IQ3_XXS/IQ3_XXS/IQ3_S (17,547,264 B) and IQ3_S x3 (18,923,520 B), and
+mixes IQ3_XXS x3 (16,859,136 B), IQ3_XXS/IQ3_XXS/IQ3_S (17,547,264 B) and IQ3_S x3 (18,923,520 B), the 2-bit i-quant mixes
+IQ2_XS x3 (12,730,368 B), IQ2_XS/IQ2_XS/IQ2_S (13,189,056 B) and IQ2_S x3 (14,106,624 B), and
 llama.cpp's K-quant mixes Q2_K/Q2_K/Q3_K (15,941,632 B), Q3_K/Q3_K/Q4_K (20,873,216 B) and Q3_K x3 (18,923,520 B).  SETS
 resident layer sets per format are cycled inside one CUDA graph, so consecutive layers never find their experts in the 50 MB
 L2 (the smallest set is 2.2 GB).  Reported per batch size (1 and 8): us per layer, algorithmic bytes (U x bytes per expert,
@@ -42,9 +43,11 @@ BF16, Q4_K, Q6_K = native.GGML_BF16, native.GGML_Q4_K, native.GGML_Q6_K
 Q2_K, Q3_K = native.GGML_Q2_K, native.GGML_Q3_K
 IQ1, IQ2, IQ1M = native.GGML_IQ1_S, native.GGML_IQ2_XXS, native.GGML_IQ1_M
 IQ3XXS, IQ3S = native.GGML_IQ3_XXS, native.GGML_IQ3_S
+IQ2XS, IQ2S = native.GGML_IQ2_XS, native.GGML_IQ2_S
 ALL_FORMATS = {"IQ1_Sx3": (IQ1, IQ1, IQ1), "IQ1_S/IQ2_XXS": (IQ1, IQ1, IQ2), "Q4_K/Q6_K": (Q4_K, Q4_K, Q6_K),
                "IQ1_M/IQ1_M/IQ2_XXS": (IQ1M, IQ1M, IQ2), "IQ1_Mx3": (IQ1M, IQ1M, IQ1M),
                "IQ3_XXSx3": (IQ3XXS, IQ3XXS, IQ3XXS), "IQ3_XXS/IQ3_XXS/IQ3_S": (IQ3XXS, IQ3XXS, IQ3S), "IQ3_Sx3": (IQ3S, IQ3S, IQ3S),
+               "IQ2_XSx3": (IQ2XS, IQ2XS, IQ2XS), "IQ2_XS/IQ2_XS/IQ2_S": (IQ2XS, IQ2XS, IQ2S), "IQ2_Sx3": (IQ2S, IQ2S, IQ2S),
                "Q2_K/Q2_K/Q3_K": (Q2_K, Q2_K, Q3_K), "Q3_K/Q3_K/Q4_K": (Q3_K, Q3_K, Q4_K), "Q3_Kx3": (Q3_K, Q3_K, Q3_K)}
 FORMATS = {f: ALL_FORMATS[f] for f in os.environ.get("FORMATS", "IQ1_Sx3,IQ1_S/IQ2_XXS,Q4_K/Q6_K").split(",")}
 lib = native.lib()
@@ -67,7 +70,7 @@ def iq_blocks(t, n_elems, seed):
     bb = int(lib.ktb200_type_size(t))
     g = torch.Generator(device="cuda").manual_seed(seed)
     b = torch.randint(0, 256, (n_elems // 256, bb), dtype=torch.uint8, device="cuda", generator=g)
-    d = ((torch.rand(n_elems // 256, device="cuda", generator=g) * 0.5 + 0.75) / (512 if t == IQ2 else 1024 if t in (IQ3XXS, IQ3S) else 64)).half()
+    d = ((torch.rand(n_elems // 256, device="cuda", generator=g) * 0.5 + 0.75) / (512 if t in (IQ2, IQ2XS, IQ2S) else 1024 if t in (IQ3XXS, IQ3S) else 64)).half()
     if t == IQ1M:
         iq1m_set_d(b, d)
     else:
@@ -78,7 +81,7 @@ def iq_blocks(t, n_elems, seed):
 def layer_set(types, seed):
     out = []
     for i, (t, (rows, cols)) in enumerate(zip(types, ((I, H), (I, H), (H, I)))):
-        out.append(iq_blocks(t, E * rows * cols, seed + i) if t in (IQ1, IQ2, IQ1M, IQ3XXS, IQ3S) else synth_blocks(t, E * rows * cols, "cuda", seed + i))
+        out.append(iq_blocks(t, E * rows * cols, seed + i) if t in (IQ1, IQ2, IQ1M, IQ3XXS, IQ3S, IQ2XS, IQ2S) else synth_blocks(t, E * rows * cols, "cuda", seed + i))
     return out
 
 
