@@ -86,17 +86,7 @@ extern "C" int ktb200_moe_gate_forward(const ktb200_gate_config* c, int qlen, co
     using namespace ktb;
     if (!c || !x || !idx || !w) { set_error("null pointer"); return KTB200_EINVAL; }
     if (qlen <= 0) return KTB200_OK;
-    if (c->n_experts > kGateThreads * kGateEPT) { set_error("gate: at most %d experts", kGateThreads * kGateEPT); return KTB200_EINVAL; }
-    if (c->n_experts <= 0 || c->hidden_size <= 0 || c->hidden_size % 4 || c->top_k <= 0 || c->top_k > 32 || c->top_k > c->n_experts) {
-        set_error("gate: bad shape (E=%d H=%d top_k=%d; top_k<=32, H%%4==0)", c->n_experts, c->hidden_size, c->top_k);
-        return KTB200_EINVAL;
-    }
-    if (c->n_group < 1 || c->n_group > 32 || c->n_experts % c->n_group || c->topk_group < 1 || c->topk_group > c->n_group) {
-        set_error("gate: bad grouping (n_group=%d topk_group=%d)", c->n_group, c->topk_group);
-        return KTB200_EINVAL;
-    }
-    if (c->scoring < 0 || c->scoring > 1 || c->topk_method < 0 || c->topk_method > 2) { set_error("gate: bad scoring/topk_method"); return KTB200_EINVAL; }
-    if (!is_hidden_type(c->hidden_type) || !c->weight) { set_error("gate: bad hidden_type or null weight"); return KTB200_EINVAL; }
+    if (!gate_config_ok(c)) return KTB200_EINVAL;
     int dev = 0;
     KTB_CUDA_CHECK(cudaGetDevice(&dev));
     const int d = dev & 63;

@@ -34,13 +34,43 @@ static inline int gate_splits(int E, int H, int nsms) {
     return S;
 }
 
+constexpr int kGateEPT = 4;   // experts per thread of the selecting CTA (E <= 512)
+
+// The router configurations gate_select_token takes: the one check of ktb200_moe_gate_forward, ktb200_moe_block_forward and
+// ktb200_moe_ep_block_forward (host only; it reads no device memory).  False, with the error set, otherwise.
+//   - noaux_tc scores a group by its two best experts: a group of one expert would score -inf, and the groups would then be
+//     chosen by index, not by score (the reference's topk(2) over a group of one raises).
+//   - top_k may not exceed the experts the group mask leaves, or masked experts would be chosen.
+static inline bool gate_config_ok(const ktb200_gate_config* c) {
+    if (c->n_experts <= 0 || c->n_experts > kGateThreads * kGateEPT || c->hidden_size <= 0 || c->hidden_size % 4 || c->top_k <= 0 ||
+        c->top_k > 32 || c->top_k > c->n_experts) {
+        set_error("gate: bad shape (E=%d H=%d top_k=%d; E<=%d, top_k<=32, H%%4==0)", c->n_experts, c->hidden_size, c->top_k,
+                  kGateThreads * kGateEPT);
+        return false;
+    }
+    if (c->n_group < 1 || c->n_group > 32 || c->n_experts % c->n_group || c->topk_group < 1 || c->topk_group > c->n_group) {
+        set_error("gate: bad grouping (n_group=%d topk_group=%d)", c->n_group, c->topk_group);
+        return false;
+    }
+    if (c->scoring < 0 || c->scoring > 1 || c->topk_method < 0 || c->topk_method > 2) { set_error("gate: bad scoring/topk_method"); return false; }
+    const int gs = c->n_experts / c->n_group;
+    if (c->topk_method == 0 && c->n_group > 1 && gs < 2) {
+        set_error("gate: noaux_tc needs at least 2 experts per group (E=%d n_group=%d)", c->n_experts, c->n_group);
+        return false;
+    }
+    if (c->topk_method != 1 && c->n_group > 1 && c->top_k > c->topk_group * gs) {
+        set_error("gate: top_k=%d exceeds the %d experts of topk_group=%d groups", c->top_k, c->topk_group * gs, c->topk_group);
+        return false;
+    }
+    if (!is_hidden_type(c->hidden_type) || !c->weight) { set_error("gate: bad hidden_type or null weight"); return false; }
+    return true;
+}
+
 // order-preserving float -> uint32 key
 __device__ __forceinline__ unsigned fkey(float f) {
     const unsigned u = __float_as_uint(f);
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
-
-constexpr int kGateEPT = 4;   // experts per thread of the selecting CTA (E <= 512)
 
 __device__ __forceinline__ float fkey_inv(unsigned k) {
     return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);

@@ -1499,6 +1499,7 @@ using namespace ktb;
 extern "C" int ktb200_moe_block_forward(const ktb200_gate_config* gc, ktb200_moe* m, ktb200_mlp* sh, int qlen, const void* input,
                                         void* output, int64_t* idx, float* w, const int* bsz, void* stream) {
     if (!gc || !m || !input || !output || !idx || !w) { set_error("null pointer"); return KTB200_EINVAL; }
+    if (!gate_config_ok(gc)) return KTB200_EINVAL;
     if (!m->loaded) { set_error("Not Loaded"); return KTB200_ESTATE; }
     if (sh && !sh->loaded) { set_error("shared expert: Not Loaded"); return KTB200_ESTATE; }
     if (qlen <= 0) return KTB200_OK;
@@ -1515,10 +1516,7 @@ extern "C" int ktb200_moe_block_forward(const ktb200_gate_config* gc, ktb200_moe
                                sh->gu_soa == m->gu_soa && sh->down_layout == m->down_layout && c.use_silu);
     const int nblk = c.hidden_size / QK_K, nb = c.intermediate_size / QK_K;
     bool fused = env_fused() && qlen <= kBlockMaxTokens && sh_ok && c.gate_type == KTB200_TYPE_Q4_K && c.up_type == KTB200_TYPE_Q4_K &&
-                 (fd == FMT_Q6K4T || fd == FMT_Q4K) && nblk >= 16 && nblk <= 32 && c.hidden_size % 4 == 0 && k <= 31 &&
-                 gc->n_experts <= kGateThreads * kGateEPT && gc->n_experts > 0 && gc->n_group >= 1 && gc->n_group <= 32 &&
-                 gc->n_experts % gc->n_group == 0 && gc->topk_group >= 1 && gc->topk_group <= gc->n_group && gc->weight &&
-                 gc->scoring >= 0 && gc->scoring <= 1 && gc->topk_method >= 0 && gc->topk_method <= 2 && k <= gc->n_experts;
+                 (fd == FMT_Q6K4T || fd == FMT_Q4K) && nblk >= 16 && nblk <= 32 && c.hidden_size % 4 == 0 && k <= 31;
     DeviceGuard guard(m->device);
     const int dev = m->device;
     cudaStream_t s = (cudaStream_t)stream;
@@ -1632,13 +1630,6 @@ extern "C" int ktb200_moe_block_forward(const ktb200_gate_config* gc, ktb200_moe
 extern "C" long ktb200_ep_msg_bytes(int hidden_size, int hidden_type) { return (long)hidden_size * type_size(hidden_type) + 128; }
 
 namespace ktb {
-// the router configurations the persistent kernels' grouped top-k (gate_select_token) takes
-static bool ep_gate_ok(const ktb200_gate_config* gc, int k) {
-    return gc->n_experts <= kGateThreads * kGateEPT && gc->n_experts > 0 && gc->n_group >= 1 && gc->n_group <= 32 &&
-           gc->n_experts % gc->n_group == 0 && gc->topk_group >= 1 && gc->topk_group <= gc->n_group && gc->weight && gc->scoring >= 0 &&
-           gc->scoring <= 1 && gc->topk_method >= 0 && gc->topk_method <= 2 && k <= gc->n_experts;
-}
-
 // Fills everything of an expert-parallel launch but the plan (nrows_max, region_a, ring_bytes, pa, ep_off).
 static int ep_block_params(EpParams& pp, const ktb200_gate_config* gc, ktb200_moe* m, ktb200_mlp* sh, const ktb200_ep_comm* comm,
                            const void* x_own, void* y_out, int64_t* idx, float* w, int phase_mask) {
@@ -1752,7 +1743,7 @@ static int ep_block_kq_forward(const ktb200_gate_config* gc, ktb200_moe* m, ktb2
     if (sh && (sh->H != c.hidden_size || sh->hidden_type != c.hidden_type)) {
         set_error("ep_block: the shared expert's hidden size / type differ from the routed experts'"); return KTB200_EINVAL;
     }
-    if (!ep_gate_ok(gc, k) || nblk % BulkQ2K::kNblkMultiple || nblk < 4 || c.hidden_size > 16384 || c.hidden_size % 16) {
+    if (nblk % BulkQ2K::kNblkMultiple || nblk < 4 || c.hidden_size > 16384 || c.hidden_size % 16) {
         set_error("ep_block: unsupported configuration (Q2_K / Q3_K gate/up rows need a multiple of 1024 columns, at most 16384)");
         return KTB200_EINVAL;
     }
@@ -1796,6 +1787,7 @@ static int ep_block_kq_forward(const ktb200_gate_config* gc, ktb200_moe* m, ktb2
 extern "C" int ktb200_moe_ep_block_forward(const ktb200_gate_config* gc, ktb200_moe* m, ktb200_mlp* sh, const ktb200_ep_comm* comm,
                                            const void* x_own, void* y_out, int64_t* idx, float* w, int phase_mask, void* stream) {
     if (!gc || !m || !comm || !x_own || !y_out || !idx || !w) { set_error("ep_block: null pointer"); return KTB200_EINVAL; }
+    if (!gate_config_ok(gc)) return KTB200_EINVAL;
     if (!m->loaded || (sh && !sh->loaded)) { set_error("Not Loaded"); return KTB200_ESTATE; }
     const ktb200_moe_config& c = m->cfg;
     const int k = gc->top_k, world = comm->world, rank = comm->rank;
@@ -1819,7 +1811,7 @@ extern "C" int ktb200_moe_ep_block_forward(const ktb200_gate_config* gc, ktb200_
                                sh->gu_soa == m->gu_soa && sh->down_layout == m->down_layout && c.use_silu);
     const int nblk = c.hidden_size / QK_K, nb = c.intermediate_size / QK_K;
     const bool ok = sh_ok && c.gate_type == KTB200_TYPE_Q4_K && c.up_type == KTB200_TYPE_Q4_K && (fd == FMT_Q6K4T || fd == FMT_Q4K) && nblk >= 16 &&
-                    nblk <= 32 && c.hidden_size % 16 == 0 && ep_gate_ok(gc, k) && c.hidden_size <= 16384;
+                    nblk <= 32 && c.hidden_size % 16 == 0 && c.hidden_size <= 16384;
     if (!ok) { set_error("ep_block: unsupported configuration (needs Q4_K gate/up rows of 4096..8192 columns, Q6_K/Q4_K down, shared expert of the same shapes)"); return KTB200_EINVAL; }
     const int dev = m->device;
     EpParams pp{};

@@ -427,8 +427,17 @@ class _KDeepseekMoEMixin:
         native.check(native.lib().ktb200_mlp_create(self.config.hidden_size, inter, raw[0].data_ptr(), raw[1].data_ptr(), raw[2].data_ptr(),
                                                     types[0], types[1], types[2], gen.hidden_type, self.BLOCK_MAX_TOKENS, gen.dev_index, C.byref(h)))
         native.check(native.lib().ktb200_mlp_load_weights(h, _stream(dev)))
-        self._ktb_mlp, self._ktb_mlp_raw = h, raw
+        self._ktb_mlp, self._ktb_mlp_raw, self._ktb_mlp_shape = h, raw, (inter, tuple(types))
         return h
+
+    def _ep_block_shared(self, gen, mlp):
+        """The shared-expert handle to pass to ktb200_moe_ep_block_forward, or None when the shared expert has to run as its
+        own MLP: the Q4_K kernel streams it only when it has the routed experts' intermediate size and weight types (not so
+        for n_shared_experts > 1); the Q2_K / Q3_K kernels take any."""
+        if mlp is None or gen.gate_type in (native.GGML_Q2_K, native.GGML_Q3_K):
+            return mlp
+        same = self._ktb_mlp_shape == (self.config.moe_intermediate_size, (gen.gate_type, gen.up_type, gen.down_type))
+        return mlp if same else None
 
     def _ep_check(self, gen):
         if getattr(gen, "ep_size", 1) > 1 and getattr(self, "ep_exchange", None) is None:
@@ -486,13 +495,17 @@ class _KDeepseekMoEMixin:
             hs = self._block_handles(hidden_states)
             if hs is not None:
                 cfg, moe, mlp = hs
+                ep_mlp = self._ep_block_shared(gen0, mlp)
                 x = hidden_states.reshape(1, orig_shape[-1]).contiguous()
                 capturing = torch.cuda.is_current_stream_capturing()
                 y = KExpertsB200.output_gpu_map[gen0.out_device][:1] if capturing else torch.empty_like(x)
                 idx = torch.empty((1, cfg.top_k), dtype=torch.int64, device=x.device)
                 wt = torch.empty((1, cfg.top_k), dtype=torch.float32, device=x.device)
-                native.check(native.lib().ktb200_moe_ep_block_forward(C.byref(cfg), moe, mlp, C.byref(self.ep_exchange.comm), x.data_ptr(),
+                native.check(native.lib().ktb200_moe_ep_block_forward(C.byref(cfg), moe, ep_mlp, C.byref(self.ep_exchange.comm), x.data_ptr(),
                                                                       y.data_ptr(), idx.data_ptr(), wt.data_ptr(), 7, _stream(x.device)))
+                if mlp is not None and ep_mlp is None:
+                    # y += round(shared(x)): the second rounded term, added by the same MLP handle as in the unsharded block
+                    native.check(native.lib().ktb200_mlp_forward(mlp, 1, x.data_ptr(), y.data_ptr(), 1, None, _stream(x.device)))
                 self.last_topk = (idx, wt)
                 return y.view(*orig_shape)
             return self.ep_tokens_forward(hidden_states, counts=counts)

@@ -489,15 +489,28 @@ def test_moe_block_full_shape_vs_oracle(oracle, name, E, H, I, k, ng, tg, scale)
 
 
 # ------------------------------------------------------------------------------------------ expert-parallel block
-@pytest.mark.parametrize("world,shared", [(1, True), (2, True), (4, True), (8, False)])
-def test_moe_ep_block_loopback_matches_single_gpu(world, shared):
+# routers of the expert-parallel loopback: (E, top_k, n_group, topk_group, scoring, topk_method, norm_topk_prob, scale)
+EP_ROUTERS = {
+    "v3": (32, 4, 4, 2, 0, 0, 1, 2.5),
+    "v2_router": (160, 6, 8, 3, 1, 2, 0, 16.0),          # softmax, group_limited_greedy, scaled, not normalised
+    "softmax_greedy": (128, 8, 1, 1, 1, 1, 1, 1.0),
+    "k1": (64, 1, 4, 2, 0, 0, 1, 2.5),
+    "e512_32_groups": (512, 8, 32, 8, 0, 0, 1, 2.5),     # 4 experts per selecting thread, 32 group scores
+}
+
+
+@pytest.mark.parametrize("world,shared,router", [pytest.param(1, True, "v3", id="1-True"), pytest.param(2, True, "v3", id="2-True"),
+                                                 pytest.param(4, True, "v3", id="4-True"), pytest.param(8, False, "v3", id="8-False")]
+                         + [pytest.param(w, True, r, id=f"{w}-True-{r}") for r in list(EP_ROUTERS)[1:] for w in (2, 4)])
+def test_moe_ep_block_loopback_matches_single_gpu(world, shared, router):
     """ktb200_moe_ep_block_forward — the one-launch expert-parallel layer — emulated on ONE GPU: `world` shard handles
     (experts E/world each) with their own message / partial / flag buffers in the same device memory; the three phases
     (route+send, experts+deliver, combine) run as separate launches rank by rank, which is a legal schedule of the
     real concurrent execution.  Every rank's token must come out as the single-GPU block (ktb200_moe_block_forward
     over all E experts) computes it: same routing bits, output within fp32 re-association of the partial sums."""
     import ctypes as C
-    E, k, H, I, ng, tg = 32, 4, 4096, 512, 4, 2
+    E, k, ng, tg, scoring, method, norm, scale = EP_ROUTERS[router]
+    H, I = 4096, 512
     El = E // world
     lib = native.lib()
     gate_w, up_w, down_w = _synth(Q4_K, E * I * H, 401), _synth(Q4_K, E * I * H, 402), _synth(Q6_K, E * H * I, 403)
@@ -505,8 +518,8 @@ def test_moe_ep_block_loopback_matches_single_gpu(world, shared):
     gb, db = gate_w.numel() // E, down_w.numel() // E
     rng = np.random.default_rng(world)
     Wr = rng.standard_normal((E, H)).astype(np.float32)
-    bias = rng.standard_normal(E).astype(np.float32)
-    gate = G.Gate(Wr, bias, k, ng, tg, hidden_type=BF16)
+    bias = rng.standard_normal(E).astype(np.float32) if method == 0 else None
+    gate = G.Gate(Wr, bias, k, ng, tg, scoring, method, norm, scale, hidden_type=BF16)
     full = G.Moe(E, k, H, I, gate_w.clone(), up_w.clone(), down_w.clone(), Q4_K, Q4_K, Q6_K, BF16, max_tokens=8)
     full_mlp = G.Mlp(H, I, *(t.clone() for t in sgs), Q4_K, Q4_K, Q6_K, BF16) if shared else None
     shards, mlps = [], []

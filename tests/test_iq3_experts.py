@@ -264,6 +264,19 @@ import numpy as np, torch
 sys.path[:0] = sys.argv[1:]
 from torch.profiler import ProfilerActivity, profile
 from test_iq3_experts import CENSUS_DECODE, IQ_MIN, TYPE_MIXES, _Experts, _ids, _x
+from ktransformers_b200 import native
+def session(run):
+    # even in this interpreter a session after others can miss kernels: repeat it (3 tries) until it recorded as
+    # many of the library's kernels as the library launched
+    for _ in range(3):
+        n0 = native.launch_count()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            run()
+            torch.cuda.synchronize()
+        seen = sum(e.device_type == torch.autograd.DeviceType.CUDA and 'ktb::' in e.name for e in prof.events())
+        if seen >= native.launch_count() - n0:
+            break
+    return prof.key_averages()
 res = {}
 for mix, H, I in CENSUS_DECODE:
     ex = _Experts(8, H, I, *TYPE_MIXES[mix], 60)
@@ -271,10 +284,7 @@ for mix, H, I in CENSUS_DECODE:
     rng = np.random.default_rng(61)
     ids, w, x = _ids(3, 8, 4, rng), rng.random((3, 4)).astype(np.float32), _x(3, H, 62, 0)[0]
     m.forward(ids, w, x)
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        m.forward(ids, w, x)
-        torch.cuda.synchronize()
-    res[f"decode {mix} {H} {I}"] = sorted({e.key for e in prof.key_averages() if "ktb::" in e.key})
+    res[f"decode {mix} {H} {I}"] = sorted({e.key for e in session(lambda: m.forward(ids, w, x)) if "ktb::" in e.key})
     m.close()
 for mix in sorted(TYPE_MIXES):
     ex = _Experts(8, 1024, 512, *TYPE_MIXES[mix], 5)
@@ -282,10 +292,7 @@ for mix in sorted(TYPE_MIXES):
     rng = np.random.default_rng(0)
     ids, w, x = _ids(IQ_MIN, 8, 4, rng), rng.random((IQ_MIN, 4)).astype(np.float32), _x(IQ_MIN, 1024, 1, 0)[0]
     m.forward(ids, w, x)
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        m.forward(ids, w, x)
-        torch.cuda.synchronize()
-    res[f"grouped {mix}"] = sorted({e.key for e in prof.key_averages() if "kernel" in e.key})
+    res[f"grouped {mix}"] = sorted({e.key for e in session(lambda: m.forward(ids, w, x)) if "kernel" in e.key})
     m.close()
 print("CENSUS " + json.dumps(res))
 """

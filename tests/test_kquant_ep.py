@@ -8,6 +8,7 @@ token per rank (same per-pair arithmetic, same fp32 cross-rank sum in rank order
 unsharded layer (gate, ktb200_moe_forward over all experts, ktb200_mlp_forward as a second rounded term)."""
 import ctypes as C
 import functools
+import threading
 import types
 
 import numpy as np
@@ -72,9 +73,10 @@ def _bits(t):
     return t.view(torch.int16).cpu().numpy().view(np.uint16) if t.dtype == torch.bfloat16 else t.cpu().numpy()
 
 
-def _loopback(world, E, k, H, I, ht, types_, shared, seed, ng=4, tg=2, use_silu=1, hot=None):
+def _loopback(world, E, k, H, I, ht, types_, shared, seed, ng=4, tg=2, use_silu=1, hot=None, router=None):
     """test_ep_tokens._Loopback with the shared expert of types `shared` (None: none) and routed experts of `types_`.
-    hot: an expert id whose router bias is raised so that every rank's token picks it (a crowded expert)."""
+    hot: an expert id whose router bias is raised so that every rank's token picks it (a crowded expert).
+    router: (scoring, topk_method, norm_topk_prob, scale) of a router without bias (default: the V3 router with its bias)."""
     import gpu_util as G
     from test_ep_tokens import _Loopback
     orig = G.Moe
@@ -86,6 +88,8 @@ def _loopback(world, E, k, H, I, ht, types_, shared, seed, ng=4, tg=2, use_silu=
     if hot is not None:
         lb.bias[hot] += 100.0
         lb.gate = G.Gate(lb.Wr, lb.bias, k, ng, tg, hidden_type=ht)
+    if router is not None:
+        lb.gate = G.Gate(lb.Wr, None, k, ng, tg, *router, hidden_type=ht)
     if shared is not None:
         from ktransformers_b200.util.synth import synth_blocks
         sgs = [synth_blocks(t, I * H, "cuda", seed + 40 + i) for i, t in enumerate(shared)]
@@ -138,7 +142,8 @@ def _check_against_tokens_and_unsharded(lb, xs):
 
 
 # ------------------------------------------------------------------------------------------------ GPU
-SHARED = {"none": None, "q4k_q6k": (Q4K, Q4K, Q6K), "routed": "routed"}
+SHARED = {"none": None, "q4k_q6k": (Q4K, Q4K, Q6K), "routed": "routed", "q4k_q6k_v2_router": (Q4K, Q4K, Q6K)}
+V2_ROUTER = (1, 2, 0, 16.0)   # DeepSeek-V2: softmax, group_limited_greedy (8 groups, top 3), not normalised, scaled by 16
 
 
 @pytest.mark.gpu
@@ -146,15 +151,18 @@ SHARED = {"none": None, "q4k_q6k": (Q4K, Q4K, Q6K), "routed": "routed"}
 @pytest.mark.parametrize("world", [1, 2, 4, 8])
 @pytest.mark.parametrize("types_", NEW_SETS, ids=_set_id)
 def test_ep_block_kquant_loopback(types_, world, shared):
-    """H 4096 (16 blocks a row, a multiple of 4), I 512, E 32, k 4.  Expert 5 is raised in the router so that every token picks
-    it (a crowded expert: world pairs on one expert of one shard); at world > 1 most ids lie outside any given shard."""
+    """H 4096 (16 blocks a row, a multiple of 4), I 512, E 32, k 4.  With the V3 router, expert 5 is raised in the router so
+    that every token picks it (a crowded expert: world pairs on one expert of one shard); at world > 1 most ids lie outside any
+    given shard.  The V2 router has no bias to raise."""
     sh = types_ if SHARED[shared] == "routed" else SHARED[shared]
-    lb = _loopback(world, 32, 4, 4096, 512, BF16, types_, sh, seed=7 * world + types_[0] + types_[2], hot=5)
+    v2 = shared.endswith("v2_router")
+    lb = _loopback(world, 32, 4, 4096, 512, BF16, types_, sh, seed=7 * world + types_[0] + types_[2], hot=None if v2 else 5,
+                   **(dict(ng=8, tg=3, router=V2_ROUTER) if v2 else {}))
     rng = np.random.default_rng(world * 31 + types_[2])
     for _ in range(2):   # the second layer reuses the buffers (epochs advance)
         xs = lb.tokens([1] * world, rng)
         _, idx = _check_against_tokens_and_unsharded(lb, xs)
-        assert all(5 in i[0].tolist() for i in idx)
+        assert v2 or all(5 in i[0].tolist() for i in idx)
     lb.close()
 
 
@@ -250,9 +258,9 @@ def test_ep_block_kquant_launch_census():
 
 
 # ------------------------------------------------------------------------------------------------ GPU: operator
-def _write_q2k_gguf(path, E, H, I):
-    """a two-layer DeepSeek GGUF: a dense Q4_K / Q6_K MLP in layer 0; in layer 1 Q2_K / Q2_K / Q3_K routed experts (llama.cpp's
-    Q2_K file) and a Q4_K / Q4_K / Q6_K shared expert"""
+def _write_moe_gguf(path, E, H, I, routed, n_shared=1):
+    """a two-layer DeepSeek GGUF: a dense Q4_K / Q6_K MLP in layer 0; in layer 1 routed experts of gate/up and down types
+    `routed` (Q2_K / Q3_K: llama.cpp's Q2_K file) and a Q4_K / Q4_K / Q6_K shared MLP of n_shared * I rows"""
     import gguf
     from ktransformers_b200.util.synth import synth_blocks
     rng = np.random.default_rng(17)
@@ -265,13 +273,14 @@ def _write_q2k_gguf(path, E, H, I):
         w.add_tensor(name, q.reshape(*shape[:-1], -1), raw_dtype=qt)
 
     T = gguf.GGMLQuantizationType
+    Ish = n_shared * I
     for n in ("gate", "up"):
         add_q(f"blk.0.ffn_{n}.weight", (I, H), T.Q4_K)
-        add_q(f"blk.1.ffn_{n}_exps.weight", (E, I, H), T.Q2_K)
-        add_q(f"blk.1.ffn_{n}_shexp.weight", (I, H), T.Q4_K)
+        add_q(f"blk.1.ffn_{n}_exps.weight", (E, I, H), T(routed[0]))
+        add_q(f"blk.1.ffn_{n}_shexp.weight", (Ish, H), T.Q4_K)
     add_q("blk.0.ffn_down.weight", (H, I), T.Q6_K)
-    add_q("blk.1.ffn_down_exps.weight", (E, H, I), T.Q3_K)
-    add_q("blk.1.ffn_down_shexp.weight", (H, I), T.Q6_K)
+    add_q("blk.1.ffn_down_exps.weight", (E, H, I), T(routed[1]))
+    add_q("blk.1.ffn_down_shexp.weight", (H, Ish), T.Q6_K)
     w.add_tensor("blk.1.ffn_gate_inp.weight", rng.standard_normal((E, H)).astype(np.float32))
     w.add_tensor("blk.1.exp_probs_b.bias", rng.standard_normal((E,)).astype(np.float32))
     w.write_header_to_file(); w.write_kv_data_to_file(); w.write_tensors_to_file(); w.close()
@@ -296,13 +305,15 @@ class _LoopbackExchange:
         return c
 
 
-class _DeferredBlockCalls:
+class _ConcurrentBlockCalls:
     """`native` as the operator module sees it, except that ktb200_moe_ep_block_forward (which the operator issues with
-    phase mask 7) is recorded: the test replays every rank's recorded call as phases 1, 2 and 4, rank by rank, the legal
-    one-GPU schedule of N concurrent ranks."""
+    phase mask 7) waits until every rank's thread has issued it.  Then every recorded call runs as phases 1, 2 and 4, rank
+    by rank, the legal one-GPU schedule of N concurrent ranks, and only then do the ranks' threads go on: whatever the
+    operator issues after the call is ordered behind the whole layer, as on N GPUs."""
 
-    def __init__(self, real):
-        self._real, self.calls = real, []
+    def __init__(self, real, world):
+        self._real, self.calls, self.last = real, [], []
+        self._barrier = threading.Barrier(world, action=self._replay)
         outer = self
 
         class _Lib:
@@ -312,6 +323,7 @@ class _DeferredBlockCalls:
             def ktb200_moe_ep_block_forward(self, *args):
                 assert args[-2] == 7
                 outer.calls.append(args)
+                outer._barrier.wait(timeout=600)
                 return 0
         self._lib = _Lib()
 
@@ -321,20 +333,37 @@ class _DeferredBlockCalls:
     def __getattr__(self, name):
         return getattr(self._real, name)
 
-    def replay(self):
+    def _replay(self):
+        self.last, self.calls = self.calls, []
         for mask in (1, 2, 4):
-            for a in self.calls:
+            for a in self.last:
                 native.check(native.lib().ktb200_moe_ep_block_forward(*a[:-2], mask, a[-1]))
-        self.calls = []
+
+    def run(self, fns):
+        """fns[r]() on rank r's own thread; their results, or the first error (a refused call rather than the broken barrier)"""
+        out, errs = [None] * len(fns), []
+
+        def go(r):
+            try:
+                out[r] = fns[r]()
+            except BaseException as e:      # noqa: BLE001 - handed to the test's thread below
+                errs.append(e)
+                self._barrier.abort()
+        ts = [threading.Thread(target=go, args=(r,)) for r in range(len(fns))]
+        for t in ts:
+            t.start()
+        for t in ts:
+            t.join()
+        if errs:
+            raise next((e for e in errs if not isinstance(e, threading.BrokenBarrierError)), errs[0])
+        return out
 
 
-@pytest.mark.gpu
-def test_sharded_q2k_moe_blocks_through_attach_expert_parallel(tmp_path, monkeypatch):
-    """N = 2 KDeepseekV3MoE blocks whose Q2_K / Q2_K / Q3_K experts are sharded (KExpertsB200 expert_parallel_rank / size),
-    each given its exchange by attach_expert_parallel.  One-token steps go through KDeepseekV3MoE.forward, which issues the
-    one-launch kernel with the block's shared-expert MLP handle; one multi-token step (begin_step) goes through the
-    multi-token layer.  Every rank's output matches the unsharded block: its routed experts over all E, then the shared
-    expert's MLP as a second rounded term."""
+def _sharded_blocks_through_attach_expert_parallel(tmp_path, monkeypatch, routed, n_shared):
+    """N = 2 KDeepseekV3MoE blocks whose experts are sharded (KExpertsB200 expert_parallel_rank / size), each given its exchange
+    by attach_expert_parallel.  One-token steps go through KDeepseekV3MoE.forward, which issues the one-launch kernel; one
+    multi-token step (begin_step) goes through the multi-token layer.  Every rank's output matches the unsharded block: its
+    routed experts over all E, then the shared expert's MLP as a second rounded term."""
     import copy
     from test_gpu_parity import assert_bf16_close
     from ktransformers_b200.models.modeling_deepseek_v3 import DeepseekV3Config, DeepseekV3MoEOnlyForCausalLM
@@ -345,19 +374,19 @@ def test_sharded_q2k_moe_blocks_through_attach_expert_parallel(tmp_path, monkeyp
     import ktransformers_b200.optimize.optimize as opt
     import os
     E, H, I, K, world, tmax = 8, 4096, 512, 4, 2, 16
-    _write_q2k_gguf(str(tmp_path / "q2k.gguf"), E, H, I)
+    _write_moe_gguf(str(tmp_path / "moe.gguf"), E, H, I, routed, n_shared)
     rule = os.path.join(os.path.dirname(opt.__file__), "optimize_rules", "DeepSeek-V3-Chat-b200.yaml")
     old = torch.get_default_dtype()
     torch.set_default_dtype(torch.bfloat16)
     try:
-        cfg = DeepseekV3Config(hidden_size=H, intermediate_size=I, moe_intermediate_size=I, n_routed_experts=E, n_shared_experts=1,
+        cfg = DeepseekV3Config(hidden_size=H, intermediate_size=I, moe_intermediate_size=I, n_routed_experts=E, n_shared_experts=n_shared,
                                num_experts_per_tok=K, n_group=2, topk_group=1, num_hidden_layers=2, first_k_dense_replace=1)
         with torch.device("meta"):
             model = DeepseekV3MoEOnlyForCausalLM(cfg)
         optimize_and_load_gguf(model, rule, str(tmp_path), cfg, default_device="cuda")
         moe = model.model.layers[1].mlp
         gen = moe.experts.generate_experts
-        assert (gen.gate_type, gen.up_type, gen.down_type) == (Q2K, Q2K, Q3K)
+        assert (gen.gate_type, gen.up_type, gen.down_type) == (routed[0], routed[0], routed[1])
         lay = ep.exchange_layout(world, H, BF16, K, tmax)
         bufs = [torch.zeros(lay["bytes"], dtype=torch.uint8, device="cuda") for _ in range(world)]
         blocks = []
@@ -400,14 +429,16 @@ def test_sharded_q2k_moe_blocks_through_attach_expert_parallel(tmp_path, monkeyp
                 assert int(bufs[r][lay["flags"]:lay["tokens"]].view(torch.int32)[2 * world + 1]) == 0
                 assert int(bufs[r][lay["tokens"] + lay["token_regions"]["flags"]:].view(torch.int32)[2 * world + 2]) == 0
 
-        deferred = _DeferredBlockCalls(native)
+        concurrent = _ConcurrentBlockCalls(native, world)
         for step in range(3):                     # one-token decode steps through KDeepseekV3MoE.forward
             xs = [(torch.randn(1, 1, H, device="cuda") / 10).to(torch.bfloat16) for _ in range(world)]
             with monkeypatch.context() as m:
-                m.setattr(experts_mod, "native", deferred)
-                ys = [b(xs[r]) for r, b in enumerate(blocks)]
-            assert len(deferred.calls) == world and all(a[2] == blocks[r]._ktb_mlp for r, a in enumerate(deferred.calls))
-            deferred.replay()
+                m.setattr(experts_mod, "native", concurrent)
+                ys = concurrent.run([lambda b=b, x=x: b(x) for b, x in zip(blocks, xs)])
+            # the kernel streams the shared expert when it has the routed experts' shapes and types; else it is its own MLP
+            handles = {id(b._ktb_mlp) for b in blocks}
+            assert len(concurrent.last) == world
+            assert all((a[2] is None) if n_shared > 1 else (id(a[2]) in handles) for a in concurrent.last)
             torch.cuda.synchronize()
             check(xs, ys)
 
@@ -423,6 +454,19 @@ def test_sharded_q2k_moe_blocks_through_attach_expert_parallel(tmp_path, monkeyp
         check(xs, ys)
     finally:
         torch.set_default_dtype(old)
+
+
+@pytest.mark.gpu
+def test_sharded_q2k_moe_blocks_through_attach_expert_parallel(tmp_path, monkeypatch):
+    """Q2_K / Q2_K / Q3_K experts and a Q4_K / Q4_K / Q6_K shared expert: the kernel takes the shared-expert handle"""
+    _sharded_blocks_through_attach_expert_parallel(tmp_path, monkeypatch, (Q2K, Q3K), 1)
+
+
+@pytest.mark.gpu
+def test_sharded_q4k_moe_blocks_with_two_shared_experts(tmp_path, monkeypatch):
+    """Q4_K / Q4_K / Q6_K experts and DeepSeek-V2's n_shared_experts = 2: the shared MLP has 2 I rows, which the Q4_K kernel
+    cannot stream, so the block passes no shared-expert handle and adds the MLP as its own second rounded term"""
+    _sharded_blocks_through_attach_expert_parallel(tmp_path, monkeypatch, (Q4K, Q6K), 2)
 
 
 # ------------------------------------------------------------------------------------------------ GPU: real peer memory
