@@ -404,6 +404,32 @@ int ktb200_mla_decode(const ktb200_mla_params* p, void* stream);
 /* Diagnostics: while non-NULL, one CTA of ktb200_mla_decode dumps the raw scores of its first tile (>= 2048 floats). */
 void ktb200_debug_mla(float* debug_dev);
 /* ------------------------------------------------------------------------------------------
+ * Absorbed-MLA attention of a prompt chunk over the paged latent cache (the reference's absorb_for_prefill path,
+ * q_len > 1 through the absorbed branch): no kv_b_proj decompression, the keys straight from the cache.
+ *   q_nope [B][q_len][Hq][512], q_pe [B][q_len][Hq][64] (bf16; the ktb200_mla_absorb_q output and the roped q_pe)
+ *   kv cache, page_table, kv_cache_rows, sm_scale, num_kv_splits as ktb200_mla_params
+ *   kv_len int32 [B]: each sequence's length AFTER the chunk was written to the cache
+ *   out [B][q_len][Hq][512] bf16 ; lse_out optional fp32 [B][q_len][Hq] (natural log)
+ * Causal, bottom-right aligned as ktb200_mla_prefill: with P = kv_len[b] - q_len, query i attends to keys j <= P + i.
+ * The arithmetic is ktb200_mla_decode's; at q_len == 1 the output equals it bit for bit.  Splits are planned on each
+ * sequence's last query; automatic splits never exceed ceil(SMs / (batch * q_len * ceil(Hq / 64))) nor 128.
+ * KTB200_EINVAL (before any device work) for q_len < 1, null pointers, batch > 65535 or batch * q_len * Hq >= 2^31, a
+ * workspace smaller than ktb200_mla_chunk_workspace_bytes for the splits used, and whatever ktb200_mla_decode refuses.
+ * kv_len is device data: a sequence with kv_len[b] < q_len is not refused but treated as empty (zeros, lse -inf).
+ * ------------------------------------------------------------------------------------------ */
+typedef struct ktb200_mla_chunk_params {
+    int batch, q_len, num_heads, page_size, max_pages_per_seq, num_kv_splits; /* splits <=0: auto; > 128: KTB200_EINVAL */
+    float sm_scale;
+    const void* q_nope; const void* q_pe; const void* kv_cache;
+    const int* page_table; const int* kv_len;
+    void* out; float* lse_out;
+    void* workspace; size_t workspace_bytes;
+    long kv_cache_rows;
+} ktb200_mla_chunk_params;
+/* bytes of split partials for batch * q_len query rows; max_splits <= 0: the 128-split maximum; 0 for a non-positive size */
+size_t ktb200_mla_chunk_workspace_bytes(int batch, int q_len, int num_heads, int max_splits);
+int ktb200_mla_decode_chunk(const ktb200_mla_chunk_params* p, void* stream);
+/* ------------------------------------------------------------------------------------------
  * Causal MLA prefill attention over the decompressed heads (the non-absorbed prefill of
  * archive/ktransformers/operators/attention.py:349-478: kv_b_proj, then flash_attn_func(..., causal=True)).
  * With P = kv_len - q_len tokens already cached, query i of the chunk sits at position P + i and attends to keys j <= P + i:

@@ -18,6 +18,9 @@
 // tile, while the second S is 36 small MMAs on a tile whose load dominates the time.  The O accumulator (64 x 256 fp32 per
 // warpgroup) stays in registers for the whole split.
 //
+// mla_chunk_tc_kernel is the same CTA for prompt chunks (ktb200_mla_decode_chunk): one query token per CTA, its own causal
+// key limit, the tokens of one KV split adjacent in the grid so that they read each tile from L2 (see mla_attend).
+//
 // Online softmax with a LAZY reference maximum: p = 2^(x - m_ref), m_ref is only raised (and the head's O row rescaled)
 // when the head's running maximum exceeds it by more than 8 — p stays <= 256, exact in bf16/fp32 terms.  Split-KV
 // partials (fp32 O, base-2 LSE) are merged by mla_merge_kernel.
@@ -62,6 +65,7 @@ struct MlaKParams {
     float* o_part;                 // [B][splits][Hq][512]
     float* lse_part;               // [B][splits][Hq]  (base-2)
     float* debug;                  // optional: S of the first tile [64][32], see ktb200_debug_mla
+    int q_len;                     // mla_chunk_tc_kernel: queries per sequence (q_nope [B][q_len][Hq][512], o_part / lse_part per row)
 };
 
 __device__ __forceinline__ float ex2(float x) {   // 2^x, one MUFU (x = -inf -> 0)
@@ -74,25 +78,52 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
     return *reinterpret_cast<const uint32_t*>(&v);
 }
 
-__global__ void __launch_bounds__(kMlaThreads, 1) mla_decode_tc_kernel(const __grid_constant__ CUtensorMap kv_map, const MlaKParams p) {
+// kChunk = false: decode, one query per sequence; CTA = (split, head group, sequence), query row b, keys [0, kv_len).
+// kChunk = true: a prompt chunk of q_len queries per sequence; CTA = (head group + token * head groups, split, sequence),
+// query row b * q_len + i, keys [0, P + i + 1) with P = kv_len - q_len.  Every token of a sequence splits the keys as its
+// last token does, so the CTAs of one split (adjacent in the grid) read the same tiles; a token whose limit ends before a
+// split's first tile writes that split's neutral element.  Within a CTA every row has the same limit, so the masking of
+// the decode path (S = -inf past the limit, V rows past it zeroed in shared memory) is the causal mask.
+template <bool kChunk>
+__device__ __forceinline__ void mla_attend(const CUtensorMap& kv_map, const MlaKParams& p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;           // 128-byte swizzle atoms are 1024-byte aligned
     uint8_t* smem = smem_raw + (base - raw);
     MlaMisc& misc = *reinterpret_cast<MlaMisc*>(smem + kOffMisc);
-    const int split = blockIdx.x, hg = blockIdx.y, b = blockIdx.z;
+    int split, hg, tok = 0;
+    const int b = blockIdx.z;
+    if constexpr (kChunk) {
+        const int head_groups = (p.num_heads + kHG - 1) / kHG;
+        tok = blockIdx.x / head_groups;
+        hg = blockIdx.x - tok * head_groups;
+        split = blockIdx.y;
+    } else {
+        split = blockIdx.x;
+        hg = blockIdx.y;
+    }
+    const int qrow = kChunk ? b * p.q_len + tok : b;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int h0 = hg * kHG;
     griddep_launch_dependents();
     griddep_wait();          // q, the newest cache row and kv_len come from the kernels before this one
-    int L = p.kv_len[b];
-    if (L > p.max_pages * p.page_size) L = p.max_pages * p.page_size;
-    const int ntiles = (L + kLT - 1) / kLT;
+    int L = p.kv_len[b], Lsplit;
+    if constexpr (kChunk) {
+        // kv_len < q_len cannot be refused on the host (kv_len is device data): the sequence's rows are empty (zeros)
+        Lsplit = L < p.q_len ? 0 : L;
+        L = L < p.q_len ? 0 : L - p.q_len + tok + 1;
+        Lsplit = min(Lsplit, p.max_pages * p.page_size);
+        L = min(L, p.max_pages * p.page_size);
+    } else {
+        if (L > p.max_pages * p.page_size) L = p.max_pages * p.page_size;
+        Lsplit = L;
+    }
+    const int ntiles = (Lsplit + kLT - 1) / kLT;
     const int tiles_per = (ntiles + p.num_splits - 1) / p.num_splits;
-    const int tile0 = split * tiles_per, tile1 = min(ntiles, tile0 + tiles_per);
+    const int tile0 = split * tiles_per, tile1 = min(kChunk ? (L + kLT - 1) / kLT : ntiles, tile0 + tiles_per);
     const int n = tile1 - tile0;
-    float* o_out = p.o_part + (((long)b * p.num_splits + split) * p.num_heads + h0) * kDV;
-    float* lse_out = p.lse_part + ((long)b * p.num_splits + split) * p.num_heads + h0;
+    float* o_out = p.o_part + (((long)qrow * p.num_splits + split) * p.num_heads + h0) * kDV;
+    float* lse_out = p.lse_part + ((long)qrow * p.num_splits + split) * p.num_heads + h0;
 
     if (n <= 0) {   // empty split: the neutral element of the merge
         for (int i = tid; i < kHG * kDV; i += kMlaThreads)
@@ -133,7 +164,7 @@ __global__ void __launch_bounds__(kMlaThreads, 1) mla_decode_tc_kernel(const __g
                 const int i = tid + (i0 + u) * kMlaThreads, r = i / (kDK / 8), j = i - r * (kDK / 8);
                 v[u] = make_uint4(0, 0, 0, 0);
                 if (h0 + r < p.num_heads) {
-                    const long hrow = (long)b * p.num_heads + h0 + r;
+                    const long hrow = (long)qrow * p.num_heads + h0 + r;
                     v[u] = j < 64 ? __ldg(reinterpret_cast<const uint4*>(p.q_nope + hrow * kDV) + j) : __ldg(reinterpret_cast<const uint4*>(p.q_pe + hrow * 64) + (j - 64));
                 }
             }
@@ -256,6 +287,13 @@ __global__ void __launch_bounds__(kMlaThreads, 1) mla_decode_tc_kernel(const __g
     }
 }
 
+__global__ void __launch_bounds__(kMlaThreads, 1) mla_decode_tc_kernel(const __grid_constant__ CUtensorMap kv_map, const MlaKParams p) {
+    mla_attend<false>(kv_map, p);
+}
+__global__ void __launch_bounds__(kMlaThreads, 1) mla_chunk_tc_kernel(const __grid_constant__ CUtensorMap kv_map, const MlaKParams p) {
+    mla_attend<true>(kv_map, p);
+}
+
 // out[b][h][:] = sum_s w_s * o_part[b][s][h][:],  w_s = 2^(lse_s - max) / sum ; lse (natural log) optional
 // 128 threads (4 warps), one per split: ktb200_mla_decode refuses num_kv_splits > kMaxSplits
 static_assert(kMaxSplits == 128, "mla_merge_kernel reduces over exactly 4 warps");
@@ -342,6 +380,22 @@ static EncodeTiledFn encode_tiled() {
     return fn;
 }
 
+// the paged cache as a 2-D tensor [token rows][576 columns]; a tile never crosses a page (page_size % 32 == 0)
+static int encode_kv_map(CUtensorMap* map, const void* kv_cache, long kv_cache_rows, const char* who) {
+    EncodeTiledFn enc = encode_tiled();
+    if (!enc) { set_error("%s: cuTensorMapEncodeTiled is not available from this driver", who); return KTB200_ECUDA; }
+    const cuuint64_t rows = kv_cache_rows > 0 ? (cuuint64_t)kv_cache_rows : (cuuint64_t)1 << 31;
+    const cuuint64_t gdim[2] = {(cuuint64_t)kDK, rows};
+    const cuuint64_t gstr[1] = {(cuuint64_t)kDK * 2};
+    const cuuint32_t box[2] = {64, (cuuint32_t)kLT};
+    const cuuint32_t estr[2] = {1, 1};
+    const CUresult cr = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(kv_cache), gdim, gstr, box, estr,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (cr != CUDA_SUCCESS) { set_error("%s: cuTensorMapEncodeTiled failed (%d)", who, (int)cr); return KTB200_ECUDA; }
+    return KTB200_OK;
+}
+
 static float* g_mla_debug = nullptr;
 
 }  // namespace ktb
@@ -375,19 +429,8 @@ int ktb200_mla_decode(const ktb200_mla_params* q, void* stream) {
     if (need > q->workspace_bytes) { set_error("mla_decode: workspace too small (%zu < %zu bytes for %d splits)", q->workspace_bytes, need, splits); return KTB200_EINVAL; }
     cudaStream_t s = (cudaStream_t)stream;
 
-    // the paged cache as a 2-D tensor [token rows][576 columns]; a tile never crosses a page (page_size % 32 == 0)
-    EncodeTiledFn enc = encode_tiled();
-    if (!enc) { set_error("mla_decode: cuTensorMapEncodeTiled is not available from this driver"); return KTB200_ECUDA; }
     CUtensorMap map;
-    const cuuint64_t rows = q->kv_cache_rows > 0 ? (cuuint64_t)q->kv_cache_rows : (cuuint64_t)1 << 31;
-    const cuuint64_t gdim[2] = {(cuuint64_t)kDK, rows};
-    const cuuint64_t gstr[1] = {(cuuint64_t)kDK * 2};
-    const cuuint32_t box[2] = {64, (cuuint32_t)kLT};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult cr = enc(&map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(q->kv_cache), gdim, gstr, box, estr,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) { set_error("mla_decode: cuTensorMapEncodeTiled failed (%d)", (int)cr); return KTB200_ECUDA; }
+    if (const int rc = encode_kv_map(&map, q->kv_cache, q->kv_cache_rows, "mla_decode")) return rc;
 
     MlaKParams p{};
     p.q_nope = (const __nv_bfloat16*)q->q_nope; p.q_pe = (const __nv_bfloat16*)q->q_pe;
@@ -406,6 +449,71 @@ int ktb200_mla_decode(const ktb200_mla_params* q, void* stream) {
     count_launch();
     KTB_CUDA_CHECK(launch_pdl(mla_merge_kernel, dim3(q->batch * q->num_heads), dim3(128), 0, s, (const float*)p.o_part, (const float*)p.lse_part, splits, q->num_heads,
                               (__nv_bfloat16*)q->out, q->lse_out));
+    count_launch();
+    return KTB200_OK;
+}
+
+size_t ktb200_mla_chunk_workspace_bytes(int batch, int q_len, int num_heads, int max_splits) {
+    if (batch <= 0 || q_len <= 0 || num_heads <= 0) return 0;
+    if (max_splits <= 0) max_splits = ktb::kMaxSplits;
+    return (size_t)batch * q_len * max_splits * num_heads * (ktb::kDV + 1) * sizeof(float);
+}
+
+int ktb200_mla_decode_chunk(const ktb200_mla_chunk_params* q, void* stream) {
+    using namespace ktb;
+    if (!q) { set_error("mla_decode_chunk: null params"); return KTB200_EINVAL; }
+    if (!q->q_nope || !q->q_pe || !q->kv_cache || !q->page_table || !q->kv_len || !q->out || !q->workspace) { set_error("mla_decode_chunk: null pointer"); return KTB200_EINVAL; }
+    if (q->q_len < 1) { set_error("mla_decode_chunk: q_len %d must be at least 1", q->q_len); return KTB200_EINVAL; }
+    if (q->batch <= 0) return KTB200_OK;
+    if (q->num_heads <= 0 || q->page_size <= 0 || q->page_size % kLT || q->max_pages_per_seq <= 0) {
+        set_error("mla_decode_chunk: page_size %d must be a positive multiple of %d (num_heads %d, max_pages_per_seq %d must be positive)",
+                  q->page_size, kLT, q->num_heads, q->max_pages_per_seq);
+        return KTB200_EINVAL;
+    }
+    if (((uintptr_t)q->kv_cache & 15) || ((uintptr_t)q->q_nope & 15) || ((uintptr_t)q->q_pe & 15)) { set_error("mla_decode_chunk: q / kv_cache must be 16-byte aligned"); return KTB200_EINVAL; }
+    if (q->num_kv_splits > kMaxSplits) {
+        set_error("mla_decode_chunk: num_kv_splits %d exceeds the maximum of %d", q->num_kv_splits, kMaxSplits);
+        return KTB200_EINVAL;
+    }
+    const long rows = (long)q->batch * q->q_len;
+    const int head_groups = (q->num_heads + kHG - 1) / kHG;
+    if (q->batch > 65535 || rows * q->num_heads > 0x7fffffffL) {   // grid z; merge CTAs and query rows are int
+        set_error("mla_decode_chunk: batch %d x q_len %d x num_heads %d is too large", q->batch, q->q_len, q->num_heads);
+        return KTB200_EINVAL;
+    }
+    int dev = 0;
+    const int max_tiles = q->max_pages_per_seq * (q->page_size / kLT);
+    // automatic splits: as decode with every query row counted as a sequence, planned on the chunk's last row
+    int splits = q->num_kv_splits;
+    if (splits <= 0) {
+        KTB_CUDA_CHECK(cudaGetDevice(&dev));
+        splits = pick_splits((int)rows, q->num_heads, max_tiles, dev);
+    }
+    if (splits > max_tiles) splits = max_tiles;
+    const size_t need = (size_t)rows * splits * q->num_heads * (kDV + 1) * sizeof(float);
+    if (need > q->workspace_bytes) { set_error("mla_decode_chunk: workspace too small (%zu < %zu bytes for %d splits)", q->workspace_bytes, need, splits); return KTB200_EINVAL; }
+    if (q->num_kv_splits > 0) KTB_CUDA_CHECK(cudaGetDevice(&dev));
+    CUtensorMap map;
+    if (const int rc = encode_kv_map(&map, q->kv_cache, q->kv_cache_rows, "mla_decode_chunk")) return rc;
+
+    MlaKParams p{};
+    p.q_nope = (const __nv_bfloat16*)q->q_nope; p.q_pe = (const __nv_bfloat16*)q->q_pe;
+    p.page_table = q->page_table; p.kv_len = q->kv_len; p.num_heads = q->num_heads; p.page_size = q->page_size;
+    p.max_pages = q->max_pages_per_seq; p.num_splits = splits; p.scale_log2 = q->sm_scale * 1.4426950408889634f;
+    p.o_part = (float*)q->workspace;
+    p.lse_part = p.o_part + (size_t)rows * splits * q->num_heads * kDV;
+    p.q_len = q->q_len;
+    static bool attr_set[64] = {};
+    if (!attr_set[dev & 63]) {
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(mla_chunk_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlaSmem));
+        attr_set[dev & 63] = true;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    KTB_CUDA_CHECK(launch_pdl(mla_chunk_tc_kernel, dim3(head_groups * q->q_len, splits, q->batch), dim3(kMlaThreads), (size_t)kMlaSmem, s, map, p));
+    count_launch();
+    // the merge is decode's over batch * q_len query rows
+    KTB_CUDA_CHECK(launch_pdl(mla_merge_kernel, dim3((unsigned)(rows * q->num_heads)), dim3(128), 0, s, (const float*)p.o_part, (const float*)p.lse_part, splits,
+                              q->num_heads, (__nv_bfloat16*)q->out, q->lse_out));
     count_launch();
     return KTB200_OK;
 }

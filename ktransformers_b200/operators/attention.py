@@ -12,7 +12,12 @@ projections, RoPE and cache update, then the first S = P + q_len cached latents 
 (dense, as the reference calls it) and ktb200_mla_prefill (csrc/mla_prefill.cu, wgmma + TMA) runs causal attention over
 the decompressed heads in place: q_nope from the q_b output, k_nope / v from the kv_b_proj output, k_pe from the cache
 rows.  P is the cache's host-side token count, so the path makes no device-to-host synchronisation; positions are
-[P, P + q_len), as StaticCache.update assumes.  bf16 only."""
+[P, P + q_len), as StaticCache.update assumes.  bf16 only.
+
+With absorb_for_prefill (the reference's switch, DeepSeek-V3-Chat.yaml) a chunk of q_len > 1 takes the absorbed branch
+instead: the decode steps up to absorb_q, then causal latent-space attention straight from the paged cache
+(MLAWrapper.run -> ktb200_mla_decode_chunk, lengths position_ids[:, -1] + 1 on the device, nothing decompressed), then
+absorb_o and o_proj.  Like decode, it makes no host synchronisation and can be captured in a CUDA graph."""
 from __future__ import annotations
 
 import ctypes as C
@@ -83,12 +88,14 @@ class KDeepseekV2Attention(BaseInjectedModule, DeepseekV3Attention):
         if self.mla_wrapper is None:
             self.mla_wrapper = MLAWrapperSingleton.get_instance(str(hidden_states.device), bsz, past_key_value.max_pages * bsz, use_cuda_graph=True)
         w = self.mla_wrapper
-        if w.need_plan:
-            # decode: one query per sequence, kv length = position + 1, identity page table of the static cache
+        if w.need_plan or w.q_len != q_len:
+            # q_len queries per sequence (the chunk's causal offsets follow from kv length = last position + 1), identity
+            # page table of the static cache; qo_indptr on the host, so planning makes no synchronisation
+            qo_indptr = None if q_len == 1 else torch.arange(0, bsz + 1, dtype=torch.int32) * q_len
             kv_len = (position_ids.reshape(bsz, -1)[:, -1] + 1).to(torch.int32)
             pages = past_key_value.max_pages
             indptr = torch.arange(0, bsz + 1, dtype=torch.int32, device=hidden_states.device) * pages
-            w.plan(None, indptr, page_table.reshape(-1), kv_len, None, self.num_heads, self.kv_lora_rank, self.qk_rope_head_dim,
+            w.plan(qo_indptr, indptr, page_table.reshape(-1), kv_len, None, self.num_heads, self.kv_lora_rank, self.qk_rope_head_dim,
                    past_key_value.page_size, self.softmax_scale, q_nope.dtype, ckv_pages.dtype)
             w.max_pages_per_seq = pages
         else:   # the plan is static (identity page table); only the lengths move from step to step (a captured device copy)
