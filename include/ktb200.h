@@ -430,6 +430,55 @@ typedef struct ktb200_mla_chunk_params {
 size_t ktb200_mla_chunk_workspace_bytes(int batch, int q_len, int num_heads, int max_splits);
 int ktb200_mla_decode_chunk(const ktb200_mla_chunk_params* p, void* stream);
 /* ------------------------------------------------------------------------------------------
+ * Absorbed-MLA attention of a ragged batch (the reference's BatchMLAPagedAttentionWrapper with a ragged qo_indptr): decode
+ * tokens and prompt chunks of sequences at their own positions in one call.  Planned on the host, run on the device:
+ *
+ * ktb200_mla_ragged_plan (host only, no CUDA call) fills the caller's host buffer `plan` with a work list:
+ *   qo_indptr int32 [batch + 1] (HOST): sequence b owns query rows [qo_indptr[b], qo_indptr[b + 1]); q_len_b may be 0
+ *   kv_len int32 [batch] (HOST): each sequence's length AFTER this step's tokens were written to the cache
+ *   Token i of sequence b attends to keys j < kv_len[b] - q_len_b + i + 1 (bottom-right aligned, as ktb200_mla_decode_chunk).
+ *   An item is (query row, 64-head group, tile range, partial slot).  Each sequence's keys are cut once into ranges of
+ *   tiles_per[b] tiles of 32 tokens that all its tokens share; a token gets one slot and one item per head group for every
+ *   range that starts below its limit.  num_kv_splits > 0: tiles_per[b] = ceil(tiles(kv_len[b]) / splits), the splits clamped
+ *   to max_pages_per_seq * page_size / 32, exactly the ranges of ktb200_mla_decode_chunk (and ktb200_mla_decode at q_len 1)
+ *   with that split count.  num_kv_splits <= 0: per sequence, the largest item is at most max(4, ceil(W / num_sms)) tiles,
+ *   W the (row, head group, tile) work of the whole batch, with at most 128 ranges per sequence; if the items then exceed
+ *   max_items, the bound doubles until they fit.
+ *   plan_ints >= ktb200_mla_ragged_plan_ints(max_items, max_rows).  n_slots / workspace_bytes (optional) receive the partial
+ *   slots and the workspace bytes this plan uses.
+ *   KTB200_EINVAL, nothing written, for null pointers, batch < 0, num_heads / max_pages_per_seq / num_sms <= 0, a page_size
+ *   that is not a positive multiple of 32, num_kv_splits > 128, qo_indptr[0] != 0 or decreasing, kv_len[b] < q_len_b,
+ *   kv_len[b] > max_pages_per_seq * page_size, more rows than max_rows, more items than max_items, a small buffer.
+ *
+ * ktb200_mla_decode_ragged runs a plan copied to the device (the same int32 buffer, 16-byte aligned):
+ *   q_nope [rows][Hq][512], q_pe [rows][Hq][64] (bf16): query rows in qo_indptr order; rows >= the plan's rows
+ *   kv cache, page_table [batch][max_pages_per_seq], kv_cache_rows, sm_scale as ktb200_mla_params
+ *   out [rows][Hq][512] bf16 ; lse_out optional fp32 [rows][Hq] (natural log): rows past the plan's rows get zeros, lse -inf
+ *   max_items: the plan's item capacity.  One CTA per item of the capacity (those past the plan's items return at once), so
+ *   a call captured in a CUDA graph serves every later plan of the same capacities; a plan made for another item capacity
+ *   reads as empty.  num_heads, page_size, max_pages_per_seq must be those the plan was made with.
+ *   The arithmetic is ktb200_mla_decode's.  KTB200_EINVAL (before any device work) for null pointers, rows < 0,
+ *   max_items <= 0, rows * Hq >= 2^31, a workspace smaller than ktb200_mla_ragged_workspace_bytes(max_items, Hq), an
+ *   unaligned plan, and whatever ktb200_mla_decode_chunk refuses.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct ktb200_mla_ragged_params {
+    int rows, max_items, num_heads, page_size, max_pages_per_seq;
+    float sm_scale;
+    const void* q_nope; const void* q_pe; const void* kv_cache;
+    const int* page_table; const int* plan;
+    void* out; float* lse_out;
+    void* workspace; size_t workspace_bytes;
+    long kv_cache_rows;
+} ktb200_mla_ragged_params;
+/* int32 elements of a plan: 8 header + 8 per item + max_rows + 1 row offsets; 0 for max_items <= 0 or max_rows < 0 */
+size_t ktb200_mla_ragged_plan_ints(int max_items, int max_rows);
+/* bytes of split partials for any plan of max_items items (max_items / ceil(Hq / 64) slots); 0 for a non-positive size */
+size_t ktb200_mla_ragged_workspace_bytes(int max_items, int num_heads);
+int ktb200_mla_ragged_plan(const int* qo_indptr, const int* kv_len, int batch, int num_heads, int page_size, int max_pages_per_seq,
+                           int num_sms, int num_kv_splits, int max_items, int max_rows, int* plan, size_t plan_ints, int* n_slots,
+                           size_t* workspace_bytes);
+int ktb200_mla_decode_ragged(const ktb200_mla_ragged_params* p, void* stream);
+/* ------------------------------------------------------------------------------------------
  * Causal MLA prefill attention over the decompressed heads (the non-absorbed prefill of
  * archive/ktransformers/operators/attention.py:349-478: kv_b_proj, then flash_attn_func(..., causal=True)).
  * With P = kv_len - q_len tokens already cached, query i of the chunk sits at position P + i and attends to keys j <= P + i:

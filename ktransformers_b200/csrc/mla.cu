@@ -21,10 +21,16 @@
 // mla_chunk_tc_kernel is the same CTA for prompt chunks (ktb200_mla_decode_chunk): one query token per CTA, its own causal
 // key limit, the tokens of one KV split adjacent in the grid so that they read each tile from L2 (see mla_attend).
 //
+// mla_ragged_tc_kernel is the same CTA for a ragged batch (ktb200_mla_decode_ragged): sequences with their own query counts
+// and lengths in one launch.  Each CTA takes its (query row, head group, tile range, key limit, partial slot) from a work
+// list the host planned (ktb200_mla_ragged_plan); mla_ragged_merge_kernel merges each row's own range of slots.
+//
 // Online softmax with a LAZY reference maximum: p = 2^(x - m_ref), m_ref is only raised (and the head's O row rescaled)
 // when the head's running maximum exceeds it by more than 8 — p stays <= 256, exact in bf16/fp32 terms.  Split-KV
 // partials (fp32 O, base-2 LSE) are merged by mla_merge_kernel.
 #include <cuda_bf16.h>
+
+#include <vector>
 
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -66,7 +72,15 @@ struct MlaKParams {
     float* lse_part;               // [B][splits][Hq]  (base-2)
     float* debug;                  // optional: S of the first tile [64][32], see ktb200_debug_mla
     int q_len;                     // mla_chunk_tc_kernel: queries per sequence (q_nope [B][q_len][Hq][512], o_part / lse_part per row)
+    const int* plan;               // mla_ragged_tc_kernel: the device work list (kPlanHeader, items, row offsets)
+    int max_items, rows;           // mla_ragged_tc_kernel: the plan's item capacity; query rows of q_nope
 };
+
+// The ragged work list (ktb200_mla_ragged_plan): int32 header {items, rows, slots, item capacity, row capacity, 0, 0, 0},
+// then `item capacity` items of kItemInts {query row, sequence, head group, first tile, end tile, key limit, slot, 0},
+// then row_off[row capacity + 1]: the partial slots of row r are [row_off[r], row_off[r + 1]).
+constexpr int kPlanHeader = 8, kItemInts = 8;
+enum MlaMode { kMlaDecode, kMlaChunk, kMlaRagged };
 
 __device__ __forceinline__ float ex2(float x) {   // 2^x, one MUFU (x = -inf -> 0)
     float y;
@@ -84,46 +98,64 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
 // last token does, so the CTAs of one split (adjacent in the grid) read the same tiles; a token whose limit ends before a
 // split's first tile writes that split's neutral element.  Within a CTA every row has the same limit, so the masking of
 // the decode path (S = -inf past the limit, V rows past it zeroed in shared memory) is the causal mask.
-template <bool kChunk>
+// kMlaRagged: CTA x = item x of the host-planned work list; the item names the query row, sequence, head group, tile
+// range, key limit and partial slot.  CTAs past the plan's item count (the grid is the item capacity) return at once.
+template <int kMode>
 __device__ __forceinline__ void mla_attend(const CUtensorMap& kv_map, const MlaKParams& p) {
+    constexpr bool kChunk = kMode == kMlaChunk;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;           // 128-byte swizzle atoms are 1024-byte aligned
     uint8_t* smem = smem_raw + (base - raw);
     MlaMisc& misc = *reinterpret_cast<MlaMisc*>(smem + kOffMisc);
-    int split, hg, tok = 0;
-    const int b = blockIdx.z;
+    int split = 0, hg = 0, tok = 0;
+    int b = blockIdx.z;
     if constexpr (kChunk) {
         const int head_groups = (p.num_heads + kHG - 1) / kHG;
         tok = blockIdx.x / head_groups;
         hg = blockIdx.x - tok * head_groups;
         split = blockIdx.y;
-    } else {
+    } else if constexpr (kMode == kMlaDecode) {
         split = blockIdx.x;
         hg = blockIdx.y;
     }
-    const int qrow = kChunk ? b * p.q_len + tok : b;
+    int qrow = kChunk ? b * p.q_len + tok : b;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int h0 = hg * kHG;
+    int h0 = hg * kHG;
     griddep_launch_dependents();
     griddep_wait();          // q, the newest cache row and kv_len come from the kernels before this one
-    int L = p.kv_len[b], Lsplit;
-    if constexpr (kChunk) {
-        // kv_len < q_len cannot be refused on the host (kv_len is device data): the sequence's rows are empty (zeros)
-        Lsplit = L < p.q_len ? 0 : L;
-        L = L < p.q_len ? 0 : L - p.q_len + tok + 1;
-        Lsplit = min(Lsplit, p.max_pages * p.page_size);
-        L = min(L, p.max_pages * p.page_size);
+    int L, tile0, tile1;
+    long slot;
+    if constexpr (kMode == kMlaRagged) {
+        // a plan made for another item capacity reads as empty (its row offsets sit elsewhere); rows past q_nope are skipped
+        if ((int)blockIdx.x >= p.plan[0] || p.plan[3] != p.max_items) return;
+        const int4* it = reinterpret_cast<const int4*>(p.plan + kPlanHeader + (long)kItemInts * blockIdx.x);
+        const int4 u = __ldg(it), v = __ldg(it + 1);
+        if (u.x >= p.rows) return;
+        qrow = u.x; b = u.y; hg = u.z; tile0 = u.w; tile1 = v.x; L = v.y; slot = v.z;
+        h0 = hg * kHG;
     } else {
-        if (L > p.max_pages * p.page_size) L = p.max_pages * p.page_size;
-        Lsplit = L;
+        L = p.kv_len[b];
+        int Lsplit;
+        if constexpr (kChunk) {
+            // kv_len < q_len cannot be refused on the host (kv_len is device data): the sequence's rows are empty (zeros)
+            Lsplit = L < p.q_len ? 0 : L;
+            L = L < p.q_len ? 0 : L - p.q_len + tok + 1;
+            Lsplit = min(Lsplit, p.max_pages * p.page_size);
+            L = min(L, p.max_pages * p.page_size);
+        } else {
+            if (L > p.max_pages * p.page_size) L = p.max_pages * p.page_size;
+            Lsplit = L;
+        }
+        const int ntiles = (Lsplit + kLT - 1) / kLT;
+        const int tiles_per = (ntiles + p.num_splits - 1) / p.num_splits;
+        tile0 = split * tiles_per;
+        tile1 = min(kChunk ? (L + kLT - 1) / kLT : ntiles, tile0 + tiles_per);
+        slot = (long)qrow * p.num_splits + split;
     }
-    const int ntiles = (Lsplit + kLT - 1) / kLT;
-    const int tiles_per = (ntiles + p.num_splits - 1) / p.num_splits;
-    const int tile0 = split * tiles_per, tile1 = min(kChunk ? (L + kLT - 1) / kLT : ntiles, tile0 + tiles_per);
     const int n = tile1 - tile0;
-    float* o_out = p.o_part + (((long)qrow * p.num_splits + split) * p.num_heads + h0) * kDV;
-    float* lse_out = p.lse_part + ((long)qrow * p.num_splits + split) * p.num_heads + h0;
+    float* o_out = p.o_part + (slot * p.num_heads + h0) * kDV;
+    float* lse_out = p.lse_part + slot * p.num_heads + h0;
 
     if (n <= 0) {   // empty split: the neutral element of the merge
         for (int i = tid; i < kHG * kDV; i += kMlaThreads)
@@ -288,12 +320,17 @@ __device__ __forceinline__ void mla_attend(const CUtensorMap& kv_map, const MlaK
 }
 
 __global__ void __launch_bounds__(kMlaThreads, 1) mla_decode_tc_kernel(const __grid_constant__ CUtensorMap kv_map, const MlaKParams p) {
-    mla_attend<false>(kv_map, p);
+    mla_attend<kMlaDecode>(kv_map, p);
 }
 __global__ void __launch_bounds__(kMlaThreads, 1) mla_chunk_tc_kernel(const __grid_constant__ CUtensorMap kv_map, const MlaKParams p) {
-    mla_attend<true>(kv_map, p);
+    mla_attend<kMlaChunk>(kv_map, p);
+}
+__global__ void __launch_bounds__(kMlaThreads, 1) mla_ragged_tc_kernel(const __grid_constant__ CUtensorMap kv_map, const MlaKParams p) {
+    mla_attend<kMlaRagged>(kv_map, p);
 }
 
+// out[b][h][:] = sum_s w_s * o_part[b][s][h][:],  w_s = 2^(lse_s - max) / sum ; lse (natural log) optional
+// 128 threads (4 warps), one per split: ktb200_mla_decode refuses num_kv_splits > kMaxSplits
 // out[b][h][:] = sum_s w_s * o_part[b][s][h][:],  w_s = 2^(lse_s - max) / sum ; lse (natural log) optional
 // 128 threads (4 warps), one per split: ktb200_mla_decode refuses num_kv_splits > kMaxSplits
 static_assert(kMaxSplits == 128, "mla_merge_kernel reduces over exactly 4 warps");
@@ -345,6 +382,63 @@ __global__ void __launch_bounds__(128) mla_merge_kernel(const float* o_part, con
     o2[0] = __floats2bfloat162_rn(acc.x, acc.y);
     o2[1] = __floats2bfloat162_rn(acc.z, acc.w);
     if (lse_out && tid == 0) lse_out[(long)b * num_heads + h] = (mx + log2f(den)) * 0.6931471805599453f;
+}
+
+// mla_merge_kernel for a ragged plan: one CTA per (row, head) of the launch's `rows` query rows; row r merges its own slots
+// [row_off[r], row_off[r + 1]) of o_part [slot][Hq][512] / lse_part [slot][Hq] with the same lane-per-slot code (lanes
+// past the row's count at -inf).  Rows past the plan's row count (padded CUDA-graph rows) write zeros and lse -inf.
+// A copy rather than a shared body: sharing it changed mla_merge_kernel's instruction schedule.
+__global__ void __launch_bounds__(128) mla_ragged_merge_kernel(const float* o_part, const float* lse_part, const int* plan, int max_items,
+                                                               int num_heads, __nv_bfloat16* out, float* lse_out) {
+    __shared__ float ws[kMaxSplits];
+    __shared__ float red[8];
+    griddep_launch_dependents();
+    griddep_wait();
+    const int r = blockIdx.x / num_heads, h = blockIdx.x % num_heads;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int* row_off = plan + kPlanHeader + (long)kItemInts * max_items;
+    const bool planned = plan[3] == max_items && r < plan[1];
+    const int slot0 = planned ? row_off[r] : 0, count = planned ? row_off[r + 1] - slot0 : 0;   // count <= kMaxSplits
+    const float my = tid < count ? lse_part[((long)slot0 + tid) * num_heads + h] : -INFINITY;
+    float mx = my;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (lane == 0) red[warp] = mx;
+    __syncthreads();
+    mx = fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
+    const int c = tid * 4;
+    __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(out + ((long)r * num_heads + h) * kDV + c);
+    if (mx == -INFINITY) {
+        o2[0] = __floats2bfloat162_rn(0.f, 0.f);
+        o2[1] = __floats2bfloat162_rn(0.f, 0.f);
+        if (lse_out && tid == 0) lse_out[(long)r * num_heads + h] = -INFINITY;
+        return;
+    }
+    const float e = tid < count ? exp2f(my - mx) : 0.f;
+    float den = warp_sum(e);
+    if (lane == 0) red[4 + warp] = den;
+    __syncthreads();
+    den = (red[4] + red[5]) + (red[6] + red[7]);
+    ws[tid] = e / den;
+    __syncthreads();
+    float4 acc = make_float4(0, 0, 0, 0);
+    const float* src = o_part + ((long)slot0 * num_heads + h) * kDV + c;
+    const long sstride = (long)num_heads * kDV;
+    for (int s0 = 0; s0 < count; s0 += 8) {
+        float4 v[8];
+#pragma unroll
+        for (int u = 0; u < 8; u++)
+            if (s0 + u < count) v[u] = __ldcs(reinterpret_cast<const float4*>(src + (s0 + u) * sstride));
+#pragma unroll
+        for (int u = 0; u < 8; u++)
+            if (s0 + u < count) {
+                const float w = ws[s0 + u];
+                acc.x += w * v[u].x; acc.y += w * v[u].y; acc.z += w * v[u].z; acc.w += w * v[u].w;
+            }
+    }
+    o2[0] = __floats2bfloat162_rn(acc.x, acc.y);
+    o2[1] = __floats2bfloat162_rn(acc.z, acc.w);
+    if (lse_out && tid == 0) lse_out[(long)r * num_heads + h] = (mx + log2f(den)) * 0.6931471805599453f;
 }
 
 // StaticCache.update (archive/ktransformers/models/custom_cache.py:147-200): one CTA per token
@@ -514,6 +608,174 @@ int ktb200_mla_decode_chunk(const ktb200_mla_chunk_params* q, void* stream) {
     // the merge is decode's over batch * q_len query rows
     KTB_CUDA_CHECK(launch_pdl(mla_merge_kernel, dim3((unsigned)(rows * q->num_heads)), dim3(128), 0, s, (const float*)p.o_part, (const float*)p.lse_part, splits,
                               q->num_heads, (__nv_bfloat16*)q->out, q->lse_out));
+    count_launch();
+    return KTB200_OK;
+}
+
+size_t ktb200_mla_ragged_plan_ints(int max_items, int max_rows) {
+    if (max_items <= 0 || max_rows < 0) return 0;
+    return (size_t)ktb::kPlanHeader + (size_t)ktb::kItemInts * max_items + (size_t)max_rows + 1;
+}
+
+size_t ktb200_mla_ragged_workspace_bytes(int max_items, int num_heads) {
+    if (max_items <= 0 || num_heads <= 0) return 0;
+    const int head_groups = (num_heads + ktb::kHG - 1) / ktb::kHG;   // every slot has one item per head group
+    return (size_t)(max_items / head_groups) * num_heads * (ktb::kDV + 1) * sizeof(float);
+}
+
+// Host only.  Token i of sequence b (row qo_indptr[b] + i) attends to keys [0, kv_len[b] - q_len_b + i + 1).  Sequence b's
+// tiles [0, tiles(kv_len[b])) are cut once into ranges of tiles_per[b]; a token takes the ranges that start below its limit,
+// one slot each (row_off), and one item per (range, head group).  Items are listed sequence by sequence, range by range,
+// token by token, so the CTAs that read one range are adjacent in the grid.
+int ktb200_mla_ragged_plan(const int* qo_indptr, const int* kv_len, int batch, int num_heads, int page_size, int max_pages_per_seq,
+                           int num_sms, int num_kv_splits, int max_items, int max_rows, int* plan, size_t plan_ints, int* n_slots,
+                           size_t* workspace_bytes) {
+    using namespace ktb;
+    if (!qo_indptr || !kv_len || !plan) { set_error("mla_ragged_plan: null pointer"); return KTB200_EINVAL; }
+    if (batch < 0 || num_heads <= 0 || page_size <= 0 || page_size % kLT || max_pages_per_seq <= 0 || num_sms <= 0) {
+        set_error("mla_ragged_plan: page_size %d must be a positive multiple of %d (batch %d >= 0; num_heads %d, max_pages_per_seq %d, num_sms %d positive)",
+                  page_size, kLT, batch, num_heads, max_pages_per_seq, num_sms);
+        return KTB200_EINVAL;
+    }
+    if (num_kv_splits > kMaxSplits) { set_error("mla_ragged_plan: num_kv_splits %d exceeds the maximum of %d", num_kv_splits, kMaxSplits); return KTB200_EINVAL; }
+    if (max_items <= 0 || max_rows < 0) { set_error("mla_ragged_plan: item capacity %d must be positive and row capacity %d non-negative", max_items, max_rows); return KTB200_EINVAL; }
+    const size_t need_ints = ktb200_mla_ragged_plan_ints(max_items, max_rows);
+    if (plan_ints < need_ints) { set_error("mla_ragged_plan: plan buffer too small (%zu < %zu ints)", plan_ints, need_ints); return KTB200_EINVAL; }
+    const long cap_len = (long)max_pages_per_seq * page_size;
+    if (qo_indptr[0] != 0) { set_error("mla_ragged_plan: qo_indptr[0] = %d, must be 0", qo_indptr[0]); return KTB200_EINVAL; }
+    for (int b = 0; b < batch; b++) {
+        const int q = qo_indptr[b + 1] - qo_indptr[b];
+        if (qo_indptr[b + 1] < qo_indptr[b]) { set_error("mla_ragged_plan: qo_indptr is not monotone at %d (%d > %d)", b, qo_indptr[b], qo_indptr[b + 1]); return KTB200_EINVAL; }
+        if (kv_len[b] < q) { set_error("mla_ragged_plan: kv_len[%d] = %d is shorter than its q_len %d", b, kv_len[b], q); return KTB200_EINVAL; }
+        if (kv_len[b] > cap_len) { set_error("mla_ragged_plan: kv_len[%d] = %d exceeds max_pages_per_seq * page_size = %ld", b, kv_len[b], cap_len); return KTB200_EINVAL; }
+    }
+    const int rows = batch ? qo_indptr[batch] : 0;
+    if (rows > max_rows) { set_error("mla_ragged_plan: %d query rows exceed the row capacity %d", rows, max_rows); return KTB200_EINVAL; }
+    const int head_groups = (num_heads + kHG - 1) / kHG;
+    auto tiles = [](long len) { return (len + kLT - 1) / kLT; };
+    std::vector<long> tiles_per(batch > 0 ? batch : 1, 1);
+    auto count_items = [&]() {   // items of the current tiles_per: sum over tokens of the ranges below the limit
+        long n = 0;
+        for (int b = 0; b < batch; b++) {
+            const int q = qo_indptr[b + 1] - qo_indptr[b];
+            for (int i = 0; i < q; i++) n += (tiles(kv_len[b] - q + i + 1) + tiles_per[b] - 1) / tiles_per[b];
+        }
+        return n * head_groups;
+    };
+    long items = 0;
+    if (num_kv_splits > 0) {   // ktb200_mla_decode_chunk's ranges: its split count (clamped to the page table), on kv_len
+        const long max_tiles = cap_len / kLT;
+        const long s = num_kv_splits < max_tiles ? num_kv_splits : max_tiles;
+        for (int b = 0; b < batch; b++) tiles_per[b] = kv_len[b] > 0 ? (tiles(kv_len[b]) + s - 1) / s : 1;
+        items = count_items();
+    } else {
+        // the largest item is at most max(4 tiles, the (row, head group, tile) work over the SMs), at most kMaxSplits ranges
+        // per sequence; when that does not fit the item capacity the bound doubles until it does
+        long work = 0;
+        for (int b = 0; b < batch; b++) {
+            const int q = qo_indptr[b + 1] - qo_indptr[b];
+            for (int i = 0; i < q; i++) work += tiles(kv_len[b] - q + i + 1);
+        }
+        work *= head_groups;
+        long bound = (work + num_sms - 1) / num_sms;
+        if (bound < 4) bound = 4;
+        for (;;) {
+            bool one_range = true;
+            for (int b = 0; b < batch; b++) {
+                const long t = tiles(kv_len[b]);
+                long s = (t + bound - 1) / bound;
+                if (s > kMaxSplits) s = kMaxSplits;
+                if (s < 1) s = 1;
+                one_range &= s == 1;
+                tiles_per[b] = t > 0 ? (t + s - 1) / s : 1;
+            }
+            items = count_items();
+            if (items <= max_items || one_range) break;
+            bound *= 2;
+        }
+    }
+    if (items > max_items) { set_error("mla_ragged_plan: %ld work items exceed the item capacity %d", items, max_items); return KTB200_EINVAL; }
+    int* item = plan + kPlanHeader;
+    int* row_off = plan + kPlanHeader + (long)kItemInts * max_items;
+    int slots = 0;
+    for (int b = 0; b < batch; b++) {
+        const int q = qo_indptr[b + 1] - qo_indptr[b];
+        for (int i = 0; i < q; i++) {
+            row_off[qo_indptr[b] + i] = slots;
+            slots += (int)((tiles(kv_len[b] - q + i + 1) + tiles_per[b] - 1) / tiles_per[b]);
+        }
+    }
+    row_off[rows] = slots;
+    long k = 0;
+    for (int b = 0; b < batch; b++) {
+        const int q = qo_indptr[b + 1] - qo_indptr[b];
+        if (q == 0) continue;
+        const int past = kv_len[b] - q;
+        const long ranges = (tiles(kv_len[b]) + tiles_per[b] - 1) / tiles_per[b];
+        for (long r = 0; r < ranges; r++) {
+            const long t0 = r * tiles_per[b];
+            // the tokens whose limit past + i + 1 reaches into tile t0: i >= t0 * kLT - past
+            for (long i = t0 * kLT - past > 0 ? t0 * kLT - past : 0; i < q; i++) {
+                const long limit = past + i + 1, t1 = tiles(limit) < t0 + tiles_per[b] ? tiles(limit) : t0 + tiles_per[b];
+                const int row = qo_indptr[b] + (int)i;
+                for (int g = 0; g < head_groups; g++, k++) {
+                    int* it = item + kItemInts * k;
+                    it[0] = row; it[1] = b; it[2] = g; it[3] = (int)t0; it[4] = (int)t1; it[5] = (int)limit; it[6] = row_off[row] + (int)r; it[7] = 0;
+                }
+            }
+        }
+    }
+    const int header[kPlanHeader] = {(int)items, rows, slots, max_items, max_rows, 0, 0, 0};
+    for (int i = 0; i < kPlanHeader; i++) plan[i] = header[i];
+    if (n_slots) *n_slots = slots;
+    if (workspace_bytes) *workspace_bytes = (size_t)slots * num_heads * (kDV + 1) * sizeof(float);
+    return KTB200_OK;
+}
+
+int ktb200_mla_decode_ragged(const ktb200_mla_ragged_params* q, void* stream) {
+    using namespace ktb;
+    if (!q) { set_error("mla_decode_ragged: null params"); return KTB200_EINVAL; }
+    if (!q->q_nope || !q->q_pe || !q->kv_cache || !q->page_table || !q->plan || !q->out || !q->workspace) { set_error("mla_decode_ragged: null pointer"); return KTB200_EINVAL; }
+    if (q->rows < 0 || q->max_items <= 0) { set_error("mla_decode_ragged: item capacity %d must be positive and rows %d non-negative", q->max_items, q->rows); return KTB200_EINVAL; }
+    if (q->num_heads <= 0 || q->page_size <= 0 || q->page_size % kLT || q->max_pages_per_seq <= 0) {
+        set_error("mla_decode_ragged: page_size %d must be a positive multiple of %d (num_heads %d, max_pages_per_seq %d must be positive)",
+                  q->page_size, kLT, q->num_heads, q->max_pages_per_seq);
+        return KTB200_EINVAL;
+    }
+    if (((uintptr_t)q->kv_cache & 15) || ((uintptr_t)q->q_nope & 15) || ((uintptr_t)q->q_pe & 15) || ((uintptr_t)q->plan & 15)) {
+        set_error("mla_decode_ragged: q / kv_cache / plan must be 16-byte aligned");
+        return KTB200_EINVAL;
+    }
+    if ((long)q->rows * q->num_heads > 0x7fffffffL) {   // merge CTAs
+        set_error("mla_decode_ragged: rows %d x num_heads %d is too large", q->rows, q->num_heads);
+        return KTB200_EINVAL;
+    }
+    const size_t need = ktb200_mla_ragged_workspace_bytes(q->max_items, q->num_heads);
+    if (need > q->workspace_bytes) { set_error("mla_decode_ragged: workspace too small (%zu < %zu bytes for %d items)", q->workspace_bytes, need, q->max_items); return KTB200_EINVAL; }
+    if (q->rows == 0) return KTB200_OK;
+    int dev = 0;
+    KTB_CUDA_CHECK(cudaGetDevice(&dev));
+    CUtensorMap map;
+    if (const int rc = encode_kv_map(&map, q->kv_cache, q->kv_cache_rows, "mla_decode_ragged")) return rc;
+
+    MlaKParams p{};
+    p.q_nope = (const __nv_bfloat16*)q->q_nope; p.q_pe = (const __nv_bfloat16*)q->q_pe;
+    p.page_table = q->page_table; p.num_heads = q->num_heads; p.page_size = q->page_size;
+    p.max_pages = q->max_pages_per_seq; p.scale_log2 = q->sm_scale * 1.4426950408889634f;
+    p.o_part = (float*)q->workspace;
+    const long slot_cap = q->max_items / ((q->num_heads + kHG - 1) / kHG);
+    p.lse_part = p.o_part + slot_cap * q->num_heads * kDV;   // o_part [slot capacity][Hq][512], then lse_part [slot capacity][Hq]
+    p.plan = q->plan; p.max_items = q->max_items; p.rows = q->rows;
+    static bool attr_set[64] = {};
+    if (!attr_set[dev & 63]) {
+        KTB_CUDA_CHECK(cudaFuncSetAttribute(mla_ragged_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlaSmem));
+        attr_set[dev & 63] = true;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    KTB_CUDA_CHECK(launch_pdl(mla_ragged_tc_kernel, dim3((unsigned)q->max_items), dim3(kMlaThreads), (size_t)kMlaSmem, s, map, p));
+    count_launch();
+    KTB_CUDA_CHECK(launch_pdl(mla_ragged_merge_kernel, dim3((unsigned)(q->rows * q->num_heads)), dim3(128), 0, s, (const float*)p.o_part,
+                              (const float*)p.lse_part, q->plan, q->max_items, q->num_heads, (__nv_bfloat16*)q->out, q->lse_out));
     count_launch();
     return KTB200_OK;
 }

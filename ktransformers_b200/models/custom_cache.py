@@ -63,6 +63,21 @@ class StaticCache:
             self.past_tokens[layer_idx] += q_len
         return k_out, self.page_table_list[layer_idx]
 
+    def write_tokens(self, ckv: torch.Tensor, k_pe: torch.Tensor, layer_idx: int, cache_rows: torch.Tensor, positions: torch.Tensor) -> torch.Tensor:
+        """Flat tokens at their own positions: token t (ckv [T, 512], k_pe [T, 64]) goes to position positions[t] of batch row
+        cache_rows[t] (device int tensors [T]), page cache_rows[t] * max_pages + pos // page_size, offset pos % page_size.
+        One ktb200_mla_kv_write launch, no host synchronisation; the host counter past_tokens is left alone (a batch at several
+        positions has no single length).  Returns the layer's buffer."""
+        k_out = self.key_cache[layer_idx]
+        pos = positions.to(torch.int32)
+        page_idx = (cache_rows.to(torch.int32) * self.max_pages + pos // self.page_size).contiguous()
+        page_off = (pos % self.page_size).contiguous()
+        ckv = ckv.reshape(-1, self.kv_lora_rank).contiguous()
+        kpe = k_pe.reshape(-1, self.qk_rope_head_dim).contiguous()
+        native.check(native.lib().ktb200_mla_kv_write(k_out.data_ptr(), self.page_size, ckv.data_ptr(), kpe.data_ptr(), page_idx.data_ptr(),
+                                                      page_off.data_ptr(), ckv.shape[0], torch.cuda.current_stream(k_out.device).cuda_stream))
+        return k_out
+
     def reset(self):
         for t in self.key_cache:
             t.zero_()

@@ -58,6 +58,14 @@ class MlaChunkParams(C.Structure):
                 ("lse_out", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("kv_cache_rows", C.c_long)]
 
 
+class MlaRaggedParams(C.Structure):
+    """struct ktb200_mla_ragged_params (include/ktb200.h)."""
+    _fields_ = [("rows", C.c_int), ("max_items", C.c_int), ("num_heads", C.c_int), ("page_size", C.c_int), ("max_pages_per_seq", C.c_int),
+                ("sm_scale", C.c_float), ("q_nope", C.c_void_p), ("q_pe", C.c_void_p), ("kv_cache", C.c_void_p),
+                ("page_table", C.c_void_p), ("plan", C.c_void_p), ("out", C.c_void_p), ("lse_out", C.c_void_p),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("kv_cache_rows", C.c_long)]
+
+
 class MlaPrefillParams(C.Structure):
     """struct ktb200_mla_prefill_params (include/ktb200.h); strides in elements, token / head / batch."""
     _fields_ = [("batch", C.c_int), ("q_len", C.c_int), ("kv_len", C.c_int), ("num_heads", C.c_int),
@@ -123,6 +131,10 @@ SYMBOLS = {
     "ktb200_debug_mla": (None, [_VP]),
     "ktb200_mla_chunk_workspace_bytes": (C.c_size_t, [_I, _I, _I, _I]),
     "ktb200_mla_decode_chunk": (_I, [C.POINTER(MlaChunkParams), _VP]),
+    "ktb200_mla_ragged_plan_ints": (C.c_size_t, [_I, _I]),
+    "ktb200_mla_ragged_workspace_bytes": (C.c_size_t, [_I, _I]),
+    "ktb200_mla_ragged_plan": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _VP, C.c_size_t, C.POINTER(_I), C.POINTER(C.c_size_t)]),
+    "ktb200_mla_decode_ragged": (_I, [C.POINTER(MlaRaggedParams), _VP]),
     "ktb200_mla_prefill": (_I, [C.POINTER(MlaPrefillParams), _VP]),
     "ktb200_debug_grouped": (None, [_VP]),
     "ktb200_mla_absorb_q": (_I, [_VP, _L, _L, _VP, _I, _I, _I, _VP, _I, _VP]),

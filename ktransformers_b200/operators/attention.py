@@ -17,7 +17,12 @@ rows.  P is the cache's host-side token count, so the path makes no device-to-ho
 With absorb_for_prefill (the reference's switch, DeepSeek-V3-Chat.yaml) a chunk of q_len > 1 takes the absorbed branch
 instead: the decode steps up to absorb_q, then causal latent-space attention straight from the paged cache
 (MLAWrapper.run -> ktb200_mla_decode_chunk, lengths position_ids[:, -1] + 1 on the device, nothing decompressed), then
-absorb_o and o_proj.  Like decode, it makes no host synchronisation and can be captured in a CUDA graph."""
+absorb_o and o_proj.  Like decode, it makes no host synchronisation and can be captured in a CUDA graph.
+
+forward_ragged is the flat-token entry of a serving step (balance_serve's flashinfer_attn.forward): tokens of several
+sequences at their own positions, decode tokens and prompt chunks mixed, through the same projections and RoPE, a per-token
+cache write (StaticCache.write_tokens), absorb_q, one ragged MLAWrapper call (ktb200_mla_decode_ragged), absorb_o and
+o_proj.  Its wrapper is one per device, shared by every layer, with its own row and item capacities."""
 from __future__ import annotations
 
 import ctypes as C
@@ -28,7 +33,9 @@ import torch
 from .. import native
 from ..models.modeling_deepseek_v3 import DeepseekV3Attention, apply_rotary_pos_emb
 from .base_operator import BaseInjectedModule
-from .flashinfer_wrapper import MLAWrapperSingleton
+from .flashinfer_wrapper import MLAWrapper, MLAWrapperSingleton
+
+_RAGGED_WRAPPERS: dict = {}   # device -> the MLAWrapper of forward_ragged (one plan and one split workspace for all layers)
 
 
 class KDeepseekV2Attention(BaseInjectedModule, DeepseekV3Attention):
@@ -110,6 +117,72 @@ class KDeepseekV2Attention(BaseInjectedModule, DeepseekV3Attention):
             attn = torch.matmul(attn.transpose(1, 2), out_absorb.mT).transpose(1, 2).contiguous()     # [b, 1, h, 128]
         attn = self.o_proj(attn.reshape(bsz, q_len, self.num_heads * self.v_head_dim))
         return attn, None, past_key_value
+
+    def forward_ragged(self, hidden_states: torch.Tensor, position_ids: torch.Tensor, qo_indptr: torch.Tensor, kv_len: torch.Tensor,
+                       cache_rows, past_key_value, max_rows: int = 1024, max_items: int = 4096) -> torch.Tensor:
+        """Attention of a ragged batch of flat tokens.  hidden_states [T, hidden]; position_ids [T] (device) each token's
+        position; qo_indptr [B + 1] (host) sequence b's tokens are rows [qo_indptr[b], qo_indptr[b + 1]); kv_len [B] (host)
+        each sequence's length after this step; cache_rows [B] (host) the StaticCache batch row (page range) sequence b
+        owns.  A sequence's tokens are its last q_len_b positions, kv_len[b] - q_len_b .. kv_len[b] - 1.  max_rows /
+        max_items size the shared wrapper when this call creates it.  Returns [T, hidden].  The host data reaches the device
+        through pinned, non-blocking copies, so the step makes no host synchronisation."""
+        T = hidden_states.shape[0]
+        cache = past_key_value
+        qo = torch.as_tensor(qo_indptr, dtype=torch.int32)
+        rows = torch.as_tensor(cache_rows, dtype=torch.int32)
+        B = rows.numel()
+        assert qo.numel() == B + 1 and int(qo[-1]) == T, f"qo_indptr {qo.tolist()} does not cover {T} tokens of {B} sequences"
+        dev = hidden_states.device
+        # the cache row of every token, then the cache row of every sequence: one pinned copy
+        host = torch.cat([torch.repeat_interleave(rows, qo[1:] - qo[:-1]), rows]).pin_memory()
+        rows_dev = host.to(dev, non_blocking=True)
+        token_rows, seq_rows = rows_dev[:T], rows_dev[T:]
+        x = hidden_states.view(1, T, -1)
+        pos = position_ids.view(1, T)
+        q = self.q_proj(x) if self.q_lora_rank is None else self.q_b_proj(self.q_a_layernorm(self.q_a_proj(x)))
+        q = q.view(1, T, self.num_heads, self.q_head_dim)
+        q_nope, q_pe = torch.split(q, [self.qk_nope_head_dim, self.qk_rope_head_dim], dim=-1)
+        compressed_kv = self.kv_a_proj_with_mqa(x)
+        compressed_kv, k_pe = torch.split(compressed_kv, [self.kv_lora_rank, self.qk_rope_head_dim], dim=-1)
+        compressed_kv = self.kv_a_layernorm(compressed_kv).view(1, T, 1, self.kv_lora_rank)
+        k_pe = k_pe.view(1, T, 1, self.qk_rope_head_dim)
+        cos, sin = self.rotary_emb(q_pe, pos)
+        q_pe, k_pe = apply_rotary_pos_emb(q_pe, k_pe, cos, sin, unsqueeze_dim=2)
+        kv_with_k_pe = cache.write_tokens(compressed_kv, k_pe, self.layer_idx, token_rows, position_ids)
+        ckv_pages = kv_with_k_pe[:, :, :, : self.kv_lora_rank].view(-1, cache.page_size, self.kv_lora_rank)
+        kpe_pages = kv_with_k_pe[:, :, :, self.kv_lora_rank:].view(-1, cache.page_size, self.qk_rope_head_dim)
+
+        q_absorb, out_absorb = self.get_absorbed()
+        fused = (q.dtype == torch.bfloat16 and q_absorb.dtype == torch.bfloat16 and q.is_contiguous())
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        if fused:
+            q_abs = torch.empty((T, self.num_heads, self.kv_lora_rank), dtype=q.dtype, device=dev)
+            native.check(native.lib().ktb200_mla_absorb_q(q.data_ptr(), self.q_head_dim, self.num_heads * self.q_head_dim, q_absorb.data_ptr(), self.num_heads,
+                                                          self.qk_nope_head_dim, self.kv_lora_rank, q_abs.data_ptr(), T, stream))
+            q_nope = q_abs
+        else:
+            q_nope = torch.matmul(q_nope.transpose(1, 2), q_absorb).transpose(1, 2).contiguous().reshape(T, self.num_heads, self.kv_lora_rank)
+        q_pe = q_pe.reshape(T, self.num_heads, self.qk_rope_head_dim).contiguous()
+
+        key = str(dev)
+        if key not in _RAGGED_WRAPPERS:
+            _RAGGED_WRAPPERS[key] = MLAWrapper(cache.max_batch_size, cache.max_pages, device=key, max_rows=max_rows, max_items=max_items)
+        w = _RAGGED_WRAPPERS[key]
+        assert B <= w.max_batch_size and cache.max_pages <= w.max_pages, "the shared ragged wrapper was made for a smaller cache"
+        # sequence b's page table is its cache row's: kv_indices = the static table's rows, cache.max_pages pages each
+        kv_indptr = torch.arange(0, B + 1, dtype=torch.int32, device=dev) * cache.max_pages
+        kv_indices = cache.page_table_list[self.layer_idx].index_select(0, seq_rows.long()).reshape(-1)
+        w.plan(qo, kv_indptr, kv_indices, torch.as_tensor(kv_len, dtype=torch.int32), None, self.num_heads, self.kv_lora_rank,
+               self.qk_rope_head_dim, cache.page_size, self.softmax_scale, q_nope.dtype, ckv_pages.dtype)
+        attn = w.run(q_nope, q_pe, ckv_pages, kpe_pages)
+        if fused:
+            o = torch.empty((T, self.num_heads, self.v_head_dim), dtype=attn.dtype, device=dev)
+            native.check(native.lib().ktb200_mla_absorb_o(attn.data_ptr(), out_absorb.data_ptr(), self.num_heads, self.v_head_dim, self.kv_lora_rank, o.data_ptr(),
+                                                          T, stream))
+            attn = o
+        else:
+            attn = torch.matmul(attn.view(T, self.num_heads, 1, -1), out_absorb.mT.unsqueeze(0)).view(T, self.num_heads, self.v_head_dim)
+        return self.o_proj(attn.reshape(1, T, self.num_heads * self.v_head_dim)).view(T, -1)
 
     def forward_prefill(self, q: torch.Tensor, q_pe: torch.Tensor, cache: torch.Tensor, max_pages: int, kv_seq_len: int) -> torch.Tensor:
         """Causal attention of a prompt chunk over the first kv_seq_len cached tokens of each sequence (attention.py:349-478,
