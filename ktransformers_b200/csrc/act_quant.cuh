@@ -92,7 +92,7 @@ __device__ __forceinline__ void load_block8(const void* src, long base, int hidd
 
 // Quantise `nrows` rows of `n` (multiple of 256) values into shared staging arrays, all warps of the CTA
 // cooperating.  Row r lives at src + row_off[r-th] ... expressed as src_off + r*src_stride (elements);
-// rows with skip[r] are left untouched.  Blocks are dealt round-robin to warps and processed G at a
+// rows r < 32 with bit r of skip_mask are left untouched.  Blocks are dealt round-robin to warps and processed G at a
 // time: the G global loads are issued back to back BEFORE any of the shuffle reductions, so the prologue
 // pays the memory latency once per group instead of once per block.
 //   q8 [nrows][n] int8    dx [nrows][n/256] float    bsums [nrows][n/16] int16
@@ -111,7 +111,7 @@ __device__ __forceinline__ void cta_quantize_q8k_rows(const void* src, long src_
             live[i] = gb < total;
             if (live[i]) {
                 const int r = gb / bpr, b = gb - r * bpr;
-                live[i] = !((skip_mask >> r) & 1u);
+                live[i] = !(r < 32 && ((skip_mask >> r) & 1u));
                 if (live[i]) load_block8(src, src_off + (long)r * src_stride + (long)b * QK_K + lane * 8, hidden_type, x[i]);
             }
         }

@@ -215,6 +215,23 @@ struct ReduceParams {
     int xw_out_type;        // xw_out[t][rows] and leave `out` = the routed sum only
 };
 
+// Slots of a token whose expert lies outside the shard contribute nothing (common.hpp:255-258): the down kernels neither read
+// their weights nor quantise their activations.  The mask holds slots 0..31 (the quantiser's row mask); a slot from 32 on
+// (k <= 200) is tested against its id where it is used.
+__device__ __forceinline__ bool slot_outside(const ReduceParams& p, int t, int j) {
+    const long e = p.ids ? (long)p.ids[(long)t * p.slots + j] - p.id_offset : 0;
+    return e < 0 || e >= p.n_experts;
+}
+__device__ __forceinline__ unsigned skip_mask32(const ReduceParams& p, int t) {
+    unsigned skip = 0;
+    for (int j = 0; j < p.slots && j < 32; j++)
+        if (slot_outside(p, t, j)) skip |= 1u << j;
+    return skip;
+}
+__device__ __forceinline__ bool slot_skipped(const ReduceParams& p, int t, unsigned skip, int j) {
+    return j < 32 ? (skip >> j) & 1u : slot_outside(p, t, j);
+}
+
 // Work item of a warp = (slot j, 4 consecutive output rows): the 4 rows share slot j's int8 activations,
 // one ids lookup and one 6-shuffle reduction.
 template <class Fmt, int NB>
@@ -236,11 +253,7 @@ __global__ void __launch_bounds__(kGemvThreads, kGemvCtasPerSm) reduce_kernel(co
     const int r0 = (int)((long)p.rows * blockIdx.x / gridDim.x), r1 = (int)((long)p.rows * (blockIdx.x + 1) / gridDim.x);
     const int nrows = r1 - r0;
 
-    unsigned skip = 0;  // skipped experts contribute nothing (common.hpp:255-258): do not even read their activations
-    for (int j = 0; j < k; j++) {
-        const long e = p.ids ? (long)p.ids[(long)t * k + j] - p.id_offset : 0;
-        if (e < 0 || e >= p.n_experts) skip |= 1u << j;
-    }
+    const unsigned skip = skip_mask32(p, t);
     const typename Fmt::Lane L = Fmt::lane(lane);
     const int ngroups = (nrows + RW - 1) / RW;
     const int total = ngroups * ns;
@@ -251,7 +264,7 @@ __global__ void __launch_bounds__(kGemvThreads, kGemvCtasPerSm) reduce_kernel(co
         wbase = p.w;
         row0 = r0 + hl0;
         if (j == k) { wbase = p.xw; return true; }
-        if ((skip >> j) & 1u) return false;
+        if (slot_skipped(p, t, skip, j)) return false;
         const long e = p.ids ? (long)p.ids[(long)t * k + j] - p.id_offset : 0;
         row0 += e * p.rows;
         return true;
@@ -268,7 +281,7 @@ __global__ void __launch_bounds__(kGemvThreads, kGemvCtasPerSm) reduce_kernel(co
         prefetch_item(item + nwarps);
         const int j = item / ngroups, hl0 = (item - j * ngroups) * RW;
         float res = 0.f;
-        if (j == k || !((skip >> j) & 1u)) {   // warp-uniform
+        if (j == k || !slot_skipped(p, t, skip, j)) {   // warp-uniform
             const void* wbase = p.w;
             long row0 = r0 + hl0;
             if (j == k) {
@@ -299,7 +312,7 @@ __global__ void __launch_bounds__(kGemvThreads, kGemvCtasPerSm) reduce_kernel(co
     for (int hl = threadIdx.x; hl < nrows; hl += kGemvThreads) {
         float acc = 0.f;
         for (int j = 0; j < k; j++) {
-            if ((skip >> j) & 1u) continue;
+            if (slot_skipped(p, t, skip, j)) continue;
             const float d = partial[hl * ns + j];
             acc = p.weights ? __fmaf_rn(d, p.weights[(long)t * k + j], acc) : acc + d;
         }

@@ -149,11 +149,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) reduce_pipe_q6k8_kernel(const R
     uint8_t* ring = smem + off + (size_t)warp * 2 * slot_bytes;
     const uint32_t ring_u32 = (uint32_t)__cvta_generic_to_shared(ring);
 
-    unsigned skip = 0;
-    for (int j = 0; j < k; j++) {
-        const long e = p.ids ? (long)p.ids[(long)t * k + j] - p.id_offset : 0;
-        if (e < 0 || e >= p.n_experts) skip |= 1u << j;
-    }
+    const unsigned skip = skip_mask32(p, t);
     const int total = nquads * ns;   // item = j * nquads + quad
     const int s_ql = 4 * 128 * nb, s_qh = 4 * 64 * nb, s_sc = 4 * 16 * nb, s_d = 4 * 2 * nb;
 
@@ -164,7 +160,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) reduce_pipe_q6k8_kernel(const R
             const uint8_t* wbase = reinterpret_cast<const uint8_t*>(p.w);
             long row = r0 + quad * RW;
             if (j == k) wbase = reinterpret_cast<const uint8_t*>(p.xw);
-            else if ((skip >> j) & 1u) ok = false;
+            else if (slot_skipped(p, t, skip, j)) ok = false;
             else row += (p.ids ? (long)p.ids[(long)t * k + j] - p.id_offset : 0L) * p.rows;
             if (ok) {
                 const long G = row >> 3, r8 = row & 7;
@@ -230,7 +226,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) reduce_pipe_q6k8_kernel(const R
     for (int hl = threadIdx.x; hl < nrows; hl += WARPS * 32) {
         float acc = 0.f;
         for (int j = 0; j < k; j++) {
-            if ((skip >> j) & 1u) continue;
+            if (slot_skipped(p, t, skip, j)) continue;
             const float d = partial[hl * ns + j];
             acc = p.weights ? __fmaf_rn(d, p.weights[(long)t * k + j], acc) : acc + d;
         }

@@ -372,13 +372,19 @@ static int launch_reduce_fmt(const ReduceParams& p, int T, int device, cudaStrea
     int gx = (kGemvCtasPerSm * num_sms(device) + T - 1) / T;
     if (gx > p.rows) gx = p.rows;
     if (gx < 1) gx = 1;
-    const int nrows_max = (p.rows + gx - 1) / gx + 1;
+    // A CTA stages its token's ns activation rows and a partial sum per (output row, slot) of its share of the rows.  At
+    // prompt sizes gx falls towards 1 and the share towards all rows: raise gx to the least that leaves room for the
+    // partial sums (unchanged wherever the share fits already); refuse only when one row per CTA does not fit.
+    constexpr size_t cap = 220 * 1024;
     const size_t per_slot = (size_t)p.ncols + (size_t)nblk * 4 + (size_t)p.ncols / 8;
-    const size_t smem = per_slot * ns + (size_t)nrows_max * ns * 4;
-    if (smem > 220 * 1024) {
+    const long rows_fit = per_slot * ns < cap ? (long)((cap - per_slot * ns) / ((size_t)ns * 4)) - 1 : 0;
+    if (rows_fit < 1) {
         set_error("reduce kernel: k=%d x ncols=%d does not fit shared memory", ns, p.ncols);
         return KTB200_EINVAL;
     }
+    if (gx < (p.rows + rows_fit - 1) / rows_fit) gx = (int)((p.rows + rows_fit - 1) / rows_fit);
+    const int nrows_max = (p.rows + gx - 1) / gx + 1;
+    const size_t smem = per_slot * ns + (size_t)nrows_max * ns * 4;
     dim3 grid(gx, T);
 #define KTB_RED(NB)                                                                        \
     do {                                                                                   \
