@@ -172,6 +172,14 @@ typedef struct ktb200_fp8_linear ktb200_fp8_linear;
 int ktb200_fp8_linear_create(int in_features, int out_features, const void* weight_e4m3_dev, const float* weight_scale_inv_dev, int hidden_type, int device,
                              ktb200_fp8_linear** out);
 void ktb200_fp8_linear_destroy(ktb200_fp8_linear* l);
+/* Two routes, chosen from qlen and the shape; the results agree within the oracle's bound (DESIGN.md §4.6).
+ *   qlen below 32 / 48 / 96 tokens (32 by default, 48 for in >= 16384, 96 for out <= 2048): decode passes of 16 tokens, each
+ *     streaming the weights; allocation-free, capturable as above.
+ *   from there on: the tokens are quantised once per chunk of at most 2048 into a grow-only per-device scratch arena shared by
+ *     every handle, and a tiled GEMM (128 weight rows x 128 tokens per CTA) reads each weight once per chunk.  Deterministic (no
+ *     K splits, no atomics).  A call that would have to grow the arena while its stream is capturing returns KTB200_ESTATE
+ *     before any device work: run one eager call on the prompt route at this in_features (or larger) on the device before
+ *     capture.  Calls on one device must be stream-ordered with each other (they share the arena). */
 int ktb200_fp8_linear_forward(ktb200_fp8_linear* l, int qlen, const void* x, void* y, const int* bsz, void* stream);
 
 /* ------------------------------------------------------------------------------------------

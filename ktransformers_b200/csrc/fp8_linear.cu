@@ -17,6 +17,14 @@
 //     each (quantise x for the CTA's K range while the first weight boxes are in flight, then MMA and scale), warp 8 the TMA
 //     producer (4-stage ring).
 // K splits add their fp32 partial sums with atomics into a zeroed workspace; the last CTA of a row tile converts and re-zeroes.
+//
+// Prompt-sized batches (qlen >= fp8_prompt_min) take a second route that reads each weight once per token chunk instead of once
+// per 16 tokens: fp8_gemm_quant_kernel quantises the chunk once into a per-device arena (fp16-widened e4m3 in the K order above,
+// scales transposed to [kb][token]), then fp8_gemm_kernel computes [128 weight rows x 128 tokens] tiles with the same arithmetic:
+//     grid = row tiles x token tiles (banded raster), one CTA per SM; 384 threads: warps 0-7 = two MMA warpgroups of 64 weight
+//     rows x 128 tokens (widen the weights in registers, 8 fp16 wgmma m64n128k16 per 128 of K into a fresh accumulator, then
+//     acc = acc + (dot * a_s) * b_s), warps 8-11 the TMA producer warpgroup (4-stage ring: weight box, two activation boxes and
+//     the 128 token scales per stage).  No K splits: every output is written once, by one CTA, in kb order.
 #include <cuda.h>
 #include <cuda_fp8.h>
 
@@ -256,6 +264,140 @@ __global__ void __launch_bounds__(kFThreads, 2) fp8_linear_kernel(const __grid_c
     }
 }
 
+// ------------------------------------------------------------------------------------------------ prompt route
+constexpr int kPT = 128;                                          // tokens per CTA (the MMA's N)
+constexpr int kPStages = 4, kPA = 128 * 128, kPB = kPT * 128 * 2, kPS = kPT * 4;   // 16 KB weights + 32 KB fp16 x + 512 B scales
+constexpr int kPOffB = kPStages * kPA, kPOffS = kPOffB + kPStages * kPB, kPOffMisc = kPOffS + kPStages * kPS;
+constexpr int kPConsumerWarps = 8, kPThreads = (kPConsumerWarps + 4) * 32;
+constexpr int kPChunk = 2048;                                     // tokens per GEMM launch: bounds the arena
+constexpr int kPBand = 16;                                        // row tiles per raster band: a wave shares weight and x boxes in L2
+struct Fp8GemmMisc {
+    unsigned long long full[kPStages], free_[kPStages];
+};
+constexpr int kPSmem = kPOffMisc + (int)sizeof(Fp8GemmMisc) + 1024;
+
+struct Fp8GemmParams {
+    void* y;                  // [T][N], already offset to the chunk
+    const float* scale_inv;   // [ceil(N/128)][nkb]
+    const int* bsz;
+    int hidden_type, T, N, nkb, row_tiles, token_tiles, t0;
+};
+
+// one warp per (token, 128 of K): fp8_quant_block, then the e4m3 values widened to fp16 at the K positions the GEMM's B tile
+// expects (the physical -> logical map of fp8_store_b), scales transposed so that one token tile's 128 scales of a kb are contiguous
+__global__ void __launch_bounds__(256) fp8_gemm_quant_kernel(const void* x, int hidden_type, int T, int K, int pitch, uint16_t* xh, float* xs) {
+    const int lane = threadIdx.x & 31, blk = blockIdx.x * 8 + (threadIdx.x >> 5), nkb = K / 128;
+    griddep_launch_dependents();
+    if (blk >= T * nkb) return;
+    const int t = blk / nkb, kb = blk - t * nkb;
+    float v[4];
+    fp8_load4(x, (long)t * K + (long)kb * 128 + lane * 4, hidden_type, v);
+    uint32_t packed;
+    const float s = fp8_quant_block(v, packed);
+    const int l0 = 64 * (lane >> 4) + 16 * (lane & 3) + 2 * ((lane >> 2) & 3);
+    uint32_t* row = reinterpret_cast<uint32_t*>(xh + (long)t * K + (long)kb * 128);
+    row[l0 >> 1] = fp8x2_to_f16x2(packed & 0xffffu);
+    row[(l0 + 8) >> 1] = fp8x2_to_f16x2(packed >> 16);
+    if (lane == 0) xs[(long)kb * pitch + t] = s;
+}
+
+__global__ void __launch_bounds__(kPThreads, 1) fp8_gemm_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ CUtensorMap xmap,
+                                                                const __grid_constant__ CUtensorMap smap, const Fp8GemmParams p) {
+    const int band_ctas = kPBand * p.token_tiles, band = blockIdx.x / band_ctas, in_band = blockIdx.x - band * band_ctas;
+    const int band_rows = min(kPBand, p.row_tiles - band * kPBand);
+    const int rt = band * kPBand + in_band % band_rows, tt = in_band / band_rows;
+    const int live = p.bsz ? max(0, min(p.T, *p.bsz - p.t0)) : p.T;   // bsz was written before the quantiser (a full dependency)
+    if (tt * kPT >= live) return;                                    // a token tile wholly beyond the live batch: no MMA, no store
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t raw = smem_u32(smem_raw);
+    const uint32_t base = (raw + 1023u) & ~1023u;
+    uint8_t* smem = smem_raw + (base - raw);
+    Fp8GemmMisc& misc = *reinterpret_cast<Fp8GemmMisc*>(smem + kPOffMisc);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) {
+        for (int s = 0; s < kPStages; s++) { bar_init(smem_u32(&misc.full[s]), 1); bar_init(smem_u32(&misc.free_[s]), kPConsumerWarps); }
+        bar_fence_init();
+        tma_prefetch_desc(&wmap); tma_prefetch_desc(&xmap); tma_prefetch_desc(&smap);
+    }
+    __syncthreads();
+
+    if (warp >= kPConsumerWarps) {
+        regs_dec<40>();
+        if (warp == kPConsumerWarps && lane == 0) {
+            griddep_wait();   // the quantised chunk comes from the kernel before this one
+            for (int i = 0; i < p.nkb; i++) {
+                const int s = i % kPStages;
+                const uint32_t full = smem_u32(&misc.full[s]), bb = base + kPOffB + s * kPB;
+                bar_wait(smem_u32(&misc.free_[s]), ((i / kPStages) & 1) ^ 1);
+                bar_expect_tx(full, kPA + kPB + kPS);
+                tma_load_2d(base + s * kPA, &wmap, full, i * 128, rt * 128);
+                tma_load_2d(bb, &xmap, full, i * 128, tt * kPT);
+                tma_load_2d(bb + kPT * 128, &xmap, full, i * 128 + 64, tt * kPT);
+                tma_load_2d(base + kPOffS + s * kPS, &smap, full, tt * kPT, i);
+            }
+        }
+        return;
+    }
+    regs_inc<232>();   // 128 x 40 + 256 x 232 <= 64 K registers
+    // warpgroup g owns weight rows 64 g .. 64 g + 63 of the tile; register 4 j + e: row r0 + 8 (e / 2), token 8 j + 2 c + e % 2
+    const int g = warp >> 2, r0 = 64 * g + 16 * (warp & 3) + (lane >> 2), c = lane & 3;
+    float acc[64], d[64];
+#pragma unroll
+    for (int q = 0; q < 64; q++) acc[q] = 0.f;
+    const float* sinv = p.scale_inv + (long)rt * p.nkb;
+    for (int i = 0; i < p.nkb; i++) {
+        const int s = i % kPStages;
+        const float bs = __ldg(sinv + i);
+        bar_wait(smem_u32(&misc.full[s]), (i / kPStages) & 1);
+        uint4 w[2][2];   // the decode kernel's A fragments: [row r0, r0 + 8][half of the 128 block], bytes 16 c .. 16 c + 15
+#pragma unroll
+        for (int rr = 0; rr < 2; rr++)
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int r = r0 + 8 * rr;
+                w[rr][h] = *reinterpret_cast<const uint4*>(smem + s * kPA + r * 128 + ((((4 * h + c) ^ (r & 7))) << 4));
+            }
+        uint32_t a[2][4][4];
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int st = 0; st < 4; st++) {
+                const uint32_t w0 = st == 0 ? w[0][h].x : st == 1 ? w[0][h].y : st == 2 ? w[0][h].z : w[0][h].w;
+                const uint32_t w1 = st == 0 ? w[1][h].x : st == 1 ? w[1][h].y : st == 2 ? w[1][h].z : w[1][h].w;
+                a[h][st][0] = fp8x2_to_f16x2(w0 & 0xffffu); a[h][st][1] = fp8x2_to_f16x2(w1 & 0xffffu);
+                a[h][st][2] = fp8x2_to_f16x2(w0 >> 16); a[h][st][3] = fp8x2_to_f16x2(w1 >> 16);
+            }
+        fence();
+        const uint32_t bb = base + kPOffB + s * kPB;
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int st = 0; st < 4; st++)
+                mma_f16_rs_m64n128(d, a[h][st], smem_desc(bb + h * (kPT * 128) + st * 32, 16, 1024, kLayoutSw128), (h | st) != 0);
+        commit();
+        wait<0>();
+        fence_regs(d);
+        const float* as = reinterpret_cast<const float*>(smem + kPOffS + s * kPS);
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            const float2 sc = *reinterpret_cast<const float2*>(as + 8 * j + 2 * c);
+#pragma unroll
+            for (int e = 0; e < 4; e++)   // (dot * a_s) * b_s, then +=
+                acc[4 * j + e] = __fadd_rn(acc[4 * j + e], __fmul_rn(__fmul_rn(d[4 * j + e], (e & 1) ? sc.y : sc.x), bs));
+        }
+        // the stage is free once the MMAs that read it have completed and its scales are in registers
+        __syncwarp();
+        if (lane == 0) bar_arrive(smem_u32(&misc.free_[s]));
+    }
+#pragma unroll
+    for (int j = 0; j < 16; j++)
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            const int t = tt * kPT + 8 * j + 2 * c + (e & 1), n = rt * 128 + r0 + 8 * (e >> 1);
+            if (t < live && n < p.N) store_hidden(p.y, (long)t * p.N + n, p.hidden_type, acc[4 * j + e]);
+        }
+}
+
 typedef CUresult (*EncodeTiledFn8)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
                                    CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 static EncodeTiledFn8 encode_tiled8() {
@@ -266,6 +408,45 @@ static EncodeTiledFn8 encode_tiled8() {
         return (EncodeTiledFn8)f;
     }();
     return fn;
+}
+
+// The route: prompt-sized batches go through fp8_gemm_kernel, everything shorter through the decode passes.  Up to 128 tokens
+// the GEMM costs one token tile whatever the count, so the crossover is where the decode route's passes (one per 16 tokens)
+// overtake it.  Measured at DeepSeek-V3's module shapes with tools/fp8_prefill_probe.py (DESIGN.md §4.6):
+//   N <= 2048   (16 row tiles or fewer: few CTAs per token tile)   from 96 tokens (64 is faster on the decode route)
+//   K >= 16384  (128 or more K blocks per CTA)                       from 48 tokens (32 is faster on the decode route)
+//   otherwise                                                       from 32 tokens, the floor: calls shorter than two decode
+//                                                                   passes always take the decode route
+static int fp8_prompt_min(int N, int K) { return N <= 2048 ? 96 : K >= 16384 ? 48 : 32; }
+static bool fp8_prompt_route(int qlen, int N, int K) { return qlen >= fp8_prompt_min(N, K); }
+
+// One grow-only arena per device, shared by every handle (calls on one device are stream-ordered by the caller):
+// [kPChunk or fewer tokens][K] fp16 activations, then [K / 128][pitch] fp32 scales.
+struct Fp8Scratch {
+    size_t cap = 0;
+    void* buf = nullptr;
+};
+static Fp8Scratch g_fp8[64];
+
+static int fp8_ensure(int dev, int N, int K, size_t need, cudaStream_t s) {
+    Fp8Scratch& a = g_fp8[dev & 63];
+    if (a.cap >= need) return KTB200_OK;
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    KTB_CUDA_CHECK(cudaStreamIsCapturing(s, &cs));
+    if (cs != cudaStreamCaptureStatusNone) {
+        set_error("fp8_linear: this prompt call needs %zu bytes of prompt scratch on device %d, which holds %zu; the arena cannot grow "
+                  "while the stream is capturing: run one eager call of %d or more tokens at in_features >= %d on this device before capture",
+                  need, dev, a.cap, fp8_prompt_min(N, K), K);
+        return KTB200_ESTATE;
+    }
+    // grow to a whole chunk at this K, so that one warm-up call of any prompt length covers every later length
+    const size_t full = (size_t)kPChunk * K * 2 + (size_t)(K / 128) * kPChunk * sizeof(float);
+    KTB_CUDA_CHECK(cudaDeviceSynchronize());   // earlier calls may still be using the arena
+    cudaFree(a.buf);
+    a = Fp8Scratch();
+    KTB_CUDA_CHECK(cudaMalloc(&a.buf, full > need ? full : need));
+    a.cap = full > need ? full : need;
+    return KTB200_OK;
 }
 }  // namespace ktb
 
@@ -279,6 +460,45 @@ struct ktb200_fp8_linear {
     uint8_t* xq;   // [kFT][K] e4m3
     float* xs;     // [kFT][nkb]
 };
+
+namespace ktb {
+// qlen tokens in balanced chunks of whole token tiles (at most kPChunk): per chunk one quantiser launch and one GEMM launch
+static int fp8_forward_prompt(ktb200_fp8_linear* l, int qlen, const void* x, void* y, const int* bsz, cudaStream_t s) {
+    const int nch = (qlen + kPChunk - 1) / kPChunk;
+    const int Tc = ((qlen + nch - 1) / nch + kPT - 1) / kPT * kPT;
+    const size_t xh_bytes = (size_t)Tc * l->K * 2, need = xh_bytes + (size_t)l->nkb * Tc * sizeof(float);
+    int rc = fp8_ensure(l->device, l->N, l->K, need, s);
+    if (rc) return rc;
+    EncodeTiledFn8 enc = encode_tiled8();
+    uint16_t* xh = reinterpret_cast<uint16_t*>(g_fp8[l->device & 63].buf);
+    float* xs = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(xh) + xh_bytes);
+    const size_t hb = type_size(l->hidden_type);
+    for (int t0 = 0; t0 < qlen; t0 += Tc) {
+        const int T = qlen - t0 < Tc ? qlen - t0 : Tc;
+        // rows T .. of a token tile and rows N .. of a weight tile are filled with zeros by TMA; no output of theirs is stored
+        CUtensorMap xmap, smap;
+        const cuuint64_t xdim[2] = {(cuuint64_t)l->K, (cuuint64_t)T}, xstr[1] = {(cuuint64_t)l->K * 2};
+        const cuuint64_t sdim[2] = {(cuuint64_t)T, (cuuint64_t)l->nkb}, sstr[1] = {(cuuint64_t)Tc * sizeof(float)};
+        const cuuint32_t xbox[2] = {64, kPT}, sbox[2] = {kPT, 1}, estr[2] = {1, 1};
+        CUresult cr = enc(&xmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, xh, xdim, xstr, xbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (cr == CUDA_SUCCESS)
+            cr = enc(&smap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, xs, sdim, sstr, sbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                     CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (cr != CUDA_SUCCESS) { set_error("fp8_linear: cuTensorMapEncodeTiled failed for the prompt scratch (%d)", (int)cr); return KTB200_ECUDA; }
+        Fp8GemmParams p{};
+        p.y = reinterpret_cast<uint8_t*>(y) + (size_t)t0 * l->N * hb;
+        p.scale_inv = l->scale_inv; p.bsz = bsz; p.t0 = t0;
+        p.hidden_type = l->hidden_type; p.T = T; p.N = l->N; p.nkb = l->nkb;
+        p.row_tiles = l->row_tiles; p.token_tiles = (T + kPT - 1) / kPT;
+        fp8_gemm_quant_kernel<<<(T * l->nkb + 7) / 8, 256, 0, s>>>(reinterpret_cast<const uint8_t*>(x) + (size_t)t0 * l->K * hb, l->hidden_type, T, l->K, Tc,
+                                                                   xh, xs);
+        KTB_CUDA_CHECK(launch_pdl(fp8_gemm_kernel, dim3(p.row_tiles * p.token_tiles), dim3(kPThreads), (size_t)kPSmem, s, l->map, xmap, smap, p));
+        count_launch(2);
+    }
+    return KTB200_OK;
+}
+}  // namespace ktb
 
 extern "C" {
 
@@ -319,6 +539,7 @@ int ktb200_fp8_linear_create(int in_features, int out_features, const void* weig
     if (e == cudaSuccess) e = cudaMalloc(&l->xq, (size_t)kFT * in_features);
     if (e == cudaSuccess) e = cudaMalloc(&l->xs, (size_t)kFT * l->nkb * sizeof(float));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(fp8_linear_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFSmem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(fp8_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPSmem);
     if (e != cudaSuccess) { set_error("fp8_linear: %s", cudaGetErrorString(e)); cudaFree(l->ws); cudaFree(l->tickets); cudaFree(l->xq); cudaFree(l->xs); delete l; return KTB200_ENOMEM; }
     *out = l;
     return KTB200_OK;
@@ -336,8 +557,9 @@ int ktb200_fp8_linear_forward(ktb200_fp8_linear* l, int qlen, const void* x, voi
     if (!l || !x || !y) { set_error("fp8_linear: null pointer"); return KTB200_EINVAL; }
     if (qlen <= 0) return KTB200_OK;
     DeviceGuard g(l->device);
+    if (fp8_prompt_route(qlen, l->N, l->K)) return fp8_forward_prompt(l, qlen, x, y, bsz, (cudaStream_t)stream);
     const size_t hb = type_size(l->hidden_type);
-    for (int t0 = 0; t0 < qlen; t0 += kFT) {   // decode-sized passes; a prefill batch re-streams the weights every 16 tokens
+    for (int t0 = 0; t0 < qlen; t0 += kFT) {   // decode-sized passes: each re-streams the weights
         Fp8Params p{};
         p.x = reinterpret_cast<const uint8_t*>(x) + (size_t)t0 * l->K * hb;
         p.y = reinterpret_cast<uint8_t*>(y) + (size_t)t0 * l->N * hb;

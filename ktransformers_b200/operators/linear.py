@@ -174,8 +174,11 @@ class KLinearB200(KLinearBase):
 class KLinearFP8(KLinearBase):
     """DeepSeek-V3's native FP8 checkpoints: e4m3 weight [out][in] + fp32 `weight_scale_inv` per 128 x 128 block, activations
     quantised per token and 128 values inside the kernel.  Same contract as the reference's KLinearFP8 (operators/linear.py:388-435:
-    `load(w=(weight, weight_scale_inv))`, `forward(x, bsz_tensor)`), which runs Triton's act_quant + fp8_gemm; here one launch of
-    `ktb200_fp8_linear_forward` (TMA -> e4m3 widened to fp16 in registers -> fp16 wgmma, csrc/fp8_linear.cu)."""
+    `load(w=(weight, weight_scale_inv))`, `forward(x, bsz_tensor)`), which runs Triton's act_quant + fp8_gemm; here
+    `ktb200_fp8_linear_forward` (TMA -> e4m3 widened to fp16 in registers -> fp16 wgmma, csrc/fp8_linear.cu).  Decode batches
+    stream the weights once per 16 tokens; prompts (from 32, 48 or 96 tokens by shape, DESIGN.md §4.6) run a tiled GEMM that
+    reads each weight once per 2048-token chunk, so `prefill_op: None` serves both phases.  The prompt route uses a grow-only
+    per-device scratch arena: before capturing a CUDA graph that contains a prompt-sized call, run one such call eagerly."""
 
     def __init__(self, key, gguf_loader, config, orig_module=None, device: str = "cuda", block_size: int = 128, **kwargs):
         super().__init__(key, gguf_loader, config, orig_module, device, **kwargs)
