@@ -196,6 +196,16 @@ int ktb200_linear_load_weights(ktb200_linear* lin, void* stream);
 /* y[qlen][out] = x[qlen][in] * W^T ; bias_dev optional fp32 [out] added before rounding */
 int ktb200_linear_forward(ktb200_linear* lin, int qlen, const void* input_dev, void* output_dev,
                           const float* bias_dev, const int* bsz_tensor_dev, void* stream);
+/* The prompt route: ktb200_linear_forward's contract at any qlen >= 1, on a tiled integer tensor-core GEMM that reads each
+ * weight once per chunk of at most 2048 tokens (DESIGN.md §4.17).  Q4_K weights, and Q6_K weights in the 8-row layout
+ * ktb200_linear_load_weights gives them when out_size % 8 == 0; any other handle returns KTB200_EINVAL.  Its activation
+ * scratch is a grow-only per-device arena: a call that would have to grow it while the stream is capturing returns
+ * KTB200_ESTATE before any device work, so run one eager call of the largest in_size before capture. */
+int ktb200_linear_forward_prompt(ktb200_linear* lin, int qlen, const void* input_dev, void* output_dev,
+                                 const float* bias_dev, const int* bsz_tensor_dev, void* stream);
+/* the qlen from which ktb200_linear_forward_prompt is the faster route for this handle (a function of its weight type,
+ * layout and shape, measured on an H100), 0 when it does not take the handle */
+int ktb200_linear_prompt_min(const ktb200_linear* lin);
 
 typedef struct ktb200_mlp ktb200_mlp;
 int ktb200_mlp_create(int hidden_size, int intermediate_size, const void* gate_dev, const void* up_dev,

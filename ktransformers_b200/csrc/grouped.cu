@@ -1333,4 +1333,32 @@ int moe_forward_grouped(ktb200_moe* m, int qlen, int k, const int64_t* ids, cons
     return KTB200_OK;
 }
 
+// The arena's Q8_K activation buffers (xq, xd, xbs) for the tiled linear GEMM (gguf_gemm.cu): at least `need` values (tokens x
+// in_features), grown to `grow` when they hold fewer.  Growing is synchronous and cannot be captured: on a capturing stream
+// it returns KTB200_ESTATE before any device work, and the caller names the warm-up.
+int grp_prompt_x(int dev, size_t need, size_t grow, cudaStream_t s, GrpX* out) {
+    GrpScratch& g = g_grp[dev & 63];
+    if (g.cap_x < need) {
+        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+        KTB_CUDA_CHECK(cudaStreamIsCapturing(s, &cs));
+        if (cs != cudaStreamCaptureStatusNone) return KTB200_ESTATE;
+        const size_t nx = grow > need ? grow : need;
+        KTB_CUDA_CHECK(cudaDeviceSynchronize());   // earlier calls may still be using the arena
+        cudaFree(g.xq); cudaFree(g.xd); cudaFree(g.xbs);
+        g.xq = nullptr; g.xd = nullptr; g.xbs = nullptr; g.cap_x = 0;
+        KTB_CUDA_CHECK(cudaMalloc(&g.xq, nx));
+        KTB_CUDA_CHECK(cudaMalloc(&g.xd, nx / 256 * sizeof(float)));
+        KTB_CUDA_CHECK(cudaMalloc(&g.xbs, nx / 16 * sizeof(int16_t)));
+        g.cap_x = nx;
+    }
+    *out = GrpX{g.xq, g.xd, g.xbs};
+    return KTB200_OK;
+}
+// T rows of x (hidden type, [T][K]) -> Q8_K in those buffers: the grouped path's quantiser, one launch
+int grp_prompt_quant(const void* x, int hidden_type, int T, int K, const GrpX& b, cudaStream_t s) {
+    grp_quant_x_kernel<<<(T * (K / QK_K) + 7) / 8, 256, 0, s>>>(x, hidden_type, T, K, b.q, b.d, b.bs);
+    KTB_LAUNCH_CHECK();
+    return KTB200_OK;
+}
+
 }  // namespace ktb

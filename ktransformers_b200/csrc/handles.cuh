@@ -62,6 +62,19 @@ static inline size_t blk_ready_words(const ktb200_moe_config& c) {
     const int t = c.group_max_len < kBlockMaxTokens ? c.group_max_len : kBlockMaxTokens;
     return (size_t)t * (c.routed_expert_num + 1) * (c.intermediate_size / QK_K);
 }
+
+// the Q8_K activation buffers of the grouped path's per-device arena (grouped.cu), lent to the tiled linear GEMM
+struct GrpX {
+    int8_t* q;     // [tokens][K]
+    float* d;      // [tokens][K / 256]
+    int16_t* bs;   // [tokens][K / 16]
+};
+int grp_prompt_x(int dev, size_t need, size_t grow, cudaStream_t s, GrpX* out);
+int grp_prompt_quant(const void* x, int hidden_type, int T, int K, const GrpX& b, cudaStream_t s);
+// the prompt route of the GGUF dense linear (gguf_gemm.cu): ktb200_linear_prompt_min, ktb200_linear_forward_prompt
+int gguf_prompt_min(int type, int layout, int K, int N);
+int gguf_forward_prompt(const void* w, int type, int layout, int K, int N, int hidden_type, int dev, int qlen, const void* x, void* y,
+                        const float* bias, const int* bsz, cudaStream_t s);
 }  // namespace ktb
 
 struct DeviceGuard {

@@ -871,6 +871,21 @@ int ktb200_linear_forward(ktb200_linear* l, int qlen, const void* input, void* o
     return launch_rows<false>(pick_fmt(l->proj_type, l->soa), rp, qlen, l->device, (cudaStream_t)stream);
 }
 
+int ktb200_linear_forward_prompt(ktb200_linear* l, int qlen, const void* input, void* output, const float* bias, const int* bsz,
+                                 void* stream) {
+    if (!l) { set_error("null handle"); return KTB200_EINVAL; }
+    if (!l->loaded) { set_error("Not Loaded"); return KTB200_ESTATE; }
+    if (qlen <= 0) return KTB200_OK;
+    if (!input || !output) { set_error("forward_prompt: null pointer"); return KTB200_EINVAL; }
+    DeviceGuard g(l->device);
+    return gguf_forward_prompt(l->proj, l->proj_type, l->soa ? LAYOUT_SOA8 : LAYOUT_RAW, l->in_size, l->out_size, l->hidden_type,
+                               l->device, qlen, input, output, bias, bsz, (cudaStream_t)stream);
+}
+
+int ktb200_linear_prompt_min(const ktb200_linear* l) {
+    return l ? gguf_prompt_min(l->proj_type, l->soa ? LAYOUT_SOA8 : LAYOUT_RAW, l->in_size, l->out_size) : 0;
+}
+
 // ------------------------------------------------------------------------------------------ mlp
 
 int ktb200_mlp_create(int H, int I, const void* gate, const void* up, const void* down, int gate_type, int up_type,

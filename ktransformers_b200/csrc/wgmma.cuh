@@ -151,6 +151,24 @@ __device__ __forceinline__ void mma_s8s8_m64n64(uint32_t (&d)[32], uint64_t desc
         : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
         : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
+// s32 (+)= u8 / s8 (A: registers; register 0 row lane / 4 and 1 row lane / 4 + 8 at K = 4 (lane % 4) + 0..3, 2 and 3 the same
+// rows at K = 16 + 4 (lane % 4) + 0..3) . s8 (B: shared memory, K-major), 64 x 64 x 32
+#define KTB_MMA_I8_RS_M64N64(NAME, ATYPE)                                                                                          \
+    __device__ __forceinline__ void NAME(uint32_t(&d)[32], const uint32_t(&a)[4], uint64_t desc_b, uint32_t accumulate) {          \
+        asm volatile(                                                                                                              \
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"                                                                          \
+            "wgmma.mma_async.sync.aligned.m64n64k32.s32." ATYPE ".s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, " \
+            "%14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, " \
+            "p;\n}\n"                                                                                                             \
+            : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]),          \
+              "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]),  \
+              "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]),              \
+              "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])                                         \
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));                                        \
+    }
+KTB_MMA_I8_RS_M64N64(mma_u8s8_rs_m64n64, "u8")
+KTB_MMA_I8_RS_M64N64(mma_s8s8_rs_m64n64, "s8")
+#undef KTB_MMA_I8_RS_M64N64
 // fp32 += bf16 (A: registers, accumulator-shaped fragment) . bf16 (B: shared memory, MN-major), 64 x 256 x 16
 __device__ __forceinline__ void mma_bf16_rs_m64n256_bt(float (&d)[128], const uint32_t (&a)[4], uint64_t desc_b, uint32_t accumulate) {
     asm volatile(

@@ -104,6 +104,8 @@ SYMBOLS = {
     "ktb200_linear_destroy": (None, [_VP]),
     "ktb200_linear_load_weights": (_I, [_VP, _VP]),
     "ktb200_linear_forward": (_I, [_VP, _I, _VP, _VP, _VP, _VP, _VP]),
+    "ktb200_linear_forward_prompt": (_I, [_VP, _I, _VP, _VP, _VP, _VP, _VP]),
+    "ktb200_linear_prompt_min": (_I, [_VP]),
     "ktb200_mlp_create": (_I, [_I, _I, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, C.POINTER(_VP)]),
     "ktb200_mlp_destroy": (None, [_VP]),
     "ktb200_mlp_load_weights": (_I, [_VP, _VP]),

@@ -104,7 +104,14 @@ class KLinearTorch(KLinearBase):
 
 
 class KLinearB200(KLinearBase):
-    """GGUF-native linear: y = x · Wᵀ with W kept as raw ggml blocks in HBM."""
+    """GGUF-native linear: y = x · Wᵀ with W kept as raw ggml blocks in HBM.
+
+    Calls of `prompt_min` tokens or more (ktb200_linear_prompt_min: a threshold per weight type and shape, 0 for types the
+    tiled GEMM does not take) run ktb200_linear_forward_prompt, which reads each weight once per chunk of up to 2048 tokens;
+    shorter calls run the decode GEMVs.  So with Q4_K / Q6_K weights, KTransformersLinear(generate_op="KLinearB200",
+    prefill_op=None) serves both phases from one resident copy.  The prompt route's activation scratch is a grow-only
+    per-device arena: before capturing a prompt-sized call in a CUDA graph, run one eager prompt-sized call (any length of
+    `prompt_min` tokens or more) of the largest in_features on the device."""
 
     def __init__(self, key, gguf_loader, config, orig_module=None, device: str = "cuda", max_tokens: int = 1024, **kwargs):
         super().__init__(key, gguf_loader, config, orig_module, device, **kwargs)
@@ -112,6 +119,7 @@ class KLinearB200(KLinearBase):
         self.weight = None       # raw block bytes on the device (modeling code may touch `.weight`)
         self.bias = None
         self.max_tokens = max_tokens
+        self.prompt_min = 0
 
     def load(self, w=None, device: str | None = None):
         if self.loaded:
@@ -143,6 +151,7 @@ class KLinearB200(KLinearBase):
                                               self.hidden_type, self.max_tokens, self.dev_index, C.byref(h)))
         self.handle = h
         native.check(lib.ktb200_linear_load_weights(self.handle, torch.cuda.current_stream(dev).cuda_stream))
+        self.prompt_min = lib.ktb200_linear_prompt_min(self.handle)
         self.loaded = True
 
     def forward(self, x: torch.Tensor, bsz_tensor: torch.Tensor = None, **kwargs) -> torch.Tensor:
@@ -151,7 +160,9 @@ class KLinearB200(KLinearBase):
         orig_shape, in_dtype = x.shape, x.dtype
         x2 = x.reshape(-1, x.shape[-1]).to(_GGML_TO_TORCH[self.hidden_type]).contiguous()
         out = torch.empty((x2.shape[0], self.out_features), dtype=x2.dtype, device=x2.device)
-        native.check(native.lib().ktb200_linear_forward(
+        prompt = self.prompt_min > 0 and x2.shape[0] >= self.prompt_min
+        lib = native.lib()
+        native.check((lib.ktb200_linear_forward_prompt if prompt else lib.ktb200_linear_forward)(
             self.handle, x2.shape[0], x2.data_ptr(), out.data_ptr(), self.bias.data_ptr() if self.has_bias else None,
             bsz_tensor.data_ptr() if bsz_tensor is not None else None, torch.cuda.current_stream(x2.device).cuda_stream))
         return out.reshape(*orig_shape[:-1], self.out_features).to(in_dtype)
