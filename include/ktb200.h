@@ -277,7 +277,12 @@ typedef struct ktb200_gate_config {
 } ktb200_gate_config;
 /* idx_dev int64 [qlen][top_k] (order: descending biased score, like torch.topk sorted=True — the
  * reference uses sorted=False whose order is unspecified; tests compare as sets), w_dev fp32.
- * logits_dev optional fp32 [qlen][n_experts] scratch/out (NULL -> internal). */
+ * logits_dev optional fp32 [qlen][n_experts] scratch/out (NULL -> internal).
+ * With bsz_tensor_dev, rows >= max(0, min(qlen, *bsz)) are not written (a negative value selects nothing, like 0).
+ * Scratch: one grow-only partial-sum buffer per device (qlen * n_experts * column splits * 4 bytes, at least 1 MB) and a
+ * ticket, allocated by the first call and grown by a call that needs more.  Growing cannot be captured: a call on a
+ * capturing stream that would allocate or grow returns KTB200_ESTATE before any device work, with a message naming the
+ * warm-up — one eager call with the same router and at least as many tokens on that device before capture. */
 int ktb200_moe_gate_forward(const ktb200_gate_config* cfg, int qlen, const void* x_dev, int64_t* idx_dev,
                             float* w_dev, float* logits_dev, const int* bsz_tensor_dev, void* stream);
 
@@ -578,6 +583,9 @@ void ktb200_debug_block_trace(unsigned long long* trace_dev);
  * barrier words [0..3], the timeout status word [4], then the per-Q8_K-block readiness words.  Every word is 0 between
  * launches.  Copies min(n, total) words to host_out (may be NULL) and returns the total, or -1 on error. */
 long ktb200_debug_block_sync_words(ktb200_moe* moe, unsigned* host_out, long n);
+/* The router's two ticket words on `device` (finished CTAs, finished selectors), copied to host_out[2] after a device
+ * synchronise.  Both are 0 between ktb200_moe_gate_forward launches.  KTB200_ESTATE before the first router call there. */
+int ktb200_debug_gate_ticket(int device, unsigned* host_out);
 
 #ifdef __cplusplus
 }

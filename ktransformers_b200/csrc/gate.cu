@@ -13,6 +13,7 @@
 //            per token — scoring, bias, group top-2 / max, group top-k, expert top-k by iterative arg-max with
 //            REDUX max/min (ties -> lowest index), gather, normalise, scale.
 #include "gate.cuh"
+#include "handles.cuh"
 
 namespace ktb {
 
@@ -21,7 +22,7 @@ __global__ void __launch_bounds__(kGateThreads) gate_kernel(const GateParams p) 
     float* xs = reinterpret_cast<float*>(smem_raw);   // [tok tile][slice cols]  (phase 1) / scores+choice (phase 2)
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int Teff = p.T;
-    if (p.bsz) Teff = min(p.T, *p.bsz);
+    if (p.bsz) Teff = max(0, min(p.T, *p.bsz));   // a negative device batch size selects nothing, like 0
     const int s = blockIdx.y, S = p.S;
     const int n4 = p.H / 4;
     const int c0 = (int)((long)n4 * s / S), c1 = (int)((long)n4 * (s + 1) / S);   // float4 column range of this split
@@ -95,11 +96,26 @@ extern "C" int ktb200_moe_gate_forward(const ktb200_gate_config* c, int qlen, co
     const int S = gate_splits(c->n_experts, c->hidden_size, num_sms(dev));
     const size_t need = (size_t)qlen * c->n_experts * S * sizeof(float);
     if (need > g_partial_cap[d] || !g_ticket[d]) {
-        // grow-only scratch; allocation is NOT capturable: call once with the largest qlen before graph capture
-        if (g_partial[d]) cudaFree(g_partial[d]);
-        const size_t cap = need < (1u << 20) ? (1u << 20) : need;
-        KTB_CUDA_CHECK(cudaMalloc(&g_partial[d], cap));
-        g_partial_cap[d] = cap;
+        // grow-only scratch.  Growing is synchronous and cannot be captured: on a capturing stream return before any device
+        // work and name the warm-up (one eager call at this qlen or more, with this router, on this device)
+        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+        KTB_CUDA_CHECK(cudaStreamIsCapturing(s, &cs));
+        if (cs != cudaStreamCaptureStatusNone) {
+            set_error("gate: this call needs %zu bytes of router scratch on device %d, which holds %zu%s; the scratch cannot grow while "
+                      "the stream is capturing: run one eager ktb200_moe_gate_forward call of %d or more tokens with n_experts %d and "
+                      "hidden_size %d on this device before capture", need, dev, g_partial_cap[d], g_ticket[d] ? "" : " (first call)", qlen,
+                      c->n_experts, c->hidden_size);
+            return KTB200_ESTATE;
+        }
+        if (need > g_partial_cap[d]) {
+            KTB_CUDA_CHECK(cudaDeviceSynchronize());   // earlier calls may still be using the scratch
+            cudaFree(g_partial[d]);
+            g_partial[d] = nullptr;
+            g_partial_cap[d] = 0;
+            const size_t cap = need < (1u << 20) ? (1u << 20) : need;
+            KTB_CUDA_CHECK(cudaMalloc(&g_partial[d], cap));
+            g_partial_cap[d] = cap;
+        }
         if (!g_ticket[d]) {
             KTB_CUDA_CHECK(cudaMalloc(&g_ticket[d], 2 * sizeof(unsigned)));
             KTB_CUDA_CHECK(cudaMemset(g_ticket[d], 0, 2 * sizeof(unsigned)));
@@ -116,5 +132,16 @@ extern "C" int ktb200_moe_gate_forward(const ktb200_gate_config* c, int qlen, co
     if (smem > 48 * 1024) KTB_CUDA_CHECK(cudaFuncSetAttribute(gate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     gate_kernel<<<dim3(row_ctas, S), kGateThreads, smem, s>>>(p);
     KTB_LAUNCH_CHECK();
+    return KTB200_OK;
+}
+
+extern "C" int ktb200_debug_gate_ticket(int device, unsigned* host_out) {
+    using namespace ktb;
+    if (!host_out) { set_error("debug_gate_ticket: null pointer"); return KTB200_EINVAL; }
+    const int d = device & 63;
+    if (!g_ticket[d]) { set_error("debug_gate_ticket: no router call has run on device %d", device); return KTB200_ESTATE; }
+    DeviceGuard guard(device);
+    KTB_CUDA_CHECK(cudaDeviceSynchronize());
+    KTB_CUDA_CHECK(cudaMemcpy(host_out, g_ticket[d], 2 * sizeof(unsigned), cudaMemcpyDeviceToHost));
     return KTB200_OK;
 }

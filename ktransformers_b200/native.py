@@ -127,6 +127,7 @@ SYMBOLS = {
     "ktb200_moe_ep_forward_tokens": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _VP]),
     "ktb200_debug_block_trace": (None, [_VP]),
     "ktb200_debug_block_sync_words": (_L, [_VP, _VP, _L]),
+    "ktb200_debug_gate_ticket": (_I, [_I, _VP]),
     "ktb200_debug_stream_read": (_I, [_VP, _L, _I, _I, _I, _I, _VP, C.POINTER(C.c_float)]),
     "ktb200_mla_workspace_bytes": (C.c_size_t, [_I, _I, _I]),
     "ktb200_mla_decode": (_I, [C.POINTER(MlaParams), _VP]),

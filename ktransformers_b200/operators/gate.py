@@ -66,7 +66,11 @@ class KMoEGate(BaseInjectedModule, KMoEGateBase):
 
 
 class KMoEGateB200(KMoEGate):
-    """Same interface, routing done by libktb200 on the GPU (no torch ops on the decode path)."""
+    """Same interface, routing done by libktb200 on the GPU (no torch ops on the decode path).
+
+    The router's partial-sum scratch is per device and grow-only, and it cannot grow inside a CUDA graph capture: before
+    capturing a forward, run one eager forward of at least as many tokens (bsz * q_len) on that device, or the captured
+    call raises KTB200Error (KTB200_ESTATE) naming that warm-up."""
 
     def load(self, w=None, device: str | None = None):
         native.lib()  # fail loudly without the CUDA library
