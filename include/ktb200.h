@@ -527,6 +527,35 @@ typedef struct ktb200_mla_prefill_params {
     void* out;
 } ktb200_mla_prefill_params;
 int ktb200_mla_prefill(const ktb200_mla_prefill_params* p, void* stream);
+/* ------------------------------------------------------------------------------------------
+ * Causal MLA prefill over decompressed heads for a batch of sequences of their own lengths (varlen): ktb200_mla_prefill's
+ * arithmetic, head dims, alignment and stride rules, with rows in place of the batch dimension.
+ *   seq int32 [batch][4] (HOST) = {q_row, q_len, k_row, kv_len}: sequence b's queries are rows q_row .. q_row + q_len - 1
+ *   of q_nope / q_pe, its keys rows k_row .. k_row + kv_len - 1 of k_nope / v / k_pe.  With P = kv_len - q_len, query i
+ *   sits at position P + i and attends to keys j <= P + i (bottom-right aligned); its output is row q_row + i of
+ *   out [q_rows][num_heads][128] bf16 (contiguous).  No other row of out is written; q_len = 0 writes nothing.
+ *   q_nope [q_rows][num_heads][128], q_pe [q_rows][num_heads][64], k_nope / v [k_rows][num_heads][128], k_pe [k_rows][64]
+ *   (strides in elements, token / head); rows outside the named ranges are never used, whatever they hold.
+ * Each sequence's output equals ktb200_mla_prefill on that sequence alone (batch 1) bit for bit.  The sequences travel in
+ * the kernel's parameter block: no allocation, no synchronisation, stream-ordered.
+ * KTB200_EINVAL (before any device work) for whatever ktb200_mla_prefill refuses, batch outside 1 ..
+ * KTB200_MLA_PREFILL_VARLEN_MAX_BATCH, a null seq, negative values, q_len > kv_len, q_len > 65535 * 128, a row range outside
+ * q_rows / k_rows, and two sequences whose output rows overlap.
+ * ------------------------------------------------------------------------------------------ */
+#define KTB200_MLA_PREFILL_VARLEN_MAX_BATCH 1024
+typedef struct ktb200_mla_prefill_varlen_params {
+    int batch, q_rows, k_rows, num_heads;
+    int qk_nope_head_dim, qk_rope_head_dim, v_head_dim;
+    float sm_scale;
+    const int* seq;
+    const void* q_nope; long q_nope_token_stride, q_nope_head_stride;
+    const void* q_pe; long q_pe_token_stride, q_pe_head_stride;
+    const void* k_nope; long k_nope_token_stride, k_nope_head_stride;
+    const void* v; long v_token_stride, v_head_stride;
+    const void* k_pe; long k_pe_token_stride;
+    void* out;
+} ktb200_mla_prefill_varlen_params;
+int ktb200_mla_prefill_varlen(const ktb200_mla_prefill_varlen_params* p, void* stream);
 /* Debug aid of the grouped (prefill) expert GEMM: when non-null, CTA 0 of the gate and down GEMMs writes clock64 stamps of its
  * first 96 stages, [kernel 2][role 3 = producer, MMA warpgroup, unused][stage 96][4] int64 (tools/grouped_probe.py prints them). */
 void ktb200_debug_grouped(long long* trace_dev);

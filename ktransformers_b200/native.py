@@ -78,6 +78,23 @@ class MlaPrefillParams(C.Structure):
                 ("out", C.c_void_p)]
 
 
+MLA_PREFILL_VARLEN_MAX_BATCH = 1024
+
+
+class MlaPrefillVarlenParams(C.Structure):
+    """struct ktb200_mla_prefill_varlen_params (include/ktb200.h); seq is a HOST int32 [batch][4] {q_row, q_len, k_row,
+    kv_len}; strides in elements, token / head."""
+    _fields_ = [("batch", C.c_int), ("q_rows", C.c_int), ("k_rows", C.c_int), ("num_heads", C.c_int),
+                ("qk_nope_head_dim", C.c_int), ("qk_rope_head_dim", C.c_int), ("v_head_dim", C.c_int), ("sm_scale", C.c_float),
+                ("seq", C.c_void_p),
+                ("q_nope", C.c_void_p), ("q_nope_token_stride", C.c_long), ("q_nope_head_stride", C.c_long),
+                ("q_pe", C.c_void_p), ("q_pe_token_stride", C.c_long), ("q_pe_head_stride", C.c_long),
+                ("k_nope", C.c_void_p), ("k_nope_token_stride", C.c_long), ("k_nope_head_stride", C.c_long),
+                ("v", C.c_void_p), ("v_token_stride", C.c_long), ("v_head_stride", C.c_long),
+                ("k_pe", C.c_void_p), ("k_pe_token_stride", C.c_long),
+                ("out", C.c_void_p)]
+
+
 _lib = None
 _lock = threading.Lock()
 
@@ -139,6 +156,7 @@ SYMBOLS = {
     "ktb200_mla_ragged_plan": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _VP, C.c_size_t, C.POINTER(_I), C.POINTER(C.c_size_t)]),
     "ktb200_mla_decode_ragged": (_I, [C.POINTER(MlaRaggedParams), _VP]),
     "ktb200_mla_prefill": (_I, [C.POINTER(MlaPrefillParams), _VP]),
+    "ktb200_mla_prefill_varlen": (_I, [C.POINTER(MlaPrefillVarlenParams), _VP]),
     "ktb200_debug_grouped": (None, [_VP]),
     "ktb200_mla_absorb_q": (_I, [_VP, _L, _L, _VP, _I, _I, _I, _VP, _I, _VP]),
     "ktb200_mla_absorb_o": (_I, [_VP, _VP, _I, _I, _I, _VP, _I, _VP]),

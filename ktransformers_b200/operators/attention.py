@@ -20,9 +20,15 @@ instead: the decode steps up to absorb_q, then causal latent-space attention str
 absorb_o and o_proj.  Like decode, it makes no host synchronisation and can be captured in a CUDA graph.
 
 forward_ragged is the flat-token entry of a serving step (balance_serve's flashinfer_attn.forward): tokens of several
-sequences at their own positions, decode tokens and prompt chunks mixed, through the same projections and RoPE, a per-token
-cache write (StaticCache.write_tokens), absorb_q, one ragged MLAWrapper call (ktb200_mla_decode_ragged), absorb_o and
-o_proj.  Its wrapper is one per device, shared by every layer, with its own row and item capacities."""
+sequences at their own positions, decode tokens and prompt chunks mixed, through the same projections and RoPE and a
+per-token cache write (StaticCache.write_tokens).  With absorb_for_prefill, or when no sequence of the step has more than one
+token, every row then takes the absorbed branch: absorb_q, one ragged MLAWrapper call (ktb200_mla_decode_ragged), absorb_o.
+Otherwise the step splits by forward's rule (SGLang's DeepSeek path makes the same split): the prompt sequences (q_len > 1)
+gather their cached latents through the layer's page table into one packed buffer, one dense kv_b_proj decompresses it and
+one ktb200_mla_prefill_varlen call (csrc/mla_prefill.cu) attends with the queries in place in the q_b output; the decode
+sequences (q_len == 1) take the absorbed branch on their rows only, and their output is scattered into the same rows.
+One o_proj follows either way.  The ragged wrapper is one per device, shared by every layer, with its own row and item
+capacities."""
 from __future__ import annotations
 
 import ctypes as C
@@ -36,6 +42,15 @@ from .base_operator import BaseInjectedModule
 from .flashinfer_wrapper import MLAWrapper, MLAWrapperSingleton
 
 _RAGGED_WRAPPERS: dict = {}   # device -> the MLAWrapper of forward_ragged (one plan and one split workspace for all layers)
+
+
+def _ragged_wrapper(cache, dev, batch: int, max_rows: int, max_items: int) -> MLAWrapper:
+    key = str(dev)
+    if key not in _RAGGED_WRAPPERS:
+        _RAGGED_WRAPPERS[key] = MLAWrapper(cache.max_batch_size, cache.max_pages, device=key, max_rows=max_rows, max_items=max_items)
+    w = _RAGGED_WRAPPERS[key]
+    assert batch <= w.max_batch_size and cache.max_pages <= w.max_pages, "the shared ragged wrapper was made for a smaller cache"
+    return w
 
 
 class KDeepseekV2Attention(BaseInjectedModule, DeepseekV3Attention):
@@ -125,7 +140,12 @@ class KDeepseekV2Attention(BaseInjectedModule, DeepseekV3Attention):
         each sequence's length after this step; cache_rows [B] (host) the StaticCache batch row (page range) sequence b
         owns.  A sequence's tokens are its last q_len_b positions, kv_len[b] - q_len_b .. kv_len[b] - 1.  max_rows /
         max_items size the shared wrapper when this call creates it.  Returns [T, hidden].  The host data reaches the device
-        through pinned, non-blocking copies, so the step makes no host synchronisation."""
+        through pinned, non-blocking copies, so the step makes no host synchronisation.
+
+        Without absorb_for_prefill, a step in which some sequence has q_len_b > 1 runs those sequences on the decompressed
+        path (kv_b_proj over their kv_len[b] cached latents, ktb200_mla_prefill_varlen; bf16 only, as forward's prefill) and
+        the q_len_b == 1 sequences on the absorbed one; otherwise every row is absorbed.  The decompressed keys and values
+        take 64 KB per cached token of the prompt sequences, as in forward."""
         T = hidden_states.shape[0]
         cache = past_key_value
         qo = torch.as_tensor(qo_indptr, dtype=torch.int32)
@@ -149,6 +169,10 @@ class KDeepseekV2Attention(BaseInjectedModule, DeepseekV3Attention):
         cos, sin = self.rotary_emb(q_pe, pos)
         q_pe, k_pe = apply_rotary_pos_emb(q_pe, k_pe, cos, sin, unsqueeze_dim=2)
         kv_with_k_pe = cache.write_tokens(compressed_kv, k_pe, self.layer_idx, token_rows, position_ids)
+        if not self.absorb_for_prefill and bool(((qo[1:] - qo[:-1]) > 1).any()):
+            attn = self._ragged_split(q, q_pe.reshape(T, self.num_heads, self.qk_rope_head_dim).contiguous(), kv_with_k_pe, qo,
+                                      torch.as_tensor(kv_len, dtype=torch.int32), rows, cache, max_rows, max_items)
+            return self.o_proj(attn.reshape(1, T, self.num_heads * self.v_head_dim)).view(T, -1)
         ckv_pages = kv_with_k_pe[:, :, :, : self.kv_lora_rank].view(-1, cache.page_size, self.kv_lora_rank)
         kpe_pages = kv_with_k_pe[:, :, :, self.kv_lora_rank:].view(-1, cache.page_size, self.qk_rope_head_dim)
 
@@ -164,11 +188,7 @@ class KDeepseekV2Attention(BaseInjectedModule, DeepseekV3Attention):
             q_nope = torch.matmul(q_nope.transpose(1, 2), q_absorb).transpose(1, 2).contiguous().reshape(T, self.num_heads, self.kv_lora_rank)
         q_pe = q_pe.reshape(T, self.num_heads, self.qk_rope_head_dim).contiguous()
 
-        key = str(dev)
-        if key not in _RAGGED_WRAPPERS:
-            _RAGGED_WRAPPERS[key] = MLAWrapper(cache.max_batch_size, cache.max_pages, device=key, max_rows=max_rows, max_items=max_items)
-        w = _RAGGED_WRAPPERS[key]
-        assert B <= w.max_batch_size and cache.max_pages <= w.max_pages, "the shared ragged wrapper was made for a smaller cache"
+        w = _ragged_wrapper(cache, dev, B, max_rows, max_items)
         # sequence b's page table is its cache row's: kv_indices = the static table's rows, cache.max_pages pages each
         kv_indptr = torch.arange(0, B + 1, dtype=torch.int32, device=dev) * cache.max_pages
         kv_indices = cache.page_table_list[self.layer_idx].index_select(0, seq_rows.long()).reshape(-1)
@@ -183,6 +203,56 @@ class KDeepseekV2Attention(BaseInjectedModule, DeepseekV3Attention):
         else:
             attn = torch.matmul(attn.view(T, self.num_heads, 1, -1), out_absorb.mT.unsqueeze(0)).view(T, self.num_heads, self.v_head_dim)
         return self.o_proj(attn.reshape(1, T, self.num_heads * self.v_head_dim)).view(T, -1)
+
+    def _ragged_split(self, q: torch.Tensor, q_pe: torch.Tensor, kv_with_k_pe: torch.Tensor, qo: torch.Tensor, kv_len: torch.Tensor,
+                      rows: torch.Tensor, cache, max_rows: int, max_items: int) -> torch.Tensor:
+        """The attention core of a ragged step with prompt sequences, before o_proj: [T, heads, 128].  q [1, T, heads, 192] is
+        the q_b output, q_pe [T, heads, 64] the roped part, kv_with_k_pe the layer's latent buffer after write_tokens; qo,
+        kv_len and rows are host int32 tensors."""
+        T, H, dev = q.shape[1], self.num_heads, q.device
+        if q.dtype != torch.bfloat16 or q_pe.dtype != torch.bfloat16 or self.kv_b_proj.weight.dtype != torch.bfloat16:
+            raise NotImplementedError(f"KDeepseekV2Attention prefill is bf16 only (q {q.dtype}, kv_b_proj {self.kv_b_proj.weight.dtype})")
+        q_lens = qo[1:] - qo[:-1]
+        pre, dec = torch.nonzero(q_lens > 1).flatten(), torch.nonzero(q_lens == 1).flatten()
+        S, n, nd, page = kv_len[pre], int(kv_len[pre].sum()), dec.numel(), cache.page_size
+        # token j of prompt sequence b is row page_table[rows[b], j // page] * page + j % page of the layer's buffer: the
+        # page-table entry's index, the offset, then the decode rows and their cache rows, in one pinned copy
+        j = torch.arange(n, dtype=torch.int32) - torch.repeat_interleave(torch.cumsum(S, 0, dtype=torch.int32) - S, S)
+        host = torch.cat([torch.repeat_interleave(rows[pre], S) * cache.max_pages + j // page, j % page, qo[dec], rows[dec]]).pin_memory()
+        idx = host.to(dev, non_blocking=True)
+        table = cache.page_table_list[self.layer_idx]
+        flat = table.reshape(-1).index_select(0, idx[:n]) * page + idx[n:2 * n]
+        lat = kv_with_k_pe.view(-1, kv_with_k_pe.shape[-1]).index_select(0, flat)                 # [sum S, 576]
+        kv = self.kv_b_proj(lat[:, : self.kv_lora_rank]).view(n, H, self.qk_nope_head_dim + self.v_head_dim)
+        k_nope, v, k_pe = kv[..., : self.qk_nope_head_dim], kv[..., self.qk_nope_head_dim:], lat[:, self.kv_lora_rank:]
+        q_nope = q.view(T, H, self.q_head_dim)[..., : self.qk_nope_head_dim]
+        seq = torch.stack([qo[pre], q_lens[pre], torch.cumsum(S, 0, dtype=torch.int32) - S, S], 1).to(torch.int32).contiguous()
+        out = torch.empty((T, H, self.v_head_dim), dtype=q.dtype, device=dev)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        p = native.MlaPrefillVarlenParams(pre.numel(), T, n, H, self.qk_nope_head_dim, self.qk_rope_head_dim, self.v_head_dim, self.softmax_scale,
+                                          seq.data_ptr(), q_nope.data_ptr(), q_nope.stride(0), q_nope.stride(1), q_pe.data_ptr(), q_pe.stride(0),
+                                          q_pe.stride(1), k_nope.data_ptr(), k_nope.stride(0), k_nope.stride(1), v.data_ptr(), v.stride(0),
+                                          v.stride(1), k_pe.data_ptr(), k_pe.stride(0), out.data_ptr())
+        native.check(native.lib().ktb200_mla_prefill_varlen(C.byref(p), stream))
+        if nd:   # the decode rows: absorb_q, one MLAWrapper call over those sequences only, absorb_o, scattered into their rows
+            d_rows, d_cache = idx[2 * n:2 * n + nd].long(), idx[2 * n + nd:]
+            q_absorb, out_absorb = self.get_absorbed()
+            q_dec = q.view(T, -1).index_select(0, d_rows)
+            q_abs = torch.empty((nd, H, self.kv_lora_rank), dtype=q.dtype, device=dev)
+            native.check(native.lib().ktb200_mla_absorb_q(q_dec.data_ptr(), self.q_head_dim, H * self.q_head_dim,
+                                                          q_absorb.data_ptr(), H, self.qk_nope_head_dim, self.kv_lora_rank, q_abs.data_ptr(), nd, stream))
+            w = _ragged_wrapper(cache, dev, nd, max_rows, max_items)
+            kv_indptr = torch.arange(0, nd + 1, dtype=torch.int32, device=dev) * cache.max_pages
+            w.plan(torch.arange(nd + 1, dtype=torch.int32), kv_indptr, table.index_select(0, d_cache).reshape(-1), kv_len[dec], None, H,
+                   self.kv_lora_rank, self.qk_rope_head_dim, page, self.softmax_scale, q_abs.dtype, kv_with_k_pe.dtype)
+            ckv_pages = kv_with_k_pe[:, :, :, : self.kv_lora_rank].view(-1, page, self.kv_lora_rank)
+            kpe_pages = kv_with_k_pe[:, :, :, self.kv_lora_rank:].view(-1, page, self.qk_rope_head_dim)
+            attn = w.run(q_abs, q_pe.index_select(0, d_rows), ckv_pages, kpe_pages)
+            o = torch.empty((nd, H, self.v_head_dim), dtype=attn.dtype, device=dev)
+            native.check(native.lib().ktb200_mla_absorb_o(attn.data_ptr(), out_absorb.data_ptr(), H, self.v_head_dim, self.kv_lora_rank, o.data_ptr(),
+                                                          nd, stream))
+            out.index_copy_(0, d_rows, o)
+        return out
 
     def forward_prefill(self, q: torch.Tensor, q_pe: torch.Tensor, cache: torch.Tensor, max_pages: int, kv_seq_len: int) -> torch.Tensor:
         """Causal attention of a prompt chunk over the first kv_seq_len cached tokens of each sequence (attention.py:349-478,
